@@ -5,7 +5,7 @@ One "step" = one pass of the hot path over one batch of synthetic input: forward
 InterpolatingAdjoint gradient of the L2 trajectory-matching loss, summed over the ensemble (+ the sum over ranks of
 [grad_theta; loss] when N_gpus > 1, fused into the final reduction kernel over NVLink peer memory).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config lv|seir|fkpp|hjb]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config lv|seir|fkpp|hjb] [--dump-outputs DIR]
 
 --config lv (default, BASELINE config 2): 2->32->32->2 tanh chain, Glorot theta (seed 1), u0 ~ U(0.2,1) x U(2,5), 30 fixed
   Tsit5 steps of 0.1, states saved at every step, fp32.  The headline `value` is WEAK scaling (65 536 trajectories per GPU);
@@ -15,6 +15,8 @@ InterpolatingAdjoint gradient of the L2 trajectory-matching loss, summed over th
 --config hjb (config 5): highdim_pde/lambaem.jl's NNPDENS solve (d = 100, hls = 110, 20 Euler-Maruyama steps), 10 000 paths per GPU
   and iteration, fp64; a step = one iteration (forward paths + reverse sweep + ADAM); metric = paths/s.
 Under torchrun one rank per GPU.  Rank 0 prints ONE JSON line.
+--dump-outputs DIR: the last timed step's outputs as DIR/<name>.npy (64 MB at most, see dump_outputs); inputs are seeded, so two
+  builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -39,9 +41,42 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 N_PER_GPU = 65536
 UNIT = "trajectories/s"
-FP32_PEAK_TFLOPS = 72.5     # measured FFMA/FFMA2 issue peak on this pool's B200 (profiles/r01_pipes_microbench.txt)
-MUFU_PER_CLK_SM = 16.0      # measured (profiles/r01_pipes_microbench.txt): 0.499 warp instructions / clk / SM
-HMMA_PER_CLK_SM = 0.468     # measured mma.sync m16n8k8.tf32 / m16n8k16.f16 warp instructions / clk / SM (profiles/r01_mma_sync_microbench.txt)
+# NVIDIA H100 SXM data sheet (card allowed up to 700 W): the denominators of the roofline fractions, never reached figures
+FP32_PEAK_TFLOPS = 67.0     # FP32 (CUDA cores)
+FP64_TC_PEAK_TFLOPS = 67.0  # FP64 tensor core
+HBM_PEAK_GBS = 3350.0       # HBM3
+DUMP_LIMIT = 64 * 10**6     # bytes --dump-outputs writes in all (64 MB), .npy headers and the sample index included
+NPY_HEADER_MAX = 4096       # bound of one .npy header
+
+
+def gpu_info(index):
+    """Name, power limit and max SM clock of the GPU the numbers were measured on (nvidia-smi, read-only query)."""
+    try:
+        o = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=10).stdout.strip()
+        name, pl, mx = [x.strip() for x in o.split(",")]
+        return {"name": name, "power_limit_w": float(pl), "sm_max_mhz": float(mx)}
+    except Exception as ex:  # noqa: BLE001
+        return {"name": None, "note": f"nvidia-smi unavailable: {ex}"}
+
+
+def dump_outputs(d, arrays):
+    """Write {name: array} as d/<name>.npy, DUMP_LIMIT bytes in all; an "out" too large is a fixed seeded sample of its last
+    (trajectory) axis, indices in out_trajectory_index.npy."""
+    os.makedirs(d, exist_ok=True)
+    rest = {k: a for k, a in arrays.items() if k != "out"}
+    budget = DUMP_LIMIT - sum(a.nbytes for a in rest.values()) - NPY_HEADER_MAX * (len(arrays) + 1)
+    out = arrays.get("out")
+    if out is not None and out.nbytes > budget:
+        per_traj = out.nbytes // out.shape[-1] + 8                # one trajectory's states + its float64 index
+        keep = budget // per_traj
+        if keep < 1:
+            raise ValueError(f"--dump-outputs: no room for even one trajectory of 'out' within {DUMP_LIMIT} bytes")
+        idx = np.sort(np.random.default_rng(0).choice(out.shape[-1], keep, replace=False))
+        np.save(os.path.join(d, "out_trajectory_index.npy"), idx.astype(np.float64))
+        arrays = dict(arrays, out=np.ascontiguousarray(out[..., idx]))
+    for k, a in arrays.items():
+        np.save(os.path.join(d, f"{k}.npy"), a)
 
 
 def host_cores():
@@ -184,7 +219,7 @@ HOST = None
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.rows, self.stop = [], threading.Event()
@@ -241,7 +276,7 @@ def reference_arm(a, cfg):
     for _ in range(max(1, min(a.warmup, 2))):
         k = min(n, 1024)
         cpu_pass(cfg, theta, np.ascontiguousarray(u0[:, :k]), np.ascontiguousarray(y[:, :, :k]), cores)
-    times = [cpu_pass(cfg, theta, u0, y, cores) for _ in range(max(3, a.steps))]
+    times = [cpu_pass(cfg, theta, u0, y, cores) for _ in range(a.steps)]
     med = float(np.median(times))
     value = n / med
     same = (cfg is LV and n == N_PER_GPU)
@@ -300,7 +335,7 @@ def main_hjb(a):
         ms = min(m, 2000)
         bo.loss_and_grad(theta, d, hls, np.zeros(d), 1.0, n_steps, 200, 1)
         times = []
-        for i in range(max(3, min(a.steps, 5))):
+        for i in range(a.steps):
             t0 = time.perf_counter(); bo.loss_and_grad(theta, d, hls, np.zeros(d), 1.0, n_steps, ms, 1 + i); times.append(time.perf_counter() - t0)
         v = ms / float(np.median(times))
         print(json.dumps({"impl": "reference", "metric": metric, "value": v, "unit": unit, "n_gpus": a.gpus, "steps": len(times), "warmup": 1,
@@ -337,10 +372,11 @@ def main_hjb(a):
         dist.all_reduce(g_all)
         s.adam_step(opt, g_all[:s.P])
 
+    hist = None
     if world == 1:
         s.train_adam(opt, m, max(a.warmup, 3), seed0=1)
         torch.cuda.synchronize()
-        s.train_adam(opt, m, a.steps, seed0=100)
+        hist = s.train_adam(opt, m, a.steps, seed0=100)
         total_ms = s.last_train_ms()
         timing = "CUDA events on the handle's stream around the K iterations (1 direct launch + K-1 replays of one CUDA graph)"
     else:
@@ -357,6 +393,12 @@ def main_hjb(a):
         total_ms = float(t)
         timing = "host clock around K synchronous iterations (each ends in a stream synchronize), max over ranks"
     value = world * m * a.steps / (total_ms * 1e-3)
+    if a.dump_outputs and rank == 0:   # the parameters after the last timed iteration (+ the loss history of the timed iterations)
+        arrays = {"theta": np.ascontiguousarray(s.get_params(), np.float64)}
+        if hist is not None:
+            arrays["loss_history"] = hist[0].cpu().numpy().astype(np.float64)
+            arrays["u0_history"] = hist[1].cpu().numpy().astype(np.float64)
+        dump_outputs(a.dump_outputs, arrays)
 
     # end to end through the host-buffer call a script makes per optimiser iteration: theta in from host, loss + gradient back to host
     th_h = np.ascontiguousarray(s.get_params())
@@ -414,7 +456,7 @@ def main_hjb(a):
     mac_f = (d + 2) * hls + 2 * (hls + 1) * hls + (hls + 1) * d          # [W | b] times the ones-augmented activations
     fwd_flops = 2.0 * n_steps * mac_f * m
     ach = fwd_flops / (fwd_ms * 1e-3) / 1e12
-    dmma_peak = 36.5   # TFLOP/s, mma.sync.m8n8k4.f64 issue-rate microbenchmark on this GPU model (profiles/r02_dmma_microbench.txt)
+    dmma_peak = FP64_TC_PEAK_TFLOPS
     cpu = None
     if world == 1 and not a.no_cpu_baseline:
         from oracle import bsde_oracle as bo
@@ -436,10 +478,10 @@ def main_hjb(a):
         "gpu_launches": (sum(1 for k in names if "::k_" in k) if names else 0) * a.steps,
         "library_launches": (sum(1 for k in names if "::k_" not in k) if names else 0) * a.steps,
         "kernels_per_step": sorted(set(names)) if names else None, "kernels_source": names_src,
-        "clocks": clk.summary(),
+        "clocks": clk.summary(), "gpu": gpu_info(local),
         "roofline": {"kernel": "k_fused_forward2 (fused DMMA forward sweep: 4 layers x 20 steps + Euler-Maruyama, two warps per 8-path tile, csrc/bsde.cu)", "bound": "tensor",
                      "achieved": ach, "peak": dmma_peak, "unit": "TFLOP/s", "frac": ach / dmma_peak, "traffic": None,
-                     "peak_source": "fp64 tensor pipe: DMMA.8x8x4 issue-rate microbenchmark (tools/microbench/dmma.cu, profiles/r02_dmma_microbench.txt); "
+                     "peak_source": "H100 SXM data sheet, FP64 tensor core (700 W card); "
                                     f"torch.matmul fp64 4096^3 in this run: {peak:.1f} TFLOP/s",
                      "algorithmic_flop_per_path_step": 2.0 * mac_f, "kernel_ms": fwd_ms,
                      "note": "share of the iteration: forward sweep / cotangent sweep / fused weight-gradient products in kernel_ms"},
@@ -462,6 +504,7 @@ def main():
     ap.add_argument("--cpu-sample", type=int, default=0, help="trajectories in the in-line CPU baseline sample (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-strong", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     a = ap.parse_args()
     global HOST
     if a.config == "hjb":
@@ -491,7 +534,7 @@ def main():
     n_save = cfg.n_steps // cfg.every + 1
     solver = cfg.make_solver(ude, n, dev)
     assert solver.P == P, (solver.P, P)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     # multi-GPU: the sum over ranks of [grad_theta; loss] runs inside the final reduction kernel over NVLink peer memory
     # (b200ude_adjoint_l2_allreduce); NCCL all-reduce only if the peer mapping cannot be set up on every rank
     peer = None
@@ -571,6 +614,10 @@ def main():
     weak = Shard(n, seed=rank)                       # every rank owns a different shard of the (world * n) ensemble
     tw = timed(weak)
     value = world * n * a.steps / (tw["total_ms"] * 1e-3)
+    if a.dump_outputs and rank == 0:   # what the last timed step returned to its caller: saved states, grad_theta, loss
+        torch.cuda.synchronize()
+        dump_outputs(a.dump_outputs, {"out": weak.out_d.cpu().numpy(), "grad_theta": weak.buf[:P].cpu().numpy(),
+                                      "loss": weak.buf[P:].cpu().numpy()})
 
     # ---- the metric's literal batch: 65 536 trajectories in total, sharded over the ranks (strong scaling) ----
     strong = None
@@ -663,60 +710,20 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
     adj_ms, fwd_ms = tw["adj_ms"], tw["fwd_ms"]
     adj_name = next((k for k in (names or []) if "adjoint" in k), "adjoint kernel")
     fwd_name = next((k for k in (names or []) if "forward" in k), "forward kernel")
-    traffic, traffic_src = None, "no ncu capture of this kernel committed for this round"
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel from this round's ncu --set full capture
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")))
-        ent = tj.get(cfg.name, {})
-        if ent and ent.get("trajectories"):
-            traffic = float(ent["dram_bytes"]) * (n / float(ent["trajectories"]))
-            traffic_src = ent.get("source", "profiles/r02_ncu_traffic.json")
-    except Exception:
-        pass
+    traffic, traffic_src = None, "not measured"
     roofline = {
         "kernel": f"{adj_name} (+ the ~5 us fixed-order reduce; events bracket both)",
         "bound": "hbm", "achieved": n * cfg.bytes_adj / (adj_ms * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s",
         "frac": n * cfg.bytes_adj / (adj_ms * 1e-3) / 1e9 / hbm_peak,
-        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6.65 TB/s (B200_PROFILING.md)",
+        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3.35 TB/s HBM3",
         "algorithmic_bytes_per_trajectory": cfg.bytes_adj, "traffic": traffic, "traffic_source": traffic_src,
         "note": "the path is compute-bound by construction (SURVEY.md 8d, ~430 FLOP/B for config 2): roofline_pipes grades the kernels against the pipes they actually use",
     }
-    sm_clock = (clocks or {}).get("sm_mhz") or 1965.0
     line_extra = {}
-    if cfg is LV:
-        wm = any("wm::" in k for k in (names or []))
-        # per-trajectory pipe work of the kernels that ran (DESIGN.md section 4.6): MUFU lane-ops, legacy tensor-pipe (HMMA) warp
-        # instructions, FMA-pipe cycles and issue slots (static SASS counts of the stage loop bodies, cuobjdump), HBM bytes
-        ev_f, ev_a = 1 + 6 * cfg.n_steps, 6 * cfg.n_steps
-        mufu = 80.0 if wm else 128.0                       # per chain evaluation: 64 tanh x 1.25 (batched inversion) / x 2
-        fam = {   # per trajectory and stage evaluation: (forward, adjoint)
-            "hmma": (24.0 / 16.0, 96.0 / 16.0) if wm else (0.0, 96.0 / 32.0),          # warp-level mma.sync instructions
-            "fma_cyc": (279.0 / 16.0, 500.0 / 16.0) if wm else (600.0 / 32.0, 1700.0 / 32.0),   # FMA-pipe cycles (FFMA2 = 2), per scheduler
-            "issue": (500.0 / 16.0, 950.0 / 16.0) if wm else (887.0 / 32.0, 2268.0 / 32.0),     # warp instructions issued
-        }
-        clk_hz = sm_clock * 1e6
-
-        def pipes(ms, evals, which, nbytes):
-            t = ms * 1e-3
-            b = {"mufu": n * evals * mufu / (148 * MUFU_PER_CLK_SM * clk_hz),
-                 "tensor_mma_sync": n * evals * fam["hmma"][which] / (148 * HMMA_PER_CLK_SM * clk_hz),
-                 "fma_pipe": n * evals * fam["fma_cyc"][which] / (148 * 4 * clk_hz),
-                 "issue_slots": n * evals * fam["issue"][which] / (148 * 4 * clk_hz),
-                 "hbm": n * nbytes / (hbm_peak * 1e9)}
-            tmin = max(b.values())
-            return {"ms": ms, "t_min_ms": 1e3 * tmin, "binding_pipe": max(b, key=b.get), "frac": tmin / t,
-                    "pipe_ms": {k: 1e3 * v for k, v in b.items()}}
-        line_extra["roofline_pipes"] = {
-            "forward": pipes(fwd_ms, ev_f, 0, cfg.bytes_fwd), "adjoint": pipes(adj_ms, ev_a, 1, cfg.bytes_adj),
-            "kernel_family": "warp-collective mma.sync (lv32_wm.cuh)" if wm else "tcgen05 (lv32_tc.cuh)",
-            "peaks": {"mufu_lanes_per_clk_sm": MUFU_PER_CLK_SM, "mma_sync_warp_instr_per_clk_sm": HMMA_PER_CLK_SM, "issue_slots_per_clk_sm": 4, "fma_pipe_cycles_per_clk_sm": 4,
-                      "hbm_gbs": hbm_peak, "sm_mhz": sm_clock},
-            "peak_source": "tools/microbench (profiles/r01_pipes_microbench.txt, r01_mma_sync_microbench.txt), MEASURED_PEAKS.json",
-            "note": "t_min = max over pipes of (work / measured pipe peak); frac = t_min / measured time; the tcgen05 pipe of the tensor-core family is far from binding and not listed",
-        }
     line_extra["roofline_fp32"] = {
         "step_achieved_tflops": n * (cfg.flop_fwd + cfg.flop_adj) / (tw["step_ms"] * 1e-3) / 1e12, "peak": FP32_PEAK_TFLOPS,
         "note": "algorithmic FLOP rate for context only: most of these FLOPs run on tensor cores, so this is not a roofline fraction",
@@ -750,7 +757,7 @@ def main():
         "gpu_launches": (len(names) if names else 3) * a.steps,
         "kernels_per_step": names, "kernels_source": names_src,
         "allreduce_check": allreduce_check,
-        "clocks": clocks, "roofline": roofline, "cpu_baseline": cpu,
+        "clocks": clocks, "gpu": gpu_info(local), "roofline": roofline, "cpu_baseline": cpu,
         "kernel_ms": {"forward": fwd_ms, "adjoint_plus_reduce": adj_ms, "step": tw["step_ms"]},
     }
     line.update(line_extra)

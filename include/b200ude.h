@@ -1,5 +1,5 @@
 /*
- * b200ude.h -- C ABI of the B200-native UDE training path.
+ * b200ude.h -- C ABI of the H100-native (sm_90a) UDE training path.
  *
  * This is the drop-in boundary for ONE hot path of
  * ChrisRackauckas/universal_differential_equations: the forward solve of a
@@ -105,10 +105,10 @@ extern "C" {
 /* error codes */
 #define B200UDE_OK 0
 #define B200UDE_EINVAL (-1)       /* bad descriptor / argument */
-#define B200UDE_EUNSUPPORTED (-2) /* configuration has no sm_100a kernel in this build */
+#define B200UDE_EUNSUPPORTED (-2) /* configuration has no sm_90a kernel in this build */
 #define B200UDE_ESTATE (-3)       /* call order violated (e.g. adjoint before forward) */
 #define B200UDE_ENOMEM (-4)
-#define B200UDE_ENODEVICE (-5)    /* no CUDA device / not an sm_100 part */
+#define B200UDE_ENODEVICE (-5)    /* no CUDA device / not an sm_90 part */
 
 #define B200UDE_MAX_LAYERS 6
 

@@ -5,7 +5,7 @@
 # surface the scripts use --
 #     concrete_solve(prob, Tsit5() / Vern7(), u0, p; saveat, abstol, reltol, sensealg = InterpolatingAdjoint(autojacvec = ReverseDiffVJP()))
 #     DiffEqFlux.sciml_train(loss, theta, ADAM(eta); cb, maxiters)           (seir_exposure.jl:137-141,160-161; Fisher-KPP-CNN.jl:136,236-238)
-# -- reaches the sm_100a kernels with ONE changed line per script: the line that builds the ODEProblem wraps the script's
+# -- reaches the sm_90a kernels with ONE changed line per script: the line that builds the ODEProblem wraps the script's
 # right-hand side in a `B200UDEFunction`, which names the UDE form (what a C ABI cannot learn from a closure):
 #     prob_nn = ODEProblem(B200UDE.SEIRExposure(dudt_, ann, p_), u0, tspan, p)            # was ODEProblem(dudt_, u0, tspan, p)  seir_exposure.jl:131
 #     prob_nn = ODEProblem(B200UDE.FisherKPP(nn_ode, rx_nn, Nx), rho0, (0.0, T), p)        # Fisher-KPP-CNN.jl:131

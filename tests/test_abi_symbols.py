@@ -1,5 +1,5 @@
 """The C-ABI library loads here (no GPU) and exports exactly what include/b200ude.h declares;
-create() fails loudly -- never silently falls back -- when no sm_100 device is present."""
+create() fails loudly -- never silently falls back -- when no sm_90 device is present."""
 import ctypes as C
 import os
 import re

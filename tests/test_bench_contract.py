@@ -1,19 +1,16 @@
-"""The JSON line bench.py prints, checked key by key against the driver's contract: on the lines committed under profiles/ (GPU runs of
-this round) and on a live run of the CPU reference arm."""
+"""The JSON line bench.py prints, checked key by key: on live GPU runs of every configuration and on a live run of the CPU
+reference arm."""
 import json
 import os
 import subprocess
 import sys
 
+import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BASE = {"metric": str, "value": (int, float), "unit": str, "n_gpus": int, "steps": int, "warmup": int, "ms_per_step": (int, float),
         "higher_is_better": bool, "scaling": str, "dtype": str, "data": str, "config": dict}
-
-
-def _line(path):
-    return json.loads([l for l in open(path) if l.startswith("{")][-1])
 
 
 def _check_common(j):
@@ -25,10 +22,20 @@ def _check_common(j):
     assert set(e) >= {"value", "unit", "h2d_bytes_per_step", "d2h_bytes_per_step"} and e["unit"] == j["unit"]
 
 
-@pytest.mark.parametrize("name", ["r02_bench_1gpu_lv.json", "r02_bench_8gpu_lv.json", "r02_bench_hjb.json", "r02_bench_1gpu_seir.json"])
-def test_committed_gpu_lines(name):
-    j = _line(os.path.join(ROOT, "profiles", name))
+GPU_RUNS = {"lv": ["--n-per-gpu", "16384", "--no-strong"], "seir": ["--n-per-gpu", "4096"], "fkpp": ["--n-per-gpu", "1024"], "hjb": ["--n-per-gpu", "2000"]}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("config", sorted(GPU_RUNS))
+def test_gpu_bench_line(config, tmp_path):
+    """One GPU run of bench.py per configuration: the JSON line, and the arrays --dump-outputs writes after the timed steps."""
+    dump = tmp_path / "out"
+    out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--config", config, "--steps", "4", "--warmup", "2",
+                          "--cpu-sample", "64", "--dump-outputs", str(dump)] + GPU_RUNS[config], capture_output=True, text=True, timeout=900)
+    assert out.returncode == 0, out.stderr[-2000:]
+    j = json.loads([l for l in out.stdout.splitlines() if l.startswith("{")][-1])
     _check_common(j)
+    assert j["steps"] == 4 and j["n_gpus"] == 1
     assert j["value"] > 0 and j["gpu_launches"] > 0 and j["e2e"]["value"] > 0
     assert j["e2e"]["h2d_bytes_per_step"] > 0 and j["e2e"]["d2h_bytes_per_step"] > 0 and abs(j["e2e"]["value"] - j["value"]) > 0
     r = j["roofline"]
@@ -36,11 +43,13 @@ def test_committed_gpu_lines(name):
     assert abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and 0 < r["frac"] <= 1
     c = j["clocks"]
     assert set(c) >= {"sm_mhz", "sm_max_mhz", "reasons"} and not ({"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"} & set(c["reasons"]))
-    if j["n_gpus"] == 1:
-        b = j["cpu_baseline"]
-        assert set(b) >= {"value", "unit", "cores", "kind", "sample"} and b["kind"] in ("port", "reference") and b["cores"] >= 1
-    else:
-        assert j["scaling"] == "weak" and j["allreduce_check"]["bitwise_identical_on_all_ranks"]
+    assert j["gpu"]["name"] and j["gpu"]["power_limit_w"] > 0
+    b = j["cpu_baseline"]
+    assert set(b) >= {"value", "unit", "cores", "kind", "sample"} and b["kind"] in ("port", "reference") and b["cores"] >= 1
+    files = {f.stem: np.load(f) for f in dump.iterdir()}
+    want = {"theta", "loss_history", "u0_history"} if config == "hjb" else {"out", "grad_theta", "loss"}
+    assert want <= set(files) and sum(f.stat().st_size for f in dump.iterdir()) <= 64 * 10**6
+    assert all(a.dtype in (np.float32, np.float64) and np.isfinite(a).all() for a in files.values())
 
 
 @pytest.mark.parametrize("extra", [["--n-per-gpu", "1024"], ["--config", "hjb", "--n-per-gpu", "200"]])
@@ -61,3 +70,25 @@ def test_reference_arm_other_ranks_exit_quietly():
     out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--gpus", "2", "--n-per-gpu", "512"],
                          capture_output=True, text=True, timeout=300, env=env)
     assert out.returncode == 0 and not [l for l in out.stdout.splitlines() if l.startswith("{")]
+
+
+def test_dump_outputs_samples_oversized_states_within_64_mb(tmp_path):
+    """dump_outputs with saved states of the fkpp default's size (11 x 256 x 8192 fp32, 92 MB): at most 64 MB in all, headers and
+    the trajectory index included; the sample keeps values and float types; two writes give the same files."""
+    shape = (11, 256, 8192)
+    make = "rng = np.random.default_rng(5); out = rng.standard_normal(%r, dtype=np.float32); grad = rng.standard_normal(311)" % (shape,)
+    code = ("import sys, numpy as np; sys.path.insert(0, sys.argv[1]); import bench\n" + make +
+            "\nfor d in sys.argv[2:]: bench.dump_outputs(d, {'out': out, 'grad_theta': grad, 'loss': np.ones(1, np.float32)})\n")
+    dirs = [tmp_path / "a", tmp_path / "b"]
+    subprocess.run([sys.executable, "-c", code, ROOT] + [str(d) for d in dirs], check=True, timeout=300)
+    exec(make, globals(), ns := {"np": np})
+    names = {"out.npy", "grad_theta.npy", "loss.npy", "out_trajectory_index.npy"}
+    for d in dirs:
+        assert {f.name for f in d.iterdir()} == names and 0.99 * 64e6 < sum(f.stat().st_size for f in d.iterdir()) <= 64e6
+        idx = np.load(d / "out_trajectory_index.npy")
+        assert idx.dtype == np.float64 and np.all(np.diff(idx) > 0) and 0 <= idx[0] and idx[-1] < shape[-1]
+        got = np.load(d / "out.npy")
+        assert got.dtype == np.float32 and got.shape == shape[:-1] + (idx.size,)
+        np.testing.assert_array_equal(got, ns["out"][..., idx.astype(np.int64)])
+        assert np.array_equal(np.load(d / "grad_theta.npy"), ns["grad"])
+    assert all((dirs[0] / n).read_bytes() == (dirs[1] / n).read_bytes() for n in names)

@@ -1,6 +1,6 @@
 """N > 1 path on CPU: world_size-2 gloo.  The ensemble shards across ranks with no data-path collective;
 the one exchange is the all-reduce of [grad_theta; loss].  Each rank evaluates its shard with the CPU
-oracle (standing in for the GPU kernels, which need a B200) and the reduced result must equal the
+oracle (standing in for the GPU kernels, which need an H100) and the reduced result must equal the
 single-process full-ensemble result."""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels, called through the C ABI, against the CPU oracle.
+"""GPU parity tests: the sm_90a kernels, called through the C ABI, against the CPU oracle.
 
 Tolerances (fp32 kernels; the oracle is evaluated in fp64 and, where stated, fp32):
   trajectories  |out - oracle64| <= 3e-4 * (1 + |oracle|)     (fp32 vs fp64 over 30 Tsit5 steps: ~1.4e-4 rel, SURVEY App. C)
@@ -58,8 +58,8 @@ def test_device_tanh_vs_fp64():
 
 
 def _family(monkeypatch, family, rows=0, groups=1):
-    """Select the kernel family of the LV 2-32-32-2 chain: "wm" = warp-collective mma.sync (lv32_wm.cuh), "tc" = tcgen05
-    (lv32_tc.cuh), "auto" = the library's own choice; read by b200ude_create."""
+    """Select the kernel family of the LV 2-32-32-2 chain: "wm" = warp-collective mma.sync (lv32_wm.cuh), "tc" = one trajectory per thread, 3xTF32 mma.sync sweeps
+    through shared memory (lv32_tc.cuh), "auto" = the library's own choice; read by b200ude_create."""
     if family != "auto":
         monkeypatch.setenv("B200UDE_FWD_WM", "1" if family == "wm" else "0")
         monkeypatch.setenv("B200UDE_ADJ_WM", "1" if family == "wm" else "0")
@@ -127,7 +127,7 @@ def test_lv32_families_share_the_forward_record(O, fwd, adj, monkeypatch):
 
 @pytest.mark.parametrize("family", ["auto", "tc"])
 def test_full_size_oracle_parity(O, family, monkeypatch):
-    """The benchmarked size itself (N = 65 536, every SM loaded, several CTAs per SM sharing tensor memory): all trajectories,
+    """The benchmarked size itself (N = 65 536, every SM loaded, several CTAs per SM): all trajectories,
     the loss, the full grad_theta and all of grad_u0 against the fp64 oracle."""
     _family(monkeypatch, family)
     ude = _ude()
@@ -610,7 +610,7 @@ def test_seir_exposure_ude_vs_oracle(O):
 
 @pytest.mark.parametrize("N", [1, 129, 300, 1000])
 def test_seir_tensor_core_vs_runtime_shape_kernels(N, monkeypatch):
-    """The tuned SEIR kernels (k_seir.cu: tcgen05 3xTF32 sweeps, two 128-trajectory groups per CTA) against the
+    """The tuned SEIR kernels (k_seir.cu: 3xTF32 mma.sync sweeps, two 128-trajectory groups per CTA) against the
     runtime-shape kernels (k_generic.cu) on ragged ensemble sizes, incl. a non-trivial cotangent path (adjoint with
     an explicit dL/dout) and grad_u0.  Both are fp32; they differ only in summation order / the 3xTF32 split."""
     ude = _ude()
@@ -889,7 +889,7 @@ def test_vern7_fixed_step_forward_vs_oracle(golden, O):
 
 @pytest.mark.parametrize("tc", ["1", "0"])
 def test_vern7_seir_tensor_core_forward_vs_oracle(O, tc, monkeypatch):
-    """BASELINE config 3 as stated: the SEIR exposure UDE solved with Vern7 (seir_exposure.jl:138) -- fixed step on the tcgen05
+    """BASELINE config 3 as stated: the SEIR exposure UDE solved with Vern7 (seir_exposure.jl:138) -- fixed step on the tensor-core
     kernels (seir::vern7_forward_kernel) and, for comparison, on the runtime-shape kernels -- against the oracle's Vern7; the
     interpolating adjoint of the Vern7 handle (a Tsit5 re-solve on the same kernels) against the oracle's Tsit5 adjoint."""
     monkeypatch.setenv("B200UDE_SEIR_VERN7_TC", tc)

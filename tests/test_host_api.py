@@ -83,8 +83,9 @@ def test_sciml_train_bfgs_and_callback_halt():
     A = torch.tensor([[3.0, 0.5], [0.5, 1.0]])
     b = torch.tensor([1.0, -2.0])
 
-    def loss(th):
-        return 0.5 * th @ (A @ th) - b @ th
+    def loss(th):   # sciml_train places a host theta on the GPU when there is one
+        A_, b_ = A.to(th.device), b.to(th.device)
+        return 0.5 * th @ (A_ @ th) - b_ @ th
     res = ude.sciml_train(loss, np.zeros(2, np.float32), ude.BFGS(initial_stepnorm=0.01), maxiters=200)
     sol = torch.linalg.solve(A, b)
     assert torch.allclose(res.minimizer.cpu(), sol, atol=1e-4)

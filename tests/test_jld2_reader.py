@@ -1,13 +1,22 @@
 """universal_differential_equations_b200/jld2.py (reader + writer of plain numeric JLD2 datasets) against the reference's own result files (LotkaVolterra/results/*.jld2, written by
 scenario_1.jl:210-213 ... hudson_bay.jl:231-235): the arrays it decodes by walking the HDF5 structure equal the committed golden vectors
-(which tools/make_golden.py cut out at fixed byte offsets).  Needs /root/reference (the build container); skipped elsewhere."""
+(which tools/make_golden.py cut out at fixed byte offsets).  The four result files are stored byte for byte (zlib-compressed) in
+tests/golden/reference_results.npz."""
 import os
 
 import numpy as np
 import pytest
 
-REF = "/root/reference/LotkaVolterra/results"
-needs_ref = pytest.mark.skipif(not os.path.isdir(REF), reason="the reference tree is only mounted in the build container")
+GOLDEN_FILES = os.path.join(os.path.dirname(__file__), "golden", "reference_results.npz")
+
+
+@pytest.fixture(scope="module")
+def REF(tmp_path_factory):
+    d = tmp_path_factory.mktemp("results")
+    with np.load(GOLDEN_FILES) as z:
+        for k in z.files:
+            (d / f"{k}.jld2").write_bytes(z[k].tobytes())
+    return str(d)
 
 
 def test_save_load_round_trip(tmp_path):
@@ -31,8 +40,7 @@ def test_save_load_round_trip(tmp_path):
     assert jld2.lookup3(b"") == 0xDEADBEEF and jld2.lookup3(b"Four score and seven years ago") == 0x17770551   # lookup3.c's own self-test values
 
 
-@needs_ref
-def test_writer_reproduces_the_reference_files_own_bytes(tmp_path):
+def test_writer_reproduces_the_reference_files_own_bytes(tmp_path, REF):
     """The dataset object headers `save` emits for the reference's X / t arrays are byte-for-byte those JLD2 itself wrote
     (Hudson_Bay_recovery.jld2: compact layout), at the same addresses; for a contiguous dataset (scenario 1's loss history) everything but
     the data address agrees and the data follows the header as it does there.  The reference files' own checksums validate."""
@@ -53,8 +61,7 @@ def test_writer_reproduces_the_reference_files_own_bytes(tmp_path):
     np.testing.assert_array_equal(mine.read("losses"), s1.read("losses"))
 
 
-@needs_ref
-def test_reader_reproduces_the_golden_vectors(golden):
+def test_reader_reproduces_the_golden_vectors(golden, REF):
     from universal_differential_equations_b200 import jld2
     cases = {
         "scenario_1": ("Scenario_1_recovery_0.005.jld2", {"X": "X", "losses": "losses"}),
@@ -71,8 +78,7 @@ def test_reader_reproduces_the_golden_vectors(golden):
             np.testing.assert_array_equal(got[fk], want, err_msg=f"{name}:{gk}")
 
 
-@needs_ref
-def test_reader_lists_structs_without_decoding_them():
+def test_reader_lists_structs_without_decoding_them(REF):
     from universal_differential_equations_b200 import jld2
     f = jld2.JLD2File(os.path.join(REF, "Scenario_1_recovery_0.005.jld2"))
     assert {"solution", "X", "t", "losses", "trained_parameters", "long_estimate"} <= set(f.keys())
@@ -84,8 +90,7 @@ def test_reader_lists_structs_without_decoding_them():
     assert set(jld2.load(os.path.join(REF, "Hudson_Bay_recovery.jld2"))) >= {"X", "t", "losses", "model_parameter"}
 
 
-@needs_ref
-def test_parameter_containers_are_followed_to_their_arrays(golden):
+def test_parameter_containers_are_followed_to_their_arrays(golden, REF):
     """`trained_parameters` (a ComponentVector) and `initial_parameters` (Lux's NamedTuple of layers) are Julia structs whose array fields
     are references to other objects of the file: read_tree follows them and returns the very arrays the golden vectors hold."""
     from universal_differential_equations_b200 import jld2

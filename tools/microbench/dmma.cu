@@ -1,4 +1,4 @@
-// dmma.cu -- fp64 tensor-core (mma.sync.m8n8k4.f64, SASS DMMA.8x8x4) issue rate on B200 (sm_100a) as a function of warps per
+// dmma.cu -- fp64 tensor-core (mma.sync.m8n8k4.f64, SASS DMMA.8x8x4) issue rate on H100 (sm_90a) as a function of warps per
 // scheduler and independent accumulator chains per warp.  Sets the ceiling of the fused deep-BSDE sweeps (csrc/bsde.cu).
 #include <cuda_runtime.h>
 #include <cstdio>

@@ -1,4 +1,4 @@
-// mma.cu -- legacy warp-level tensor-core (mma.sync) throughput on B200 (sm_100a): TF32 m16n8k8,
+// mma.cu -- legacy warp-level tensor-core (mma.sync) throughput on H100 (sm_90a): TF32 m16n8k8,
 // BF16 m16n8k16.  Decides whether the 32x32 layers of the UDE chain can be moved off the FP32 pipe
 // with a 3xTF32 split.  Reports MMA instructions / clk / SM and dense TFLOP/s.
 #include <cuda_runtime.h>
@@ -35,7 +35,7 @@ __global__ void k_mma(float *out)
     for (int i = 0; i < NACC; ++i) s += d[i][0] + d[i][1] + d[i][2] + d[i][3];
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-// mixed: FFMA2 stream and MMA stream interleaved in the same warp: do the pipes overlap?
+// mixed: FFMA stream (two per float2) and MMA stream interleaved in the same warp: do the pipes overlap?
 __global__ void k_mix(float *out, float x)
 {
     float d[8][4];
@@ -51,11 +51,7 @@ __global__ void k_mix(float *out, float x)
             mma_tf32(d[i], a, b);
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
-                unsigned long long ra = *reinterpret_cast<unsigned long long *>(&f[i * 2 + q]), rd;
-                float2 xx = make_float2(x, x);
-                unsigned long long rb = *reinterpret_cast<unsigned long long *>(&xx);
-                asm volatile("fma.rn.f32x2 %0, %1, %2, %1;" : "=l"(rd) : "l"(ra), "l"(rb));
-                f[i * 2 + q] = *reinterpret_cast<float2 *>(&rd);
+                f[i * 2 + q] = make_float2(__fmaf_rn(f[i * 2 + q].x, x, f[i * 2 + q].x), __fmaf_rn(f[i * 2 + q].y, x, f[i * 2 + q].y));
             }
         }
     }
@@ -94,7 +90,7 @@ int main()
                 case 3: k_mma<1, 1><<<blocks, threads>>>(out); name = "bf16 m16n8k16 1 chain"; mmas = ITER; flop_per_mma = 2.0 * 16 * 8 * 16; break;
                 case 4: k_mma<1, 4><<<blocks, threads>>>(out); name = "bf16 m16n8k16 4 chains"; mmas = 4.0 * ITER; flop_per_mma = 2.0 * 16 * 8 * 16; break;
                 case 5: k_mma<1, 16><<<blocks, threads>>>(out); name = "bf16 m16n8k16 16 chains"; mmas = 16.0 * ITER; flop_per_mma = 2.0 * 16 * 8 * 16; break;
-                case 6: k_mix<<<blocks, threads>>>(out, 1.0000001f); name = "mix 8 tf32 mma + 16 ffma2"; mmas = 8.0 * ITER; flop_per_mma = 2.0 * 16 * 8 * 8; extra_flop = 16.0 * ITER * 2 * 2 * 32; break;
+                case 6: k_mix<<<blocks, threads>>>(out, 1.0000001f); name = "mix 8 tf32 mma + 32 ffma"; mmas = 8.0 * ITER; flop_per_mma = 2.0 * 16 * 8 * 8; extra_flop = 16.0 * ITER * 2 * 2 * 32; break;
                 }
                 cudaEventRecord(e1);
                 cudaEventSynchronize(e1);

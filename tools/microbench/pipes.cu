@@ -1,6 +1,6 @@
 // pipes.cu -- instruction-throughput microbenchmarks that set the FP32 roofline denominators for
-// the UDE kernels on B200 (sm_100a): scalar FFMA vs packed FFMA2, register vs uniform-register
-// (constant-bank) operands, MUFU, LDCU.128 / LDS.128 feeding rates.  Build: nvcc -arch=sm_100a.
+// the UDE kernels on H100 (sm_90a): scalar FFMA vs float2 pairs (two FFMAs each), register vs uniform-register
+// (constant-bank) operands, MUFU, LDC.128 / LDS.128 feeding rates.  Build: nvcc -gencode arch=compute_90a,code=sm_90a.
 // Each kernel runs ITER iterations of an unrolled body on `warps` warps per SM sub-partition and
 // reports instructions/clk/SM (from clock64) and the derived GFLOP/s at the measured wall time.
 #include <cuda_runtime.h>
@@ -14,10 +14,7 @@ __constant__ float cw[2048];
 
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c)
 {
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b),
-                       rc = *reinterpret_cast<unsigned long long *>(&c), rd;
-    asm volatile("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    return *reinterpret_cast<float2 *>(&rd);
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));   // sm_90 has no packed fp32 FMA
 }
 __device__ __forceinline__ float ffma_v(float a, float b, float c)
 {
@@ -60,7 +57,7 @@ __global__ void k_ffma_const(float *out, float y)
     for (int i = 0; i < 16; ++i) s += a[i];
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-// 2: packed FFMA2, 3 register operands, 16 independent chains (32 FMA lanes-worth per thread)
+// 2: float2 pairs (two FFMAs each), 3 register operands, 16 independent chains (32 FMA lanes-worth per thread)
 __global__ void k_ffma2_reg(float *out, float x, float y)
 {
     float2 a[16];
@@ -78,7 +75,7 @@ __global__ void k_ffma2_reg(float *out, float x, float y)
     for (int i = 0; i < 16; ++i) s += a[i].x + a[i].y;
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-// 3: packed FFMA2 with a scalar (broadcast) multiplier from the constant bank
+// 3: float2 pairs with a scalar (broadcast) multiplier from the constant bank
 __global__ void k_ffma2_const(float *out, float y)
 {
     float2 a[16];
@@ -121,7 +118,7 @@ __global__ void k_mufu(float *out)
     for (int i = 0; i < 8; ++i) s += a[i];
     out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-// 7: the real inner loop shape, scalar: 32x32 layer, weights from the constant bank (LDCU.128 : 4 FFMA)
+// 7: the real inner loop shape, scalar: 32x32 layer, weights from the constant bank (LDC.128 : 4 FFMA)
 __global__ void k_layer_const_t1(float *out)
 {
     float h[32];
@@ -147,7 +144,7 @@ __global__ void k_layer_const_t1(float *out)
     }
     out[blockIdx.x * blockDim.x + threadIdx.x] = keep;
 }
-// 8: same with two trajectories per thread packed in FFMA2 (LDCU.128 : 4 FFMA2 = 8 FMA)
+// 8: same with two trajectories per thread in float2 pairs (LDC.128 : 8 FFMA)
 __global__ void k_layer_const_t2(float *out)
 {
     float2 h[32];
@@ -267,15 +264,15 @@ int main()
                 switch (kid) {
                 case 0: k_ffma_reg<<<blocks, threads>>>(out, 1.0000001f, 1e-9f); name = "ffma_reg"; fma = 64.0 * ITER; inst = fma; break;
                 case 1: k_ffma_const<<<blocks, threads>>>(out, 1e-9f); name = "ffma_const(UR)"; fma = 64.0 * ITER; inst = fma; break;
-                case 2: k_ffma2_reg<<<blocks, threads>>>(out, 1.0000001f, 1e-9f); name = "ffma2_reg"; fma = 128.0 * ITER; inst = 64.0 * ITER; break;
-                case 3: k_ffma2_const<<<blocks, threads>>>(out, 1e-9f); name = "ffma2_const(UR)"; fma = 128.0 * ITER; inst = 64.0 * ITER; break;
+                case 2: k_ffma2_reg<<<blocks, threads>>>(out, 1.0000001f, 1e-9f); name = "ffma2_reg"; fma = 128.0 * ITER; inst = fma; break;
+                case 3: k_ffma2_const<<<blocks, threads>>>(out, 1e-9f); name = "ffma2_const(UR)"; fma = 128.0 * ITER; inst = fma; break;
                 case 4: k_mufu<0><<<blocks, threads>>>(out); name = "mufu_ex2"; fma = 0; inst = 64.0 * ITER; break;
                 case 5: k_mufu<1><<<blocks, threads>>>(out); name = "mufu_rcp"; fma = 0; inst = 64.0 * ITER; break;
                 case 6: k_mufu<2><<<blocks, threads>>>(out); name = "mufu_tanh"; fma = 0; inst = 64.0 * ITER; break;
                 case 7: k_layer_const_t1<<<blocks, threads>>>(out); name = "layer32 const T1"; fma = 1024.0 * (ITER / 16); inst = fma * 1.25; break;
-                case 8: k_layer_const_t2<<<blocks, threads>>>(out); name = "layer32 const T2/FFMA2"; fma = 2048.0 * (ITER / 16); inst = 1024.0 * (ITER / 16) * 1.25; break;
+                case 8: k_layer_const_t2<<<blocks, threads>>>(out); name = "layer32 const T2"; fma = 2048.0 * (ITER / 16); inst = fma * 1.125; break;
                 case 9: k_layer_smem_t1<<<blocks, threads>>>(out); name = "layer32 smem T1"; fma = 1024.0 * (ITER / 16); inst = fma * 1.25; break;
-                case 10: k_layer_smem_t2<<<blocks, threads>>>(out); name = "layer32 smem T2/FFMA2"; fma = 2048.0 * (ITER / 16); inst = 1024.0 * (ITER / 16) * 1.25; break;
+                case 10: k_layer_smem_t2<<<blocks, threads>>>(out); name = "layer32 smem T2"; fma = 2048.0 * (ITER / 16); inst = fma * 1.125; break;
                 }
                 cudaEventRecord(e1);
                 cudaEventSynchronize(e1);

@@ -68,7 +68,7 @@ flop = 2.0 * fma * (1 + 6 * 84) + 2.0 * 3 * fma * 6 * 84
 from oracle import oracle as O
 cpu = cpu_rate(O.seir_model(), theta, u0, y, w, 0.25, 84, 4, 2048)
 report("SEIR exposure UDE 7-state 3-64-64-1, Tsit5 dt=0.25 x84, N=65536 (BASELINE config 3, reference shape)", N, tf, ta, flop, cpu,
-       {"kernels": "seir::forward_kernel / seir::adjoint_kernel (tcgen05 3xTF32)", "flop_per_trajectory": flop})
+       {"kernels": "seir::forward_kernel / seir::adjoint_kernel (3xTF32 mma.sync)", "flop_per_trajectory": flop})
 
 # ---- config 4: Fisher-KPP UPDE, 256-point grid, 1-16-16-1 tanh reaction chain + 3-tap periodic stencil, Tsit5
 Nx, N = 256, 8192

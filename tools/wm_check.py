@@ -1,5 +1,5 @@
 """Dev check of the warp-collective LV kernels (lv32_wm.cuh): parity vs the fp64 oracle and timings per family.
-Run on a B200:  python tools/wm_check.py"""
+Run on an H100:  python tools/wm_check.py"""
 import os, sys, json
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,8 +1,8 @@
-"""B200-native drop-in for the UDE training path of ChrisRackauckas/universal_differential_equations.
+"""H100-native (sm_90a) drop-in for the UDE training path of ChrisRackauckas/universal_differential_equations.
 
 Only the hot path is here: ensemble forward solve of a universal differential equation
 (known physics + embedded dense chain, Tsit5) and its interpolating-adjoint gradient,
-as hand-written sm_100a kernels behind a C ABI (include/b200ude.h), plus a host-side
+as hand-written sm_90a kernels behind a C ABI (include/b200ude.h), plus a host-side
 mirror of the reference's call surface (sciml.py).  See DESIGN.md.
 """
 from . import _lib  # noqa: F401

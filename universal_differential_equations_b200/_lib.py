@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library (include/b200ude.h -> csrc/libb200ude.so).
 
 This is the only place Python touches the product's native code.  There is no
-CPU fallback: if the shared library is missing, or there is no sm_100 device,
+CPU fallback: if the shared library is missing, or there is no sm_90 device,
 the calls raise.  Nothing here imports the CPU oracle.
 """
 import ctypes as C
@@ -78,7 +78,7 @@ class B200UDEError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile csrc/ for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/ for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
     jobs = str(min(8, os.cpu_count() or 1))
     subprocess.check_call(["make", "-C", CSRC, "-j", jobs] + ([] if verbose else ["-s"]))
     return SO_PATH

@@ -1,4 +1,4 @@
-// b200ude.cu -- C-ABI entry points (include/b200ude.h) over the sm_100a kernels.
+// b200ude.cu -- C-ABI entry points (include/b200ude.h) over the sm_90a kernels.
 //
 // No torch types, no exceptions across the boundary, no CPU fallback: if there is no usable
 // CUDA device, or the requested configuration has no kernel, the call fails with a code and a
@@ -241,7 +241,7 @@ int32_t tsit5_forward(b200ude_handle *h, const float *u0, size_t N, float *out, 
     }
     switch (h->kid) {
     case K_LV32:
-        // small / medium ensembles: the warp-collective family (latency per stage ~4x lower); large ones: tcgen05
+        // small / medium ensembles: the warp-collective family (latency per stage ~4x lower); large ones: one trajectory per thread
         e = use_wm(h->var.fwd_wm, N, h->wm_fwd_max) ? launch_fwd_lv32_wm(h->var, h->tab, p, st) : launch_fwd_lv32(h->var, h->tab, p, st);
         break;
     case K_LV5P0: e = launch_fwd_lv5(0, h->var, h->tab, p, st); break;
@@ -600,7 +600,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                     "create: the discrete adjoint has kernels for fixed-step Tsit5 on the LV chains 2-32-32-2 and 2-5-5-5-2 (the scripts that use ForwardDiffSensitivity)");
     if (kid == K_NONE)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
-                    "create: no sm_100a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");
+                    "create: no sm_90a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0) return fail(nullptr, B200UDE_ENODEVICE, "create: no CUDA device (%s)", cudaGetErrorString(e));
@@ -608,8 +608,8 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, d->device);
     if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 10)
-        return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_100a code only", d->device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_90a code only", d->device, prop.major, prop.minor);
     e = cudaSetDevice(d->device);
     if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaSetDevice: %s", cudaGetErrorString(e));
 
@@ -641,15 +641,15 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     h->var.fwd_smem = env_int("B200UDE_FWD_SMEM", 0);
     h->var.fwd_T = env_int("B200UDE_FWD_T", 1) == 2 ? 2 : 1;
     h->var.adj_smem = env_int("B200UDE_ADJ_SMEM", 0);
-    // default: tcgen05 (3xTF32) kernels; B200UDE_FWD_TC=0 / B200UDE_ADJ_TC=0 select the FFMA2-packed CUDA-core kernels
+    // default: tensor-core (3xTF32 mma.sync) kernels; B200UDE_FWD_TC=0 / B200UDE_ADJ_TC=0 select the packed CUDA-core kernels
     h->var.fwd_tc = env_int("B200UDE_FWD_TC", 1);
-    h->var.adj_tc = env_int("B200UDE_ADJ_TC", 2);   // 2: gradient GEMM on mma.sync (3xTF32), 1: on the FMA pipe (FFMA2)
+    h->var.adj_tc = env_int("B200UDE_ADJ_TC", 2);   // 2: gradient GEMM on mma.sync (3xTF32), 1: on the FMA pipe
     // warp-collective mma.sync family (lv32_wm.cuh): -1 = chosen per call from the ensemble size, 0 = off, 1 = always
     h->var.fwd_wm = env_int("B200UDE_FWD_WM", -1);
     h->var.adj_wm = env_int("B200UDE_ADJ_WM", -1);
     h->var.wm_groups = env_int("B200UDE_WM_G", 1);
     h->var.wm_rows = env_int("B200UDE_WM_R", 0);
-    h->var.wm_r1_max = env_int("B200UDE_WM_R1_MAX", 4736);
+    h->var.wm_r1_max = env_int("B200UDE_WM_R1_MAX", h->sm_count * 4 * 8);   // one 8-trajectory warp per scheduler: 4224 on 132 SMs
     h->wm_fwd_max = (size_t)env_int("B200UDE_WM_FWD_MAX", 1 << 26);
     h->wm_adj_max = (size_t)env_int("B200UDE_WM_ADJ_MAX", 1 << 26);
 

@@ -16,7 +16,7 @@
 //   * fp32, and wider networks: one library GEMM per layer (cuBLAS) with hand-written kernels between them (fused Euler-Maruyama
 //     with the increments regenerated in place, relu / masks, the loss and its cotangents);
 //   * the backward sweep is the exact reverse-mode derivative of the discretised solve (what Tracker computes through the SDE
-//     solver in the reference).  Nothing is recomputed: with 180 GB of HBM every step's activations and cotangents stay resident
+//     solver in the reference).  Nothing is recomputed: with 80 GB of HBM every step's activations and cotangents stay resident
 //     ((4 d + 6 hls) x paths x n_steps elements, 1.5 GB for the benchmark's 10 000 fp64 paths);
 //   * every activation matrix carries a constant row of ones below it, and theta stores a layer as vec(W) followed by b, i.e.
 //     the column-major out x (in + 1) matrix [W | b]: the forward product over the augmented activations adds the bias for free,
@@ -74,7 +74,7 @@ __device__ __forceinline__ void normals4(uint64_t seed, uint32_t path, uint32_t 
 
 // Brownian increments of a whole iteration for the fused sweeps: dW[n][path][m] = sqrt(dt) * normal(path, m, n), one thread per
 // (step, path, block of 4 components).  A separate, fully parallel pass: inside the forward sweep the fp64 log / sincos chains of the
-// Box-Muller transform sat on every warp's critical path (a third of the sweep's time, measured with clock64()).
+// Box-Muller transform sit on every warp's critical path.
 __global__ void k_dw_tape(double *__restrict__ dW, const uint64_t *seed, uint32_t path0, int M, int N, int d, double sq)
 {
     const int nq = (d + 3) / 4;
@@ -931,7 +931,7 @@ struct b200ude_bsde_handle {
     void *mask = nullptr;     // relu' bits of the hidden layers (fused sweeps)
     void *dW = nullptr;       // Brownian increments of the iteration (fused sweeps)
     FusedArgs fa;             // slab tables (the pointers are filled per call)
-    int sm_count = 148;
+    int sm_count = 0;         // the device's SM count (set at create; sizes the persistent cotangent-sweep grid)
     bool fwd_pairs = true;    // forward sweep with two warps per path tile (k_fused_forward2)
     void *wg_partial = nullptr;   // per-CTA partial sums of the fused weight-gradient products (null: library GEMMs)
     int wg_splits = 0;
@@ -1240,8 +1240,8 @@ int32_t b200ude_bsde_create(const b200ude_bsde_desc *d, b200ude_bsde_handle **ou
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return bfail(nullptr, B200UDE_ENODEVICE, "bsde_create: no CUDA device");
     if (d->device < 0 || d->device >= ndev) return bfail(nullptr, B200UDE_EINVAL, "bsde_create: device %d of %d", d->device, ndev);
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, d->device) != cudaSuccess || prop.major != 10)
-        return bfail(nullptr, B200UDE_ENODEVICE, "bsde_create: device %d is not an sm_100 part", d->device);
+    if (cudaGetDeviceProperties(&prop, d->device) != cudaSuccess || prop.major != 9 || prop.minor != 0)
+        return bfail(nullptr, B200UDE_ENODEVICE, "bsde_create: device %d is not an sm_90 part", d->device);
     if (cudaSetDevice(d->device) != cudaSuccess) return bfail(nullptr, B200UDE_ENODEVICE, "bsde_create: cudaSetDevice failed");
     b200ude_bsde_handle *h = new (std::nothrow) b200ude_bsde_handle();
     if (!h) return bfail(nullptr, B200UDE_ENOMEM, "bsde_create: out of host memory");

@@ -8,7 +8,7 @@
 // runtime-shape kernels in ude_generic.cuh, which remain the path for every other chain shape).  What is tuned here:
 //   * chain weights are compile-time-indexed 128-bit constant-bank loads (uniform registers), the RHS is one function;
 //   * u and lambda neighbours travel through ONE double-buffered shared-memory exchange per stage (one barrier);
-//   * the ensemble-summed gradient of the H x H layer is a per-warp FFMA2 outer-product GEMM over the warp's 32 points
+//   * the ensemble-summed gradient of the H x H layer is a per-warp FFMA outer-product GEMM over the warp's 32 points
 //     (operands staged as conflict-free 128-bit rows, 2 x 4 register tile per lane), everything thin (first/last layer,
 //     biases, stencil weights, D0) accumulates in per-lane registers and is reduced once, at the end of the kernel, with
 //     a fixed shuffle tree and a fixed-order sum over the CTA's warps -> bitwise reproducible.
@@ -400,7 +400,7 @@ __global__ void __launch_bounds__(256) adjoint_kernel(AdjParams p, Geom geo)
 
 // =====================================================================================================================
 // Packed variant (even grids): a thread carries TWO adjacent grid points in the halves of 64-bit register pairs and does
-// the chain arithmetic with FFMA2 (weights are scalar broadcast operands), which halves the FMA / constant-load instruction
+// the chain arithmetic on float2 pairs (weights are scalar broadcast operands), which halves the constant-load instruction
 // count of the one-point-per-thread kernels above (those were at 90 % issue-slot utilisation).  Same algorithm, same
 // handle-internal layouts; a trajectory occupies Nx/2 consecutive threads.
 // =====================================================================================================================
@@ -439,8 +439,8 @@ __device__ __noinline__ float2 chain_value2(float2 g, int zsel)
 #pragma unroll
     for (int j4 = 0; j4 < H; j4 += 4) {
         const float4 w = ldw4(zb + O::W3 + j4);
-        // (the batched-inversion tanh of lv32_packed.cuh was measured 1-3 % SLOWER here: these kernels are issue-bound and its
-        // overflow clamps cost more slots than the saved reciprocals)
+        // (the batched-inversion tanh of lv32_packed.cuh is not used here: these kernels are issue-bound and its overflow clamps
+        // cost more issue slots than the saved reciprocals)
         y0 = fma2(bc(w.x), tanh2<TM>(a2[j4 + 0]), y0);
         y1 = fma2(bc(w.y), tanh2<TM>(a2[j4 + 1]), y1);
         y0 = fma2(bc(w.z), tanh2<TM>(a2[j4 + 2]), y0);

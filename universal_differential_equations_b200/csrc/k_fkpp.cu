@@ -5,7 +5,7 @@
 namespace b200ude {
 
 #include <cstdlib>
-// packed kernels (two adjacent grid points per thread, FFMA2) for even grids; B200UDE_FKPP_PACKED=0 selects the scalar ones
+// packed kernels (two adjacent grid points per thread) for even grids; B200UDE_FKPP_PACKED=0 selects the scalar ones
 static bool use_packed(int Nx)
 {
     const char *e = getenv("B200UDE_FKPP_PACKED");

@@ -30,7 +30,7 @@ static cudaError_t launch_one(const AdjParams &p, int grid, cudaStream_t st)
 template <int TM, int GEMM, bool DISC = false>
 static cudaError_t launch_tc(const AdjParams &p, int *rows_out, cudaStream_t st)
 {
-    auto kern = lv32::tc::adjoint_kernel<TM, 128, 4, GEMM, false, DISC>;
+    auto kern = lv32::tc::adjoint_kernel<TM, 128, 3, GEMM, false, DISC>;
     constexpr size_t smem = sizeof(lv32::tc::WarpStageT) * 4;
     static PerDeviceOnce once;
     bool &attr_set = once.flag();
@@ -51,7 +51,7 @@ static cudaError_t launch_tc(const AdjParams &p, int *rows_out, cudaStream_t st)
 template <int TM>
 static cudaError_t launch_tc_adaptive(const AdjParams &p, const AdaptiveGrid &ag, int *rows_out, cudaStream_t st)
 {
-    auto kern = lv32::tc::adjoint_kernel<TM, 128, 4, 1, true>;
+    auto kern = lv32::tc::adjoint_kernel<TM, 128, 3, 1, true>;
     constexpr size_t smem = sizeof(lv32::tc::WarpStageT) * 4;
     static PerDeviceOnce once;
     bool &attr_set = once.flag();

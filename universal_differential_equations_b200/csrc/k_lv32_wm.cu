@@ -41,8 +41,7 @@ cudaError_t launch_fwd_lv32_wm(const Variant &v, const ConstTables &t, const Fwd
 template <int TM, int R>
 static cudaError_t launch_adj(const ConstTables &t, const AdjParams &p, int *rows_out, cudaStream_t st)
 {
-    // single-warp CTAs, no register cap: capping at 168 registers (3 warps per scheduler instead of 2) was measured 9 % slower at
-    // N = 65536 and 35 % slower at N = 8192 (spill code in the stage loop)
+    // single-warp CTAs, no register cap: a 168-register cap (3 warps per scheduler instead of 2) puts spill code in the stage loop
     constexpr int WPC = 1;
     auto kern = lv32::wm::adjoint_kernel<TM, R, WPC, 1>;
     constexpr size_t smem = lv32::wm::RAW_FLOATS * 4 + sizeof(lv32::wm::WarpTiles<R>) * WPC;

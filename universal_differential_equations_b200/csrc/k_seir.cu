@@ -24,7 +24,7 @@ template <int TM>
 static cudaError_t launch_fwd(const FwdParams &p, cudaStream_t st)
 {
     auto kern = seir::forward_kernel<TM>;
-    constexpr size_t smem = 2 * seir::HS * seir::HS * sizeof(float);
+    constexpr size_t smem = (2 * seir::HS * seir::SWS + seir::BLOCK * seir::SLD64) * sizeof(float);
     static PerDeviceOnce once;
     cudaError_t e = set_smem(kern, smem, &once.flag());
     if (e != cudaSuccess) return e;
@@ -36,7 +36,7 @@ template <int TM>
 static cudaError_t launch_fwd_adaptive_t(const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
 {
     auto kern = seir::adaptive_forward_kernel<TM>;
-    constexpr size_t smem = 2 * seir::HS * seir::HS * sizeof(float);
+    constexpr size_t smem = (2 * seir::HS * seir::SWS + seir::BLOCK * seir::SLD64) * sizeof(float);
     static PerDeviceOnce once;
     cudaError_t e = set_smem(kern, smem, &once.flag());
     if (e != cudaSuccess) return e;
@@ -48,7 +48,7 @@ template <int TM, int GEMM>
 static cudaError_t launch_adj(const AdjParams &p, cudaStream_t st)
 {
     auto kern = seir::adjoint_kernel<TM, GEMM>;
-    constexpr size_t smem = 4 * seir::HS * seir::HS * sizeof(float) + seir::GROUPS * sizeof(seir::GroupStage);
+    constexpr size_t smem = 2 * seir::HS * seir::SWS * sizeof(float) + seir::GROUPS * sizeof(seir::GroupStage) + seir::BLOCK * 33 * sizeof(float);
     static PerDeviceOnce once;
     cudaError_t e = set_smem(kern, smem, &once.flag());
     if (e != cudaSuccess) return e;
@@ -60,7 +60,7 @@ template <int TM>
 static cudaError_t launch_adj_adaptive_t(const AdjParams &p, const AdaptiveGrid &ag, cudaStream_t st)
 {
     auto kern = seir::adjoint_kernel<TM, 1, true>;
-    constexpr size_t smem = 4 * seir::HS * seir::HS * sizeof(float) + seir::GROUPS * sizeof(seir::GroupStage);
+    constexpr size_t smem = 2 * seir::HS * seir::SWS * sizeof(float) + seir::GROUPS * sizeof(seir::GroupStage) + seir::BLOCK * 33 * sizeof(float);
     static PerDeviceOnce once;
     cudaError_t e = set_smem(kern, smem, &once.flag());
     if (e != cudaSuccess) return e;
@@ -79,7 +79,7 @@ template <int TM>
 static cudaError_t launch_fwd_vern7_t(const FwdParams &p, cudaStream_t st)
 {
     auto kern = seir::vern7_forward_kernel<TM>;
-    constexpr size_t smem = 2 * seir::HS * seir::HS * sizeof(float);
+    constexpr size_t smem = (2 * seir::HS * seir::SWS + seir::BLOCK * seir::SLD64) * sizeof(float);
     static PerDeviceOnce once;
     cudaError_t e = set_smem(kern, smem, &once.flag());
     if (e != cudaSuccess) return e;
@@ -99,7 +99,7 @@ cudaError_t launch_adj_seir(const Variant &v, const ConstTables &t, const AdjPar
     cudaError_t e = upload_tables(t, st);
     if (e != cudaSuccess) return e;
     *rows_out = adj_rows_seir(p.N);
-    if (v.adj_tc == 1) return v.approx_tanh ? launch_adj<1, 0>(p, st) : launch_adj<0, 0>(p, st);   // B200UDE_ADJ_TC=1: FFMA2 gradient GEMM
+    if (v.adj_tc == 1) return v.approx_tanh ? launch_adj<1, 0>(p, st) : launch_adj<0, 0>(p, st);   // B200UDE_ADJ_TC=1: FFMA gradient GEMM
     return v.approx_tanh ? launch_adj<1, 1>(p, st) : launch_adj<0, 1>(p, st);
 }
 

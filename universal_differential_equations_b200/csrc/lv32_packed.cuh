@@ -1,15 +1,13 @@
 // lv32_packed.cuh -- the headline kernels: Lotka-Volterra UDE with the 2 -> 32 -> 32 -> 2 tanh chain
-// (BASELINE config 2), two trajectories per thread packed into FFMA2 lanes.
+// (BASELINE config 2), two trajectories per thread packed into float2 pairs.
 //
-// Blackwell's FFMA2 (PTX fma.rn.f32x2) performs two fp32 FMAs per issue slot and accepts a SCALAR
-// operand that is broadcast to both halves -- from a uniform register (weights read from the
-// constant bank by LDCU.128, four weights per load) or from a normal register.  A thread therefore
-// carries a PAIR of trajectories (a, b) in the two halves of every 64-bit register pair:
+// A thread carries a PAIR of trajectories (a, b) in the two halves of a float2, and every weight
+// (read from the constant bank, four weights per 128-bit load) is applied to both halves:
 //   - chain forward / reverse sweeps:  acc(a,b) = fma2(w_scalar, h(a,b), acc(a,b))
 //   - ensemble-summed parameter gradient: acc(a,b)[j][i] = fma2(q(a,b)[j], h(a,b)[i], acc(a,b)[j][i]),
 //     halves added together once at the end of the kernel.
-// This halves the issue slots of the FP32 work (the scalar version is issue-bound: 1 LDCU per 4 FFMA)
-// and amortises every weight load over 8 FMAs.
+// This amortises every weight load over 8 FMAs (the one-trajectory version is issue-bound: 1 constant
+// load per 4 FFMA).  On sm_90 fma2 is two scalar FFMAs (there is no packed fp32 FMA).
 //
 // Reference semantics replaced: see ude_common.cuh / ude_adjoint.cuh headers.
 #pragma once
@@ -28,27 +26,13 @@ constexpr int OFF_B3 = OFF_W3 + 64;    // 1216
 constexpr int P = OFF_B3 + 2;          // 1218
 
 // ---- packed helpers -------------------------------------------------------------------------------
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c)
-{
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b),
-                       rc = *reinterpret_cast<unsigned long long *>(&c), rd;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    return *reinterpret_cast<float2 *>(&rd);
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b)
-{
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b), rd;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2 *>(&rd);
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b)
-{
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b), rd;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2 *>(&rd);
-}
+// sm_90 has no packed fp32 instruction: each half is one round-to-nearest FFMA / FMUL / FADD, which gives the same
+// result per element as fma.rn.f32x2 and keeps the pairing (weight loads amortised over both trajectories).
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 bc(float s) { return make_float2(s, s); }  // scalar broadcast operand
-// s * x + y with scalar s (broadcast form of FFMA2)
+// s * x + y with scalar s broadcast to both halves
 __device__ __forceinline__ float2 fmas(float s, float2 x, float2 y) { return fma2(bc(s), x, y); }
 
 template <int TM>
@@ -111,7 +95,7 @@ struct Pair2 {
 };
 
 // ---- UDE right-hand side for a pair of trajectories (NOT inlined: keeps the weight loads next to
-// their FFMA2s instead of hoisted out of the time loop and spilled; see ude_common.cuh) -------------
+// their FFMAs instead of hoisted out of the time loop and spilled; see ude_common.cuh) -------------
 template <int TM, class W>
 __device__ __noinline__ Pair2 rhs_pair(W w, Pair2 u)
 {

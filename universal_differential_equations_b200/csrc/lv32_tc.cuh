@@ -1,17 +1,15 @@
-// lv32_tc.cuh -- tensor-core (tcgen05 / TMEM) variant of the LV 2 -> 32 -> 32 -> 2 kernels.
+// lv32_tc.cuh -- tensor-core variant of the LV 2 -> 32 -> 32 -> 2 kernels (one trajectory per thread).
 //
-// The chain's 32 x 32 layer, evaluated for the 128 trajectories of a CTA, is a [128 x 32] x [32 x 32]
-// GEMM: exactly one tcgen05.mma tile (M = 128 = one trajectory per TMEM lane / per thread, N = 32, K = 32).
+// The chain's 32 x 32 layer, evaluated for the 32 trajectories of a warp, is a [32 x 32] x [32 x 32] GEMM: 2 x 4 tiles of
+// mma.sync.m16n8k8 (M = trajectories, N = output units, K = input units) per k-step.
 // fp32 accuracy is kept with the 3xTF32 split  A_hi B_hi + A_lo B_hi + A_hi B_lo  (weights: hi = round-to-nearest
 // TF32, lo = remainder, split once per launch; activations: the tensor core reads only the upper 19 bits of a tf32
-// operand, so the value itself is the hi operand and lo = x - trunc(x)): 12 UTCHMMA instructions per layer instead of
-// 1024 FFMAs per trajectory, measured max error 3.4e-6 on |D| <= 8 (profiles/r01_tcgen05_unit_test.txt).
-//   - A (the activations) never touches shared memory: every thread writes its own row straight into
-//     tensor memory (tcgen05.st, 32x32b) and reads its row of the accumulator back with tcgen05.ld;
-//   - B (weights, hi and lo) sits in shared memory in the canonical K-major no-swizzle layout;
-//   - one elected thread issues the MMAs and commits them to an mbarrier the CTA waits on.
-// TMEM per CTA: 128 columns (accumulator 32, A_hi 32, A_lo 32, running dW2 sums of the adjoint 32) -> four CTAs share
-// an SM's 512 columns.
+// operand, so the value itself is the hi operand and lo = x - trunc(x)): 96 HMMA per warp and sweep instead of
+// 1024 FFMAs per trajectory.
+//   - every thread owns a trajectory and writes its 32-wide activation row into the warp's rows in shared memory; the
+//     warp reads A fragments from those rows, B fragments from the staged weights (row stride 36 floats: conflict-free
+//     fragment loads), and writes D back into the rows, from where each thread reads its own row again;
+//   - a sweep is warp-collective (__syncwarp only): no CTA barrier inside the time loops of the fixed-step kernels.
 // Kernels in this file: forward_kernel (fixed step), adaptive_forward_kernel (PI controller, saveat interpolation, step
 // record), adjoint_kernel<GEMM, ADAPT, DISC> (interpolating adjoint on the fixed grid / replay of an adaptive solve /
 // discrete adjoint; gradient GEMM on the FMA pipe or on mma.sync).
@@ -23,87 +21,92 @@ namespace b200ude {
 namespace lv32 {
 namespace tc {
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // round-to-nearest (ties away) to TF32's 10-bit mantissa == cvt.rna.tf32.f32, done with two integer ops on
 // the ALU pipe (the cvt instruction issues on the XU pipe, which the tanh's MUFUs already load)
 __device__ __forceinline__ float tf32_rna(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
-// K-major SWIZZLE_NONE shared-memory matrix descriptor (layout of cute::UMMA::SmemDescriptor):
-// [0,14) start>>4 | [16,30) leading byte offset>>4 | [32,46) stride byte offset>>4 | [46,48) version=1 | [61,64) layout=0
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo)
+
+// defined with the gradient GEMM of the adjoint kernel below
+__device__ __forceinline__ void mma_m16n8k8(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]);
+__device__ __forceinline__ void split_tf32(float x, uint32_t &hi, uint32_t &lo);
+
+// D = A B for the 32 rows of the calling warp (3xTF32 mma.sync.m16n8k8; M = the warp's trajectories, N = NO output units,
+// K = input units).  A: src[r * SA + k], r = 0..31.  B(k, n) = Bm[n * SB + k] (BT = false) or Bm[k * SB + n] (BT = true),
+// given as the hi / lo split made at staging.  D goes to dst[r * SA + n]; dst may alias src (every A fragment is read
+// before the first store).  Warp-collective; starts and ends with __syncwarp, so the rows may be written right before.
+template <int K, int NO, int SA, int SB, bool BT>
+__device__ __forceinline__ void warp_gemm(const float *src, float *dst, const float *Bhi, const float *Blo)
 {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) | (1ull << 46);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, both K-major
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N)
-{
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t db, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(db), "r"(idesc), "r"(accumulate), "r"(0), "r"(0), "r"(0), "r"(0)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
-{
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32])
-{
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    float d[2][NO / 8][4];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < NO / 8; ++nt)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) d[mt][nt][q] = 0.0f;
+    __syncwarp();
+#pragma unroll
+    for (int ks = 0; ks < K / 8; ++ks) {
+        uint32_t ah[2][4], al[2][4];
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+            const float *r0 = src + (16 * mt + g) * SA + 8 * ks + t, *r1 = r0 + 8 * SA;
+            split_tf32(r0[0], ah[mt][0], al[mt][0]);
+            split_tf32(r1[0], ah[mt][1], al[mt][1]);
+            split_tf32(r0[4], ah[mt][2], al[mt][2]);
+            split_tf32(r1[4], ah[mt][3], al[mt][3]);
+        }
+#pragma unroll
+        for (int nt = 0; nt < NO / 8; ++nt) {
+            const int n = 8 * nt + g, k = 8 * ks + t;
+            const int o0 = BT ? k * SB + n : n * SB + k, o1 = BT ? (k + 4) * SB + n : n * SB + k + 4;
+            const uint32_t bh[2] = {__float_as_uint(Bhi[o0]), __float_as_uint(Bhi[o1])};
+            const uint32_t bl[2] = {__float_as_uint(Blo[o0]), __float_as_uint(Blo[o1])};
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+                mma_m16n8k8(d[mt][nt], al[mt], bh);
+                mma_m16n8k8(d[mt][nt], ah[mt], bl);
+                mma_m16n8k8(d[mt][nt], ah[mt], bh);
+            }
+        }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < NO / 8; ++nt) {
+            float *o = dst + (16 * mt + g) * SA + 8 * nt + 2 * t;
+            *reinterpret_cast<float2 *>(o) = make_float2(d[mt][nt][0], d[mt][nt][1]);
+            *reinterpret_cast<float2 *>(o + 8 * SA) = make_float2(d[mt][nt][2], d[mt][nt][3]);
+        }
+    __syncwarp();
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32])
+
+template <int NV>
+__device__ __forceinline__ void store_row(float *row, const float (&v)[NV])
 {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-        "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-          "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-          "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-          "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-          "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-        : "memory");
+#pragma unroll
+    for (int j = 0; j < NV; j += 4) *reinterpret_cast<float4 *>(row + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+template <int NV>
+__device__ __forceinline__ void load_row(const float *row, float (&v)[NV])
+{
+#pragma unroll
+    for (int j = 0; j < NV; j += 4) {
+        const float4 q = *reinterpret_cast<const float4 *>(row + j);
+        v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
+    }
+}
 
-constexpr uint32_t LBO = 128, SBO = 1024;   // weights tile [n/8][k/4][n%8][k%4]: the 8 K-chunks of a row group are adjacent
-constexpr int TMEM_COLS = 128;              // D [0,32) | A_hi [32,64) | A_lo [64,96) | [96,128) running dW2 sums of the adjoint (tmem_flush32)
-constexpr uint32_t IDESC = make_idesc(128, 32);
+constexpr int SW = 36;   // row stride (floats) of the staged W2 copies and of the activation rows: conflict-free fragment loads
 
-// per-CTA tensor-core context
+// per-warp tensor-core context: the warp's 32 activation rows (row r belongs to lane r)
 struct TcCtx {
-    uint32_t tmem;      // base TMEM address of this CTA's allocation
-    uint32_t lane_base; // this warp's lane quadrant (warp*32) << 16
-    uint32_t bar;       // shared address of the MMA-completion mbarrier
-    uint32_t parity;    // phase of the next completion
+    float *rows;
 };
+__device__ __forceinline__ TcCtx tc_ctx(float *cta_rows) { return TcCtx{cta_rows + (threadIdx.x >> 5) * 32 * SW}; }
 
-// weights tile B[n][k] (K-major): element at (n/8)*SBO + (k/4)*LBO + (n%8)*16 + (k%4)*4 bytes.
+// weights Wt[n][k] = B(k, n) at n * SW + k, hi / lo split.
 // FWD orientation: n = output unit j, k = input unit i  ->  W2[j][i] = theta[OFF_W2 + i*32 + j]
 // BWD orientation: n = input unit i,  k = output unit j ->  W2[j][i]   (for q1 = W2^T q2)
 template <bool BWD>
@@ -113,87 +116,18 @@ __device__ __forceinline__ void stage_weights(const float *__restrict__ theta, f
         const int n = e >> 5, k = e & 31;
         const float x = BWD ? theta[OFF_W2 + n * 32 + k] : theta[OFF_W2 + k * 32 + n];
         const float hi = tf32_rna(x);
-        const int off = (n >> 3) * (SBO / 4) + (k >> 2) * (LBO / 4) + (n & 7) * 4 + (k & 3);
-        sBhi[off] = hi;
-        sBlo[off] = x - hi;
+        sBhi[n * SW + k] = hi;
+        sBlo[n * SW + k] = x - hi;
     }
 }
 
-// all 128 threads: write this thread's row of A (hi/lo split) into TMEM; the elected thread issues the
-// 12 MMAs (3xTF32, K = 4 x 8) and commits.  tc_collect() waits for them and reads this thread's row of D.
-// Independent work placed between the two calls overlaps the tensor core's latency.
-__device__ __forceinline__ void tc_issue(TcCtx &c, const float (&a)[32], const float *sBhi, const float *sBlo)
+// d = a W2^T (FWD weights) or a W2 (BWD weights) for this thread's row a, through the warp's rows
+__device__ __forceinline__ void gemm_row32(const TcCtx &c, const float (&a)[32], const float *sBhi, const float *sBlo, float (&d)[32])
 {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {   // 8 columns at a time keeps the hi/lo temporaries short-lived
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            // the tensor core reads the upper 19 bits of a tf32 operand: the value itself is the hi operand (see split_tf32)
-            hi[k] = __float_as_uint(a[8 * q + k]);
-            lo[k] = __float_as_uint(a[8 * q + k] - __uint_as_float(hi[k] & 0xFFFFE000u));
-        }
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(c.tmem + 32 + 8 * q + c.lane_base),
-                     "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]), "r"(hi[4]), "r"(hi[5]), "r"(hi[6]), "r"(hi[7]) : "memory");
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(c.tmem + 64 + 8 * q + c.lane_base),
-                     "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]), "r"(lo[4]), "r"(lo[5]), "r"(lo[6]), "r"(lo[7]) : "memory");
-    }
-    tmem_st_wait();
-    tc_fence_before();
-    __syncthreads();   // every row of A is in TMEM; every thread has finished reading the previous D
-    if (threadIdx.x == 0) {
-        tc_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) {
-            const uint64_t dbh = make_desc(smem_u32(sBhi) + kb * 2 * LBO, LBO, SBO);
-            const uint64_t dbl = make_desc(smem_u32(sBlo) + kb * 2 * LBO, LBO, SBO);
-            mma_ts(c.tmem, c.tmem + 32 + kb * 8, dbh, IDESC, kb > 0);
-            mma_ts(c.tmem, c.tmem + 64 + kb * 8, dbh, IDESC, 1);
-            mma_ts(c.tmem, c.tmem + 32 + kb * 8, dbl, IDESC, 1);
-        }
-        mma_commit(c.bar);
-    }
-}
-__device__ __forceinline__ void tc_collect(TcCtx &c, float (&d)[32])
-{
-    mbar_wait(c.bar, c.parity);
-    c.parity ^= 1;
-    tc_fence_after();
-    tmem_ld32(c.tmem + c.lane_base, d);
-}
-__device__ __forceinline__ void gemm128x32x32(TcCtx &c, const float (&a)[32], const float *sBhi, const float *sBlo, float (&d)[32])
-{
-    tc_issue(c, a, sBhi, sBlo);
-    tc_collect(c, d);
-}
-
-__device__ __forceinline__ TcCtx tc_setup(uint64_t *mbar, uint32_t *tmem_slot)
-{
-    const int warp = threadIdx.x >> 5;
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(mbar)) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    TcCtx c;
-    c.tmem = *tmem_slot;
-    c.lane_base = (uint32_t)(warp * 32) << 16;
-    c.bar = smem_u32(mbar);
-    c.parity = 0;
-    return c;
-}
-__device__ __forceinline__ void tc_teardown(const TcCtx &c)
-{
-    tc_fence_before();
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(c.tmem), "r"(TMEM_COLS) : "memory");
+    float *row = c.rows + (threadIdx.x & 31) * SW;
+    store_row(row, a);
+    warp_gemm<32, 32, SW, SW, false>(c.rows, c.rows, sBhi, sBlo);
+    load_row(row, d);
 }
 
 // ---- UDE right-hand side, one trajectory per thread, the 32x32 layer on the tensor core.  A real function
@@ -201,7 +135,7 @@ __device__ __forceinline__ void tc_teardown(const TcCtx &c)
 template <int TM>
 __device__ __noinline__ float2 rhs_tc(TcCtx *cp, const float *sBhi, const float *sBlo, float x0, float x1, int zsel)
 {
-    TcCtx c = *cp;
+    const TcCtx c = *cp;
     const int zb = c_zero[zsel & 7] << 2;   // opaque zero: keeps the constant-bank loads inside the caller's loops
     float h[32], a2[32];
 #pragma unroll
@@ -212,7 +146,7 @@ __device__ __noinline__ float2 rhs_tc(TcCtx *cp, const float *sBhi, const float 
         for (int k = 0; k < 4; ++k) h[j4 + k] = fmaf(w1_[k], x1, fmaf(w0_[k], x0, b_[k]));
         tanh_quad_s<TM>(h[j4], h[j4 + 1], h[j4 + 2], h[j4 + 3]);   // one reciprocal per four values (lv32_packed.cuh)
     }
-    gemm128x32x32(c, h, sBhi, sBlo, a2);
+    gemm_row32(c, h, sBhi, sBlo, a2);
     float y0 = c_theta[zb + OFF_B3], y1 = c_theta[zb + OFF_B3 + 1];
 #pragma unroll
     for (int j4 = 0; j4 < 32; j4 += 4) {
@@ -230,7 +164,6 @@ __device__ __noinline__ float2 rhs_tc(TcCtx *cp, const float *sBhi, const float 
             y1 = fmaf(w3_[2 * k + 1], v_[k], y1);
         }
     }
-    cp->parity = c.parity;
     // du1 = p1*u1 + NN1(u), du2 = -p4*u2 + NN2(u)   (scenario_1.jl:71-72)
     return make_float2(fmaf(c_consts[0], x0, y0), fmaf(-c_consts[1], x1, y1));
 }
@@ -239,13 +172,10 @@ __device__ __noinline__ float2 rhs_tc(TcCtx *cp, const float *sBhi, const float 
 template <int TM, int BLOCK, int MINB>
 __global__ void __launch_bounds__(BLOCK, MINB) forward_kernel(FwdParams p)
 {
-    static_assert(BLOCK == 128, "one TMEM lane per thread: 128 trajectories per CTA");
-    __shared__ __align__(1024) float sBhi[32 * 32], sBlo[32 * 32];
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
-    TcCtx c = tc_setup(&mbar, &tmem_slot);
+    static_assert(BLOCK % 32 == 0, "whole warps: the 32 x 32 sweeps are warp-collective");
+    __shared__ __align__(16) float sBhi[32 * SW], sBlo[32 * SW], sRows[BLOCK * SW];
+    TcCtx c = tc_ctx(sRows);
     stage_weights<false>(p.theta, sBhi, sBlo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // weights are read by the tensor core (async proxy)
     __syncthreads();
 
     const size_t N = (size_t)p.N;
@@ -313,7 +243,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) forward_kernel(FwdParams p)
         k1[0] = k1[6];
     }
     if (p.status && live) p.status[n] = ((fabsf(u0) <= 3.0e38f) && (fabsf(u1) <= 3.0e38f)) ? 0 : 1;   // false for NaN/Inf
-    tc_teardown(c);
 }
 
 // ---- adaptive forward kernel (abstol / reltol; scenario_1.jl:84-85, seir_exposure.jl:138-139 style calls) --------------
@@ -337,13 +266,10 @@ __device__ __forceinline__ void tsit5_weights_fwd(float Th, float (&bw)[7])
 template <int TM, int BLOCK, int MINB>
 __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams p, AdaptiveGrid ag)
 {
-    static_assert(BLOCK == 128, "one TMEM lane per thread: 128 trajectories per CTA");
-    __shared__ __align__(1024) float sBhi[32 * 32], sBlo[32 * 32];
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
-    TcCtx c = tc_setup(&mbar, &tmem_slot);
+    static_assert(BLOCK % 32 == 0, "whole warps: the 32 x 32 sweeps are warp-collective");
+    __shared__ __align__(16) float sBhi[32 * SW], sBlo[32 * SW], sRows[BLOCK * SW];
+    TcCtx c = tc_ctx(sRows);
     stage_weights<false>(p.theta, sBhi, sBlo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
 
     const size_t N = (size_t)p.N;
@@ -487,12 +413,11 @@ __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams
         const bool ok = (fabsf(u0) <= 3.0e38f) && (fabsf(u1) <= 3.0e38f);
         p.status[n] = bad == 2 ? 2 : ((bad || !ok) ? 1 : 0);
     }
-    tc_teardown(c);
 }
 
 // ---- adjoint kernel: one trajectory per thread, 128 per CTA; the two 32x32 sweeps of every backward stage
-// (chain forward and W2^T q2) run on the tensor core, the ensemble-summed parameter gradient stays an FFMA2
-// outer-product GEMM per warp (32 trajectories) that is executed WHILE the second sweep's MMAs are in flight. ----
+// (chain forward and W2^T q2) run on the tensor core; the ensemble-summed parameter gradient is a per-warp GEMM over
+// the warp's 32 trajectories (FFMA or mma.sync), run before the second sweep overwrites the staged q2 rows. ----
 constexpr int SLD = 36;   // staged row stride (floats): 32 + 4 -> conflict-free 128-bit row stores and tile loads
 struct __align__(16) WarpStageT {
     float B1[32 * SLD];   // h2 rows, then q2 rows, then q1 rows   [lane][j]
@@ -531,28 +456,20 @@ __device__ __forceinline__ void split_tf32(float x, uint32_t &hi, uint32_t &lo)
 #endif
 }
 
-// Running sums kept in spare tensor-memory columns (one 32-column row per thread): sum += m with ordinary round-to-nearest
-// adds, m = 0.  The tensor core adds into its accumulator with truncation, so a long mma accumulation chain drifts
-// (measured: 2.4e-5 relative on dW2 after the 2160 MMAs of a whole backward solve); short chains flushed through this
-// keep the error at the FFMA level without spending 32 more registers or any shared / global memory.
-__device__ __forceinline__ void tmem_flush32(uint32_t taddr, float (&m)[32], bool first)
+// Running sums kept in a per-thread row of shared memory (stride 33 words: conflict-free): sum += m with ordinary
+// round-to-nearest adds, m = 0.  The tensor core adds into its accumulator with truncation, so a long mma accumulation
+// chain drifts (2.4e-5 relative on dW2 after the 2160 MMAs of a whole backward solve); short chains flushed through this
+// keep the error at the FFMA level without spending 32 more registers.
+__device__ __forceinline__ void flush32(float *sum, float (&m)[32], bool first)
 {
-    float r[32];
-    if (!first) {
-        tmem_ld32(taddr, r);
 #pragma unroll
-        for (int q = 0; q < 32; ++q) r[q] += m[q];
-    } else {
-#pragma unroll
-        for (int q = 0; q < 32; ++q) r[q] = m[q];
+    for (int q = 0; q < 32; ++q) {
+        sum[q] = first ? m[q] : sum[q] + m[q];
+        m[q] = 0.0f;
     }
-    tmem_st32(taddr, r);
-    tmem_st_wait();
-#pragma unroll
-    for (int q = 0; q < 32; ++q) m[q] = 0.0f;
 }
 
-// GEMM = 0: the per-warp gradient GEMM dW2 += q2 (x) h1 on the FMA pipe (FFMA2, 8 x 4 register tile per lane);
+// GEMM = 0: the per-warp gradient GEMM dW2 += q2 (x) h1 on the FMA pipe (FFMA, 8 x 4 register tile per lane);
 // GEMM = 1: the same product as 3xTF32 warp-level mma.sync.m16n8k8 (M = j, N = i, K = the warp's 32 trajectories):
 //           fragments are read straight from the staged rows; the contraction index inside a k-step is permuted
 //           (k = tig -> t = 2 tig, k = tig + 4 -> t = 2 tig + 1) so that every fragment load is bank-conflict free.
@@ -560,15 +477,12 @@ __device__ __forceinline__ void tmem_flush32(uint32_t taddr, float (&m)[32], boo
 template <int TM, int BLOCK, int MINB, int GEMM, bool ADAPT = false, bool DISC = false>
 __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, AdaptiveGrid ag)
 {
-    static_assert(BLOCK == 128, "one TMEM lane per thread: 128 trajectories per CTA");
-    __shared__ __align__(1024) float sWf_hi[32 * 32], sWf_lo[32 * 32], sWb_hi[32 * 32], sWb_lo[32 * 32];
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
+    static_assert(BLOCK == 128, "four warps: the partial-gradient rows are laid out as blockIdx.x * 4 + warp");
+    __shared__ __align__(16) float sWf_hi[32 * SW], sWf_lo[32 * SW], sWb_hi[32 * SW], sWb_lo[32 * SW];
+    __shared__ float s_sum[GEMM == 1 ? BLOCK * 33 : 1];   // running dW2 sums of the mma.sync gradient GEMM (flush32)
     extern __shared__ __align__(16) unsigned char s_raw[];
-    TcCtx c = tc_setup(&mbar, &tmem_slot);
     stage_weights<false>(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
     stage_weights<true>(p.theta, sWb_hi, sWb_lo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -597,6 +511,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
     float loss = 0.0f;
     const int n_save = p.n_steps / p.save_every + 1;
     bool first_flush = true;
+    float *const sum_row = s_sum + (GEMM == 1 ? threadIdx.x * 33 : 0);
 
     // One evaluation of (df/du)^T g and of the theta-gradient quadrature term at state x, stage argument g:
     // sc = quadrature weight (h b_i), isc = 1 / sc (0 for a masked lane), lvm = 0/1 mask.  Returns kn = (df/du)^T g.
@@ -617,8 +532,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
             tanh_quad_s<TM>(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);
             *reinterpret_cast<float4 *>(rowB2 + j4) = make_float4(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);   // h1 row
         }
-        tc_issue(c, v, sWf_hi, sWf_lo);
-        tc_collect(c, v);    // v = W2 h1
+        warp_gemm<32, 32, SLD, SW, false>(st->B2, st->B1, sWf_hi, sWf_lo);
+        load_row(rowB1, v);  // v = W2 h1
         // h2 = tanh(. + b2) -> B1 row;  q2 = (W3^T sg) * (1 - h2^2) stays in v
 #pragma unroll
         for (int j4 = 0; j4 < 32; j4 += 4) {
@@ -647,8 +562,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
         __syncwarp();
 #pragma unroll
         for (int j4 = 0; j4 < 32; j4 += 4) *reinterpret_cast<float4 *>(rowB1 + j4) = make_float4(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);   // q2 row
-        // ---- W2^T q2 on the tensor core; the gradient GEMM of this warp runs while the MMAs are in flight ----
-        tc_issue(c, v, sWb_hi, sWb_lo);
+        // ---- gradient GEMM of this warp, then W2^T q2 on the tensor core (in place over the q2 rows) ----
         __syncwarp();
         if constexpr (GEMM == 1) {
 #pragma unroll
@@ -709,7 +623,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
                 use_row(1);
             }
         }
-        tc_collect(c, v);    // v = W2^T q2
+        warp_gemm<32, 32, SLD, SW, false>(st->B1, st->B1, sWb_hi, sWb_lo);
+        load_row(rowB1, v);  // v = W2^T q2
         // q1 = v * (1 - h1^2) (h1 re-read from this lane's own row), (df/du)^T g
         float dx0 = 0.0f, dx1 = 0.0f;
         __syncwarp();        // all lanes are done reading B2 rows in the GEMM pass before q1 overwrites B1
@@ -802,7 +717,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
             }
         }
         if (s % p.save_every == 0) loss_jump<2>(p, s / p.save_every, n, N, lam, loss);
-        if constexpr (GEMM == 1) { tmem_flush32(c.tmem + 96 + c.lane_base, macc, first_flush); first_flush = false; }   // per step: 72-MMA chains
+        if constexpr (GEMM == 1) { flush32(sum_row, macc, first_flush); first_flush = false; }   // per step: 72-MMA chains
     }
     } else {
     // ---- adaptive: replay the accepted forward steps backwards, split at the save times where the loss cotangent jumps in
@@ -896,11 +811,11 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
                 cur = ta;
                 if (isave >= 0 && fabsf(ts - ta) <= eps) { jump(isave); --isave; }
             }
-            if constexpr (GEMM == 1) { tmem_flush32(c.tmem + 96 + c.lane_base, macc, first_flush); first_flush = false; }
+            if constexpr (GEMM == 1) { flush32(sum_row, macc, first_flush); first_flush = false; }
         }
     }
     if constexpr (GEMM == 1) {
-        if (first_flush) tmem_flush32(c.tmem + 96 + c.lane_base, macc, true);   // no accepted step at all: the sums are zero
+        if (first_flush) flush32(sum_row, macc, true);   // no accepted step at all: the sums are zero
     }
     }
     if (p.grad_u0 && live) {
@@ -913,7 +828,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
     // this warp's partial gradient
     float *dst = p.partial + ((size_t)blockIdx.x * 4 + warp) * (P + 1);
     if constexpr (GEMM == 1) {
-        tmem_ld32(c.tmem + 96 + c.lane_base, macc);
+#pragma unroll
+        for (int q = 0; q < 32; ++q) macc[q] = sum_row[q];
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -944,7 +860,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
         dst[OFF_B3 + 1] = g_b31;
         dst[P] = loss;
     }
-    tc_teardown(c);
 }
 
 }  // namespace tc

@@ -1,8 +1,7 @@
 // lv32_wm.cuh -- warp-collective variant of the LV 2 -> 32 -> 32 -> 2 kernels ("one warp = 16 trajectories").
 //
-// The tcgen05 family (lv32_tc.cuh) gives every trajectory a thread and every 128 trajectories a CTA-wide tensor-memory
-// round trip per 32 x 32 sweep; its latency per right-hand-side evaluation (~3600 cycles measured) is what bounds a small
-// ensemble: 8192 trajectories (the metric's batch on 8 GPUs) take as long as 30 000.  Here a warp integrates 16 trajectories
+// The one-trajectory-per-thread family (lv32_tc.cuh) passes every 32 x 32 sweep through shared-memory rows; its latency
+// per right-hand-side evaluation is what bounds a small ensemble.  Here a warp integrates 16 trajectories
 // (G groups of 16) with the hidden units spread over its lanes, so that nothing is wider than a warp:
 //   * lane (fg, tig) = (lane >> 2, lane & 3) holds, for the two trajectories r in {fg, fg + 8} of a group, the eight
 //     hidden units f in {8 q + 2 tig, 8 q + 2 tig + 1 : q = 0..3} -- exactly the C/D fragment layout of mma.sync.m16n8k8
@@ -11,7 +10,7 @@
 //     contraction index may be permuted freely (k = tig <-> unit 2 tig, k = tig + 4 <-> unit 2 tig + 1 inside a k-step), a
 //     D fragment IS the A fragment of the next product: the chain forward, W2^T q2 of the adjoint and all element-wise
 //     work stay in registers with no layout change; W2 (hi/lo split once per CTA) is read from shared memory as B fragments;
-//   * the thin layers are FFMA2 partial sums over the lane's 8 units + a 3-shuffle reduce-scatter over the 4 lanes of a quad,
+//   * the thin layers are FFMA partial sums over the lane's 8 units + a 3-shuffle reduce-scatter over the 4 lanes of a quad,
 //     which leaves every lane with the ONE (trajectory, component) pair it owns: the Runge-Kutta state, the stage
 //     derivatives and the adjoint state are kept once per (trajectory, component), not once per lane;
 //   * tanh = 1 - 2 / (1 + 2^(2 log2(e) x)) with ONE reciprocal per four values (Montgomery's batched inversion: the MUFU
@@ -19,7 +18,7 @@
 //   * adjoint: the ensemble-summed dW2 += q2^T h1 (K = the group's 16 trajectories) is a third 3xTF32 mma.sync product whose
 //     operands are transposed through a per-warp shared-memory tile; thin-layer gradients are per-lane register sums reduced
 //     once at the end of the kernel.
-// No tensor memory and no CTA-wide barrier inside the time loops; theta is bulk-copied by the TMA from the handle's device copy
+// No CTA-wide barrier inside the time loops; theta is bulk-copied by the TMA from the handle's device copy
 // into shared memory once per CTA (no constant bank: handles are independent, any number can be in flight on a device).
 //
 // Reference semantics replaced: RHS scenario_1.jl:69-76; Tsit5 perform_step! and InterpolatingAdjoint as in

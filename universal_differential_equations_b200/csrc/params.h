@@ -48,14 +48,14 @@ struct Variant {
     int fwd_T = 1;       // trajectories per thread in the forward kernel
     int adj_smem = 0;
     int approx_tanh = 0;
-    int fwd_tc = 0;      // 1: tcgen05 (3xTF32) forward kernel
-    int adj_tc = 0;      // 1: tcgen05 (3xTF32) adjoint kernel, FFMA2 gradient GEMM; 2: mma.sync gradient GEMM
+    int fwd_tc = 0;      // 1: tensor-core (3xTF32 mma.sync) forward kernel
+    int adj_tc = 0;      // 1: tensor-core (3xTF32 mma.sync) adjoint kernel, FFMA gradient GEMM; 2: mma.sync gradient GEMM
     int discrete = 0;    // 1: discrete adjoint (exact gradient of the fixed-step scheme) instead of the interpolating adjoint
     int fwd_wm = 0;      // 1: warp-collective mma.sync forward kernel (lv32_wm.cuh)
     int adj_wm = 0;      // 1: warp-collective mma.sync adjoint kernel
     int wm_groups = 1;   // groups per warp in the warp-collective forward kernel (1 or 2)
     int wm_rows = 0;     // trajectories per group / 8: 1, 2, or 0 = by ensemble size (<= wm_r1_max -> 1)
-    int wm_r1_max = 4736;   // 8 trajectories per warp while that still leaves one warp per scheduler (148 x 4 x 8)
+    int wm_r1_max = 0;      // 8 trajectories per warp while that still leaves one warp per scheduler (SMs x 4 x 8; b200ude_create)
 };
 
 // function attributes (dynamic shared-memory size) are per device: one-time flags are kept per device ordinal

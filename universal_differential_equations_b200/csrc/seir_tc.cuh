@@ -1,16 +1,14 @@
 // seir_tc.cuh -- tensor-core kernels of the SEIR exposure UDE (SEIR_exposure/seir_exposure.jl:114-130):
 // 7 states (S, E, I, R, N, D, C), chain 3 -> 64 -> 64 -> 1 (tanh, tanh, linear) on [S/N, I, D/N], P = 4481.
 //
-// Same building block as lv32_tc.cuh, one size up: the 64 x 64 layer of the 128 trajectories of a GROUP is a
-// [128 x 64] x [64 x 64] tcgen05 GEMM with the 3xTF32 split (24 UTCHMMA of N = 64), activations written to / read
-// from tensor memory by the thread that owns the trajectory.  A CTA holds TWO independent groups (256 threads)
-// that share the 64 KB of staged weights (W2 hi/lo in both orientations); each group has its own TMEM columns
-// (accumulator 64 + A_hi 64 + A_lo 64), mbarrier, named barrier and staging buffers.  One CTA per SM
-// (204 KB shared memory, all 512 TMEM columns).
+// Same building block as lv32_tc.cuh, one size up: the 64 x 64 layer of the 32 trajectories of a warp is a
+// [32 x 64] x [64 x 64] GEMM of 3xTF32 mma.sync.m16n8k8 tiles (384 HMMA per warp and sweep), activations passed through
+// the warp's rows in shared memory by the thread that owns the trajectory.  A CTA holds TWO independent groups of 128
+// trajectories (256 threads) that share one staged copy of W2 (hi/lo; the transposed product reads it transposed); each
+// group has its own named barrier and staging buffers.  One CTA per SM (up to 209 KB of shared memory).
 // Adjoint: the two sweeps (chain forward, W2^T q2) on the tensor core; the ensemble-summed dW2 += q2 (x) h1
-// (64 x 64 outputs, K = the group's 128 trajectories) is an FFMA2 outer-product GEMM over conflict-free 128-bit
-// shared-memory rows with an 8 x 4 register tile per thread, run while the second sweep's MMAs are in flight;
-// the thin layers are thread-owned column sums.  Deterministic: per-group partials, fixed-order final reduce.
+// (64 x 64 outputs, K = the group's 128 trajectories) is a 3xTF32 mma.sync GEMM (or FFMA 8 x 4 register tiles) over the
+// staged rows; the thin layers are thread-owned column sums.  Deterministic: per-group partials, fixed-order final reduce.
 #pragma once
 #include "vern7.cuh"
 #include "lv32_tc.cuh"
@@ -21,7 +19,7 @@ namespace seir {
 using lv32::ldw4;
 using lv32::bc;
 using lv32::fma2;
-using namespace lv32::tc;   // low-level tcgen05 helpers (mma_ts, make_desc, tf32_rna, mbar_wait, fences, ...)
+using namespace lv32::tc;   // tensor-core helpers (warp_gemm, split_tf32, tf32_rna, row load / store)
 
 constexpr int D = 7, DIN = 3, HS = 64;
 constexpr int OFF_W1 = 0;               // W1[j, m] at m*64 + j
@@ -32,107 +30,37 @@ constexpr int OFF_W3 = OFF_B2 + HS;     // 4416, W3[0, j] at j
 constexpr int OFF_B3 = OFF_W3 + HS;     // 4480
 constexpr int PS = OFF_B3 + 1;          // 4481
 
-constexpr uint32_t LBO64 = 128, SBO64 = (HS / 4) * 128;   // weights tile [n/8][k/4][n%8][k%4], 16 K-chunks per row group
-constexpr uint32_t IDESC64 = make_idesc(128, HS);
+constexpr int SWS = HS + 4;   // row stride (floats) of the staged W2: conflict-free B fragments of the forward product
+constexpr int SLD64 = 68;     // staged activation row stride (floats): 64 + 4
 constexpr int GROUP = 128, GROUPS = 2, BLOCK = GROUP * GROUPS;
-constexpr int TMEM_PER_GROUP = 3 * HS;   // D | A_hi | A_lo
-constexpr int TMEM_ALLOC = 512;
 
-template <bool BWD>
+// W2[j][i] (theta[OFF_W2 + i*64 + j]) at j * SWS + i, hi / lo split: B(k = i, n = j) of the forward product h1 W2^T and,
+// read transposed, B(k = j, n = i) of q2 W2
 __device__ __forceinline__ void stage_weights64(const float *__restrict__ theta, float *sBhi, float *sBlo, int tid, int nthreads)
 {
     for (int e = tid; e < HS * HS; e += nthreads) {
-        const int n = e >> 6, k = e & 63;
-        const float x = BWD ? theta[OFF_W2 + n * HS + k] : theta[OFF_W2 + k * HS + n];
+        const int j = e >> 6, i = e & 63;
+        const float x = theta[OFF_W2 + i * HS + j];
         const float hi = tf32_rna(x);
-        const int off = (n >> 3) * (SBO64 / 4) + (k >> 2) * (LBO64 / 4) + (n & 7) * 4 + (k & 3);
-        sBhi[off] = hi;
-        sBlo[off] = x - hi;
+        sBhi[j * SWS + i] = hi;
+        sBlo[j * SWS + i] = x - hi;
     }
 }
 
 struct GrpCtx {
-    uint32_t tmem;       // this group's first TMEM column
-    uint32_t lane_base;  // (warp % 4) * 32 << 16
-    uint32_t bar;        // mbarrier of this group
-    uint32_t parity;
-    int bar_id;          // named barrier of this group (1 + group)
+    float *rows;   // this warp's 32 activation rows (row r belongs to lane r)
+    int bar_id;    // named barrier of this group (1 + group)
 };
 __device__ __forceinline__ void group_sync(int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(GROUP) : "memory"); }
+__device__ __forceinline__ GrpCtx group_ctx(float *cta_rows) { return GrpCtx{cta_rows + (threadIdx.x >> 5) * 32 * SLD64, 1 + (int)(threadIdx.x / GROUP)}; }
 
-// write this thread's 64-wide row (hi/lo split) into TMEM, group barrier, elected thread issues 24 MMAs + commit
-__device__ __forceinline__ void tc_issue64(GrpCtx &c, const float (&a)[HS], const float *sBhi, const float *sBlo, bool issuer)
+// d = a W2^T for this thread's 64-wide row a, through the warp's rows
+__device__ __forceinline__ void gemm_row64(const GrpCtx &c, const float (&a)[HS], const float *sBhi, const float *sBlo, float (&d)[HS])
 {
-#pragma unroll
-    for (int q = 0; q < HS / 8; ++q) {
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            // the tensor core reads the upper 19 bits of a tf32 operand: the value itself is the hi operand (see split_tf32)
-            hi[k] = __float_as_uint(a[8 * q + k]);
-            lo[k] = __float_as_uint(a[8 * q + k] - __uint_as_float(hi[k] & 0xFFFFE000u));
-        }
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(c.tmem + HS + 8 * q + c.lane_base),
-                     "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]), "r"(hi[4]), "r"(hi[5]), "r"(hi[6]), "r"(hi[7]) : "memory");
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(c.tmem + 2 * HS + 8 * q + c.lane_base),
-                     "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]), "r"(lo[4]), "r"(lo[5]), "r"(lo[6]), "r"(lo[7]) : "memory");
-    }
-    tmem_st_wait();
-    tc_fence_before();
-    group_sync(c.bar_id);
-    if (issuer) {
-        tc_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < HS / 8; ++kb) {
-            const uint64_t dbh = make_desc(smem_u32(sBhi) + kb * 2 * LBO64, LBO64, SBO64);
-            const uint64_t dbl = make_desc(smem_u32(sBlo) + kb * 2 * LBO64, LBO64, SBO64);
-            mma_ts(c.tmem, c.tmem + HS + kb * 8, dbh, IDESC64, kb > 0);
-            mma_ts(c.tmem, c.tmem + 2 * HS + kb * 8, dbh, IDESC64, 1);
-            mma_ts(c.tmem, c.tmem + HS + kb * 8, dbl, IDESC64, 1);
-        }
-        mma_commit(c.bar);
-    }
-}
-__device__ __forceinline__ void tc_collect64(GrpCtx &c, float (&d)[HS])
-{
-    mbar_wait(c.bar, c.parity);
-    c.parity ^= 1;
-    tc_fence_after();
-    float lo[32], hi[32];
-    tmem_ld32(c.tmem + c.lane_base, lo);
-    tmem_ld32(c.tmem + 32 + c.lane_base, hi);
-#pragma unroll
-    for (int k = 0; k < 32; ++k) { d[k] = lo[k]; d[32 + k] = hi[k]; }
-}
-
-__device__ __forceinline__ GrpCtx cta_setup(uint64_t *mbars, uint32_t *tmem_slot)
-{
-    const int warp = threadIdx.x >> 5, group = threadIdx.x / GROUP;
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_ALLOC) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (threadIdx.x == 0) {
-        for (int g = 0; g < GROUPS; ++g) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&mbars[g])) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    GrpCtx c;
-    c.tmem = *tmem_slot + group * TMEM_PER_GROUP;
-    c.lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    c.bar = smem_u32(&mbars[group]);
-    c.parity = 0;
-    c.bar_id = 1 + group;
-    return c;
-}
-__device__ __forceinline__ void cta_teardown(uint32_t tmem_base)
-{
-    tc_fence_before();
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_ALLOC) : "memory");
+    float *row = c.rows + (threadIdx.x & 31) * SLD64;
+    store_row(row, a);
+    warp_gemm<HS, HS, SLD64, SWS, false>(c.rows, c.rows, sBhi, sBlo);
+    load_row(row, d);
 }
 
 struct State7 {
@@ -150,9 +78,9 @@ __device__ __forceinline__ void seir_inputs(const float (&u)[D], float (&x)[3])
 
 // ---- UDE right-hand side (seir_exposure.jl:117-130), the 64 x 64 layer on the tensor core ----
 template <int TM>
-__device__ __noinline__ State7 rhs_seir(GrpCtx *cp, const float *sWhi, const float *sWlo, State7 us, int zsel, bool issuer)
+__device__ __noinline__ State7 rhs_seir(const GrpCtx *cp, const float *sWhi, const float *sWlo, State7 us, int zsel)
 {
-    GrpCtx c = *cp;
+    const GrpCtx c = *cp;
     const int zb = lv32::c_zero[zsel & 7] << 2;
     float x[3];
     seir_inputs(us.v, x);
@@ -165,8 +93,7 @@ __device__ __noinline__ State7 rhs_seir(GrpCtx *cp, const float *sWhi, const flo
         for (int k = 0; k < 4; ++k) h[j4 + k] = fmaf(w2_[k], x[2], fmaf(w1_[k], x[1], fmaf(w0_[k], x[0], b_[k])));
         lv32::tanh_quad_s<TM>(h[j4], h[j4 + 1], h[j4 + 2], h[j4 + 3]);   // one reciprocal per four values (lv32_packed.cuh)
     }
-    tc_issue64(c, h, sWhi, sWlo, issuer);
-    tc_collect64(c, h);
+    gemm_row64(c, h, sWhi, sWlo, h);
     float z = c_theta[zb + OFF_B3];
 #pragma unroll
     for (int j4 = 0; j4 < HS; j4 += 4) {
@@ -179,7 +106,6 @@ __device__ __noinline__ State7 rhs_seir(GrpCtx *cp, const float *sWhi, const flo
 #pragma unroll
         for (int k = 0; k < 4; ++k) z = fmaf(w3_[k], t_[k], z);
     }
-    cp->parity = c.parity;
     // consts = F, beta0, alpha, kappa, mu, sigma, gamma, d, lambda (seir_exposure.jl:33)
     const float F = c_consts[0], b0 = c_consts[1], mu = c_consts[4], sg = c_consts[5], gm = c_consts[6], dd = c_consts[7], lm = c_consts[8];
     const float S = us.v[0], E = us.v[1], I = us.v[2], R = us.v[3], N = us.v[4], Dd = us.v[5];
@@ -199,17 +125,12 @@ __device__ __noinline__ State7 rhs_seir(GrpCtx *cp, const float *sWhi, const flo
 template <int TM>
 __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(FwdParams p)
 {
-    extern __shared__ __align__(1024) float s_dyn[];
-    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * HS;
-    __shared__ __align__(8) uint64_t mbars[GROUPS];
-    __shared__ uint32_t tmem_slot;
-    GrpCtx c = cta_setup(mbars, &tmem_slot);
-    const uint32_t tmem_base = tmem_slot;
-    stage_weights64<false>(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    extern __shared__ __align__(16) float s_dyn[];
+    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * SWS;
+    const GrpCtx c = group_ctx(s_dyn + 2 * HS * SWS);
+    stage_weights64(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
     __syncthreads();
 
-    const bool issuer = (threadIdx.x % GROUP) == 0;
     const size_t N = (size_t)p.N;
     const int gid = blockIdx.x * BLOCK + threadIdx.x;
     const bool live = gid < p.N;
@@ -259,7 +180,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(FwdParams p)
 #pragma unroll
             for (int cc = 0; cc < D; ++cc) g.v[cc] = fmaf(dt, g.v[cc], u.v[cc]);
             if (i == 6) u = g;   // stage 7's argument is u_{n+1} (row 7 = b, FSAL)
-            const State7 kk = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, i, issuer);
+            const State7 kk = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, i);
             switch (i) {
             case 0: k[0] = kk; break;
             case 1: k[1] = kk; break;
@@ -284,7 +205,6 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(FwdParams p)
         for (int cc = 0; cc < D; ++cc) ok = ok && (fabsf(u.v[cc]) <= 3.0e38f);
         p.status[n] = ok ? 0 : 1;
     }
-    cta_teardown(tmem_base);
 }
 
 // ---- Vern7 forward kernel (fixed step): the reference's solver for this model (seir_exposure.jl:138, Vern7()), 9 stages per step
@@ -294,17 +214,12 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(FwdParams p)
 template <int TM>
 __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
 {
-    extern __shared__ __align__(1024) float s_dyn[];
-    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * HS;
-    __shared__ __align__(8) uint64_t mbars[GROUPS];
-    __shared__ uint32_t tmem_slot;
-    GrpCtx c = cta_setup(mbars, &tmem_slot);
-    const uint32_t tmem_base = tmem_slot;
-    stage_weights64<false>(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    extern __shared__ __align__(16) float s_dyn[];
+    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * SWS;
+    const GrpCtx c = group_ctx(s_dyn + 2 * HS * SWS);
+    stage_weights64(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
     __syncthreads();
 
-    const bool issuer = (threadIdx.x % GROUP) == 0;
     const size_t N = (size_t)p.N;
     const int gid = blockIdx.x * BLOCK + threadIdx.x;
     const bool live = gid < p.N;
@@ -335,7 +250,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
                     if (Vern7::a(i, j) != 0.0) a = fmaf((float)Vern7::a(i, j), k[j].v[cc], a);
                 g.v[cc] = fmaf(dt, a, u.v[cc]);
             }
-            k[i] = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, i, issuer);
+            k[i] = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, i);
         }
 #pragma unroll
         for (int cc = 0; cc < D; ++cc) {
@@ -356,7 +271,6 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
         for (int cc = 0; cc < D; ++cc) ok = ok && (fabsf(u.v[cc]) <= 3.0e38f);
         p.status[n] = ok ? 0 : 1;
     }
-    cta_teardown(tmem_base);
 }
 
 // ---- adaptive forward kernel (abstol / reltol): Tsit5 + OrdinaryDiffEq's PI controller per trajectory, saveat by the free
@@ -364,17 +278,12 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
 template <int TM>
 __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p, AdaptiveGrid ag)
 {
-    extern __shared__ __align__(1024) float s_dyn[];
-    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * HS;
-    __shared__ __align__(8) uint64_t mbars[GROUPS];
-    __shared__ uint32_t tmem_slot;
-    GrpCtx c = cta_setup(mbars, &tmem_slot);
-    const uint32_t tmem_base = tmem_slot;
-    stage_weights64<false>(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    extern __shared__ __align__(16) float s_dyn[];
+    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * SWS;
+    const GrpCtx c = group_ctx(s_dyn + 2 * HS * SWS);
+    stage_weights64(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
     __syncthreads();
 
-    const bool issuer = (threadIdx.x % GROUP) == 0;
     const size_t N = (size_t)p.N;
     const int gid = blockIdx.x * BLOCK + threadIdx.x;
     const bool live = gid < p.N;
@@ -399,7 +308,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
     for (int j = 0; j < 7; ++j)
 #pragma unroll
         for (int cc = 0; cc < D; ++cc) k[j].v[cc] = 0.0f;
-    k[0] = rhs_seir<TM>(&c, sWf_hi, sWf_lo, u, 0, issuer);
+    k[0] = rhs_seir<TM>(&c, sWf_hi, sWf_lo, u, 0);
     store(p.dense, 0, k[0]);
     float dt;
     {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
@@ -416,7 +325,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
         State7 g;
 #pragma unroll
         for (int cc = 0; cc < D; ++cc) g.v[cc] = fmaf(dt0, k[0].v[cc], u.v[cc]);
-        const State7 f1 = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, 1, issuer);
+        const State7 f1 = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, 1);
 #pragma unroll
         for (int cc = 0; cc < D; ++cc) {
             const float sk = abstol + reltol * fabsf(u.v[cc]);
@@ -464,7 +373,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
 #pragma unroll
             for (int cc = 0; cc < D; ++cc) g.v[cc] = fmaf(h, g.v[cc], u.v[cc]);
             if (i == 6) un = g;
-            const State7 kk = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, i, issuer);
+            const State7 kk = rhs_seir<TM>(&c, sWf_hi, sWf_lo, g, i);
             switch (i) {
             case 1: k[1] = kk; break;
             case 2: k[2] = kk; break;
@@ -543,11 +452,9 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
         for (int cc = 0; cc < D; ++cc) ok = ok && (fabsf(u.v[cc]) <= 3.0e38f);
         p.status[n] = bad == 2 ? 2 : ((bad || !ok) ? 1 : 0);
     }
-    cta_teardown(tmem_base);
 }
 
 // ---- adjoint kernel --------------------------------------------------------------------------------------
-constexpr int SLD64 = 68;   // staged row stride (floats): 64 + 4
 struct __align__(16) GroupStage {
     float B1[GROUP * SLD64];   // h2 rows, then q2 rows, then q1 rows   [trajectory][j]
     float B2[GROUP * SLD64];   // h1 rows                                [trajectory][i]
@@ -558,25 +465,19 @@ struct __align__(16) GroupStage {
 
 // GEMM = 1: the group's gradient GEMM dW2 += q2 (x) h1 (64 x 64 outputs, K = 128 trajectories) as 3xTF32 warp-level
 // mma.sync.m16n8k8 -- warp w of the group owns the 16 rows j = 16 w .. 16 w + 15 and all 8 column tiles; fragments are read
-// from the staged rows with the bank-conflict-free k permutation of lv32_tc.cuh.  GEMM = 0: FFMA2 8 x 4 register tiles.
+// from the staged rows with the bank-conflict-free k permutation of lv32_tc.cuh.  GEMM = 0: FFMA 8 x 4 register tiles.
 template <int TM, int GEMM, bool ADAPT = false>
 __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, AdaptiveGrid ag)
 {
-    extern __shared__ __align__(1024) float s_dyn[];
-    float *sWf_hi = s_dyn, *sWf_lo = s_dyn + HS * HS, *sWb_hi = s_dyn + 2 * HS * HS, *sWb_lo = s_dyn + 3 * HS * HS;
-    __shared__ __align__(8) uint64_t mbars[GROUPS];
-    __shared__ uint32_t tmem_slot;
-    GrpCtx c = cta_setup(mbars, &tmem_slot);
-    const uint32_t tmem_base = tmem_slot;
-    stage_weights64<false>(p.theta, sWf_hi, sWf_lo, threadIdx.x, BLOCK);
-    stage_weights64<true>(p.theta, sWb_hi, sWb_lo, threadIdx.x, BLOCK);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    extern __shared__ __align__(16) float s_dyn[];
+    float *sW_hi = s_dyn, *sW_lo = s_dyn + HS * SWS;
+    stage_weights64(p.theta, sW_hi, sW_lo, threadIdx.x, BLOCK);
     __syncthreads();
 
     const int group = threadIdx.x / GROUP, tg = threadIdx.x % GROUP;
-    const bool issuer = tg == 0;
-    GroupStage *st = reinterpret_cast<GroupStage *>(s_dyn + 4 * HS * HS) + group;
+    GroupStage *st = reinterpret_cast<GroupStage *>(s_dyn + 2 * HS * SWS) + group;
     float *const rowB1 = st->B1 + tg * SLD64, *const rowB2 = st->B2 + tg * SLD64;
+    const GrpCtx c{st->B1 + (tg & ~31) * SLD64, 1 + group};   // this warp's q2 / q1 rows, the group's barrier
     const int jt = tg >> 4, it = tg & 15;        // dW2 tile: j = jt*8 + jj, i = it*4 + {0,1},{2,3}
     const size_t N = (size_t)p.N;
     const int gid = blockIdx.x * BLOCK + threadIdx.x;
@@ -592,7 +493,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
     float macc[32];   // GEMM = 1: C fragments of this warp's 8 column tiles, tile nt at 4 nt
 #pragma unroll
     for (int q = 0; q < 32; ++q) macc[q] = 0.0f;
-    const uint32_t sum_taddr = tmem_base + GROUPS * TMEM_PER_GROUP + 32 * group + c.lane_base;   // spare columns [384, 448)
+    float *const sum_row = reinterpret_cast<float *>(reinterpret_cast<GroupStage *>(s_dyn + 2 * HS * SWS) + GROUPS) + threadIdx.x * 33;   // running dW2 sums
     const int lane = threadIdx.x & 31, fg = lane >> 2, tig = lane & 3, wg = tg >> 5;
     // thin layers: thread tg owns column j = tg % 64 over the staged rows [64 * (tg / 64), +64) of its group:
     // a_w3 (dW3[j]), a_b2 (db2[j]), a_b3 (db3), a_w1[m] (dW1[j][m]), a_b1 (db1[j]); the two halves are added at the end
@@ -628,8 +529,8 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
             lv32::tanh_quad_s<TM>(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);
             *reinterpret_cast<float4 *>(rowB2 + j4) = make_float4(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);   // h1 row
         }
-        tc_issue64(c, v, sWf_hi, sWf_lo, issuer);
-        tc_collect64(c, v);   // v = W2 h1
+        warp_gemm<HS, HS, SLD64, SWS, false>(st->B2 + (tg & ~31) * SLD64, c.rows, sW_hi, sW_lo);
+        load_row(rowB1, v);   // v = W2 h1
         // h2 = tanh(. + b2) -> B1 row;  q2 = W3 * sg * (1 - h2^2) stays in v
 #pragma unroll
         for (int j4 = 0; j4 < HS; j4 += 4) {
@@ -654,8 +555,8 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
         group_sync(c.bar_id);
 #pragma unroll
         for (int j4 = 0; j4 < HS; j4 += 4) *reinterpret_cast<float4 *>(rowB1 + j4) = make_float4(v[j4], v[j4 + 1], v[j4 + 2], v[j4 + 3]);   // q2 row
-        // ---- W2^T q2 on the tensor core; gradient GEMM of the group while the MMAs are in flight ----
-        tc_issue64(c, v, sWb_hi, sWb_lo, issuer);
+        // ---- gradient GEMM of the group, then W2^T q2 on the tensor core (in place over the q2 rows) ----
+        group_sync(c.bar_id);
         if constexpr (GEMM == 1) {
 #pragma unroll 1
             for (int ks = 0; ks < GROUP / 8; ++ks) {
@@ -683,7 +584,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
                     }
                 }
             }
-            lv32::tc::tmem_flush32(sum_taddr, macc, first_flush); first_flush = false;   // per evaluation: 48-MMA chains
+            lv32::tc::flush32(sum_row, macc, first_flush); first_flush = false;   // per evaluation: 48-MMA chains
 #pragma unroll 8
             for (int t = tlo; t < tlo + 64; ++t) a_b2 += st->B1[t * SLD64 + jc];   // db2[j] += sum_t q2[t][j]
         } else {
@@ -714,8 +615,9 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
 #pragma unroll 8
             for (int t = tlo; t < tlo + 64; ++t) a_b2 += st->B1[t * SLD64 + jc];   // db2[j] += sum_t q2[t][j]
         }
-        tc_collect64(c, v);   // v = W2^T q2
         group_sync(c.bar_id);  // everyone is done reading q2 / h1 rows
+        warp_gemm<HS, HS, SLD64, SWS, true>(c.rows, c.rows, sW_hi, sW_lo);
+        load_row(rowB1, v);   // v = W2^T q2
         float dx0 = 0.0f, dx1 = 0.0f, dx2 = 0.0f;
 #pragma unroll
         for (int j4 = 0; j4 < HS; j4 += 4) {
@@ -895,7 +797,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
         }
     }
     if constexpr (GEMM == 1) {
-        if (first_flush) lv32::tc::tmem_flush32(sum_taddr, macc, true);   // no accepted step at all: the sums are zero
+        if (first_flush) lv32::tc::flush32(sum_row, macc, true);   // no accepted step at all: the sums are zero
     }
     }
 #undef B200UDE_SEIR_SETKL_ALL
@@ -913,7 +815,8 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
     group_sync(c.bar_id);
     float *dst = p.partial + ((size_t)blockIdx.x * GROUPS + group) * (PS + 1);
     if constexpr (GEMM == 1) {
-        lv32::tc::tmem_ld32(sum_taddr, macc);
+#pragma unroll
+        for (int q = 0; q < 32; ++q) macc[q] = sum_row[q];
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) {
             const int j = 16 * wg + fg, i = 8 * nt + 2 * tig;
@@ -946,7 +849,6 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
             dst[PS] = ls;
         }
     }
-    cta_teardown(tmem_base);
 }
 
 }  // namespace seir

@@ -1,4 +1,4 @@
-// ude_adjoint.cuh -- InterpolatingAdjoint backward solve as one fused sm_100a kernel per launch.
+// ude_adjoint.cuh -- InterpolatingAdjoint backward solve as one fused sm_90a kernel per launch.
 //
 // Replaces, for the whole ensemble at once, what DiffEqSensitivity does for
 //   concrete_solve(...; sensealg = InterpolatingAdjoint(autojacvec = ReverseDiffVJP()))

@@ -1,4 +1,4 @@
-// ude_common.cuh -- shared pieces of the sm_100a kernels of the UDE hot path (+ the forward kernel).
+// ude_common.cuh -- shared pieces of the sm_90a kernels of the UDE hot path (+ the forward kernel).
 //
 //   ude_forward_kernel : whole fixed-step Tsit5 solve of an ensemble in ONE launch.  One thread
 //                        integrates T trajectories: state and stage derivatives live in registers,
@@ -41,7 +41,7 @@ static __constant__ float c_lossw[16];
 static __constant__ int c_acts[8];
 
 // weight sources ---------------------------------------------------------------------------------
-struct WConst {  // constant bank: sm_100a reads it through LDCU.128 into uniform registers (4 weights per load)
+struct WConst {  // constant bank: warp-uniform weights, 4 per 128-bit load
     __device__ __forceinline__ float operator()(int i) const { return c_theta[i]; }
 };
 struct WSmem {  // shared-memory copy (bulk-copied once per CTA); compile-time offsets -> LDS[.128]

@@ -6,7 +6,7 @@
 // on the fixed grid and the replay of an adaptive solve -- in fp64: one trajectory per thread, runtime chain shape (widths
 // <= 64, <= 5 layers), models LV (0/1/2 trainable rates), SEIR, SEIR_NODE, NODE.  theta is read from the handle's device
 // copy (global memory, L1-resident), the shape / constants from one small __constant__ struct.  Reference precision, not
-// throughput: B200's fp64 rate is half its fp32 rate and these are the untuned one-thread-per-trajectory kernels.
+// throughput: H100's fp64 rate is half its fp32 rate and these are the untuned one-thread-per-trajectory kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

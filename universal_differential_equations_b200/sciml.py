@@ -15,7 +15,7 @@ surface in Python with the same names, argument meaning and error behaviour, on 
 of the C-ABI library (the Julia `ccall` shim a maintainer would add is in
 INTEGRATION.md).  torch is used only for device memory, streams and autograd
 plumbing (the pullback of `concrete_solve` calls the adjoint kernel, the way Zygote
-calls DiffEqSensitivity's rule); every number is produced by the sm_100a kernels.
+calls DiffEqSensitivity's rule); every number is produced by the sm_90a kernels.
 
 Arbitrary closures cannot cross a C ABI: the right-hand side must be one of the UDE
 forms the library recognises (`LotkaVolterraUDE` ...), built from a dense chain.
@@ -312,7 +312,7 @@ class UDESolver:
         if not isinstance(sensealg, (InterpolatingAdjoint, ForwardDiffSensitivity)):
             raise TypeError(f"unsupported sensealg {sensealg!r}")
         if not torch.cuda.is_available():
-            raise RuntimeError("b200ude needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("b200ude needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else torch.device(device).index or 0)
         self.f = f
         self.n_steps, self.save_every, self.dt, self.t0 = int(n_steps), int(save_every), float(dt), float(t0)
