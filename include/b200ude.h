@@ -55,8 +55,8 @@ extern "C" {
 #define B200UDE_F32 0
 #define B200UDE_F64 1 /* double precision: EVERY device array of the calls (theta, u0, out, data, dL_dout, grad_theta, grad_u0, loss) is
                         * double.  Runtime-shape kernels for the LV / SEIR / NODE forms, Tsit5 and Vern7, fixed step and adaptive,
-                        * interpolating adjoint -- the precision the reference's scenario 1 / 2 and SEIR scripts run in (Float64,
-                        * abstol = reltol = 1e-6).  Entry points: create / set_params / get_params / forward / adjoint / adjoint_l2;
+                        * and for the Fisher-KPP UPDE with adaptive Tsit5 (fixed-step Fisher-KPP is fp32 only); interpolating
+                        * adjoint -- the precision the reference's scenario 1 / 2, SEIR and Fisher-KPP scripts run in (Float64).  Entry points: create / set_params / get_params / forward / adjoint / adjoint_l2;
                         * the host-buffer, ADAM and peer entry points return B200UDE_EUNSUPPORTED for such handles. */
 
 /* model kinds: the UDE right-hand sides of the reference */
@@ -139,7 +139,9 @@ typedef struct b200ude_desc {
     uint64_t max_trajectories; /* capacity: scratch is sized for this many trajectories */
     uint32_t flags;
     int32_t adaptive;   /* 0: fixed step dt (adaptive = false). 1: Tsit5 with OrdinaryDiffEq's PI controller, abstol / reltol;
-                           saveat = t0 + i*save_every*dt, i = 0..n_steps/save_every (dt only defines the save grid) */
+                           saveat = t0 + i*save_every*dt, i = 0..n_steps/save_every (dt only defines the save grid).
+                           LV / SEIR / NODE forms (Tsit5 or Vern7) and the Fisher-KPP UPDE (Tsit5; its error norm is taken over the
+                           whole grid, as OrdinaryDiffEq's default norm over the state vector), fp32 and fp64 */
     int32_t max_steps;  /* adaptive: capacity of ACCEPTED steps per trajectory (status 2 when exceeded) */
     int32_t n_stages;   /* B200UDE_RKC2: stages per step (2..64); choose dt * spectral_radius <= 0.65 n_stages^2.  0 otherwise */
 } b200ude_desc;

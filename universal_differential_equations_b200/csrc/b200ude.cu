@@ -230,7 +230,8 @@ int32_t tsit5_forward(b200ude_handle *h, const float *u0, size_t N, float *out, 
     cudaError_t e = cudaSuccess;
     if (h->adaptive) {
         e = h->kid == K_LV32 ? launch_fwd_lv32_adaptive(h->var, h->tab, p, h->ag, st)
-            : h->kid == K_SEIR64 ? launch_fwd_seir_adaptive(h->var, h->tab, p, h->ag, st) : launch_fwd_adaptive(h->gen, h->tab, p, h->ag, st);
+            : h->kid == K_SEIR64 ? launch_fwd_seir_adaptive(h->var, h->tab, p, h->ag, st)
+            : h->kid == K_FKPP ? launch_fwd_fkpp_adaptive(h->gen, h->tab, p, h->ag, st) : launch_fwd_adaptive(h->gen, h->tab, p, h->ag, st);
         CUDA_TRY(h, e);
         h->last_out = out;
         return B200UDE_OK;
@@ -327,6 +328,7 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
         }
         if (h->kid == K_LV32) CUDA_TRY(h, launch_adj_lv32_adaptive(h->var, h->tab, p, h->ag, st, &grid));
         else if (h->kid == K_SEIR64) CUDA_TRY(h, launch_adj_seir_adaptive(h->var, h->tab, p, h->ag, st, &grid));
+        else if (h->kid == K_FKPP) CUDA_TRY(h, launch_adj_fkpp_adaptive(h->gen, h->tab, p, h->ag, st, &grid));
         else CUDA_TRY(h, launch_adj_adaptive(h->gen, h->tab, p, h->ag, st, &grid));
         CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
         if (l2 && loss) CUDA_TRY(h, launch_l2_finish(h->d_block_loss, loss, st));
@@ -467,7 +469,8 @@ int32_t tsit5_forward64(b200ude_handle *h, const double *u0, size_t N, double *o
 {
     Fwd64Host p{u0, out, h->q_ustep, h->q_dense, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
     const Adapt64Host a = adapt64(h);
-    CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 0, h->adaptive ? &a : nullptr, st));
+    if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_fwd_fkpp_f64(h->sh64, p, a, st));   // adaptive only (b200ude_create)
+    else CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 0, h->adaptive ? &a : nullptr, st));
     h->q_last_out = out;
     return B200UDE_OK;
 }
@@ -522,7 +525,8 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
             p.fused_l2 = 0;
             loss_l2 = loss;
         }
-        CUDA_TRY(h, launch_adj_f64(h->sh64, p, &a, st, &rows));
+        if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_adj_fkpp_f64(h->sh64, p, a, st, &rows));
+        else CUDA_TRY(h, launch_adj_f64(h->sh64, p, &a, st, &rows));
         CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss_l2 ? nullptr : loss, st));
         return B200UDE_OK;
     }
@@ -565,10 +569,14 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     const bool want64 = d->dtype == B200UDE_F64;
     if (want64) {
         // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_f64.cuh): LV / SEIR / NODE forms, Tsit5 and Vern7,
-        // fixed step and adaptive, interpolating adjoint
-        if (!generic_ok(*d) || d->model == B200UDE_MODEL_FKPP || d->solver == B200UDE_RKC2 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT)
+        // fixed step and adaptive, interpolating adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
+        if (!generic_ok(*d) || d->solver == B200UDE_RKC2 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT)
             return fail(nullptr, B200UDE_EUNSUPPORTED,
-                        "create: B200UDE_F64 kernels exist for the LV / SEIR / NODE forms (chain widths <= 64), Tsit5 / Vern7, interpolating adjoint");
+                        "create: B200UDE_F64 kernels exist for the LV / SEIR / NODE forms (chain widths <= 64), Tsit5 / Vern7, and the Fisher-KPP UPDE "
+                        "with adaptive Tsit5; interpolating adjoint");
+        if (d->model == B200UDE_MODEL_FKPP && (!d->adaptive || d->solver != B200UDE_TSIT5))
+            return fail(nullptr, B200UDE_EUNSUPPORTED,
+                        "create: B200UDE_F64 Fisher-KPP runs adaptive Tsit5 only (adaptive = 1, solver = B200UDE_TSIT5); fixed-step Fisher-KPP is fp32");
         if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1))
             return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
         kid = K_F64;
@@ -583,10 +591,17 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (!want64 && d->adaptive) {
         if (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)
             return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
-        if (!generic_ok(*d) || d->model == B200UDE_MODEL_FKPP)
-            return fail(nullptr, B200UDE_EUNSUPPORTED, "create: adaptive stepping is implemented for the LV / SEIR / NODE forms (chain widths <= 64)");
-        // adaptive solves run on the runtime-shape kernels, except the headline chain (tensor-core kernels with CTA-uniform attempt loops)
-        if (!((kid == K_LV32 || kid == K_SEIR64) && d->solver == B200UDE_TSIT5 && env_int("B200UDE_ADAPTIVE_TC", 1))) kid = K_GENERIC;
+        if (!generic_ok(*d))
+            return fail(nullptr, B200UDE_EUNSUPPORTED, "create: adaptive stepping is implemented for the LV / SEIR / NODE forms and the Fisher-KPP UPDE (chain widths <= 64)");
+        if (d->model == B200UDE_MODEL_FKPP) {
+            // Fisher-KPP: runtime-shape grid-per-CTA kernels (fkpp_adaptive.cuh), the tuned 1-16-16-1 chain included
+            if (d->solver != B200UDE_TSIT5)
+                return fail(nullptr, B200UDE_EUNSUPPORTED, "create: adaptive stepping of the Fisher-KPP UPDE is implemented for Tsit5 only");
+            kid = K_FKPP;
+        } else if (!((kid == K_LV32 || kid == K_SEIR64) && d->solver == B200UDE_TSIT5 && env_int("B200UDE_ADAPTIVE_TC", 1))) {
+            // adaptive solves run on the runtime-shape kernels, except the headline chain (tensor-core kernels with CTA-uniform attempt loops)
+            kid = K_GENERIC;
+        }
     }
     if (d->solver == B200UDE_RKC2) {
         if (d->n_stages < 2 || d->n_stages > 64) return fail(nullptr, B200UDE_EINVAL, "create: RKC2 needs 2 <= n_stages <= 64 (stability interval ~ 0.65 n_stages^2 >= dt * spectral radius)");
@@ -610,6 +625,16 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaGetDeviceProperties: %s", cudaGetErrorString(e));
     if (prop.major != 9 || prop.minor != 0)
         return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_90a code only", d->device, prop.major, prop.minor);
+    if (d->model == B200UDE_MODEL_FKPP && d->adaptive) {
+        // the adjoint keeps one gradient vector (P + 1 entries) per warp in shared memory: refuse here what could not launch
+        int P = d->n_prefix + d->n_suffix;
+        for (int l = 0; l < d->n_layers; ++l) P += d->widths[l] * d->widths[l + 1] + d->widths[l + 1];
+        const size_t smem = fkpp_adaptive_smem(d->state_dim, P, want64 ? (int)sizeof(double) : (int)sizeof(float)) + 16;   // + static
+        if (smem > prop.sharedMemPerBlockOptin)
+            return fail(nullptr, B200UDE_EUNSUPPORTED,
+                        "create: adaptive Fisher-KPP with %d grid points and %d parameters needs %zu B of shared memory per CTA (device limit %zu B)",
+                        d->state_dim, P, smem, (size_t)prop.sharedMemPerBlockOptin);
+    }
     e = cudaSetDevice(d->device);
     if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaSetDevice: %s", cudaGetErrorString(e));
 
@@ -656,7 +681,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (kid == K_F64) {
         const size_t N64 = h->cap, D64 = (size_t)h->D;
         const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
-        h->partial_blocks = (size_t)adj_rows_f64((int)N64);
+        h->partial_blocks = (size_t)(d->model == B200UDE_MODEL_FKPP ? adj_rows_fkpp((int)N64, d->state_dim) : adj_rows_f64((int)N64));
         bool ok64 = dalloc(h, &h->q_theta, (size_t)h->P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D64 * N64) == cudaSuccess &&
                     dalloc(h, &h->q_dense, (rec * 6 + 1) * D64 * N64) == cudaSuccess &&
                     dalloc(h, &h->q_partial, h->partial_blocks * (size_t)(h->P + 1)) == cudaSuccess;

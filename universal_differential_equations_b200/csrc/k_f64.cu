@@ -1,5 +1,6 @@
 // k_f64.cu -- double-precision kernels (dtype = B200UDE_F64): launchers of ude_f64.cuh + the fp64 reduction / L2 helpers.
 #include "ude_f64.cuh"
+#include "fkpp_adaptive.cuh"
 
 #include "params.h"
 
@@ -84,6 +85,65 @@ cudaError_t launch_adj_f64(const Shape64Host &s, const Adj64Host &p, const Adapt
         if (e != cudaSuccess) return e;
         kern<<<grid, F64_BLOCK, smem, st>>>(adj(p));
     }
+    return cudaGetLastError();
+}
+
+// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp64: theta from the handle's device copy) ----
+struct FkppOps64 {
+    using real = double;
+    static __device__ __forceinline__ double theta(int i) { return f64::c_gen.theta[i]; }
+    static __device__ __forceinline__ int P() { return f64::c_gen.P; }
+    static __device__ __forceinline__ double chain(double x)
+    {
+        double y;
+        f64::chain_fwd<false>(&x, &y, nullptr, nullptr);
+        return y;
+    }
+    static __device__ __forceinline__ double chain_vjp(double x, double dy, double w, double *gw, int lane)
+    {
+        double dx;
+        f64::chain_vjp(&x, &dy, w, &dx, gw, lane);
+        return dx;
+    }
+    static __device__ __forceinline__ void warp_acc(double *gw, int idx, double v, int lane) { f64::warp_acc(gw, idx, v, lane); }
+    static __device__ __forceinline__ void interp(double Th, double *bw) { f64::tsit5_bw_rt(Th, bw); }
+    static __device__ __forceinline__ double btilde(int j) { return f64::tsit5_btilde(j); }
+};
+
+cudaError_t launch_fwd_fkpp_f64(const Shape64Host &s, const Fwd64Host &p, const Adapt64Host &a, cudaStream_t st)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    fkpp_adapt::Fwd<double> q;
+    int th;
+    fkpp_adapt::cta_geometry(s.D, &q.tpc, &th);
+    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.tgrid = a.tgrid; q.nacc = a.nacc;
+    q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.max_steps = a.max_steps;
+    q.t0 = a.t0; q.save_dt = a.save_dt; q.abstol = a.abstol; q.reltol = a.reltol;
+    auto kern = fkpp_adapt::forward_kernel<FkppOps64>;
+    const size_t smem = fkpp_adapt::fwd_smem(s.D, sizeof(double));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<(p.N + q.tpc - 1) / q.tpc, th, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adj_fkpp_f64(const Shape64Host &s, const Adj64Host &p, const Adapt64Host &a, cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    fkpp_adapt::Adj<double> q;
+    int th;
+    fkpp_adapt::cta_geometry(s.D, &q.tpc, &th);
+    q.ustep = p.ustep; q.dense = p.dense; q.tgrid = a.tgrid; q.nacc = a.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.t0 = a.t0; q.save_dt = a.save_dt;
+    auto kern = fkpp_adapt::adjoint_kernel<FkppOps64>;
+    const size_t smem = fkpp_adapt::adj_smem(s.D, s.P, sizeof(double));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + q.tpc - 1) / q.tpc;
+    *rows_out = grid * (th / 32);
+    kern<<<grid, th, smem, st>>>(q);
     return cudaGetLastError();
 }
 

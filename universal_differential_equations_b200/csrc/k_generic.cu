@@ -1,5 +1,8 @@
 // k_generic.cu -- shape-generic UDE kernels (runtime chain widths / activations; LV, SEIR, NODE forms).
 #include "ude_generic.cuh"
+#include "fkpp_adaptive.cuh"
+
+#include <algorithm>
 
 namespace b200ude {
 
@@ -185,6 +188,74 @@ cudaError_t launch_adj_fkpp(const GenericShape &gs, const ConstTables &t, const 
     if (e != cudaSuccess) return e;
     *rows_out = grid * (th / 32);
     kern<<<grid, th, smem, st>>>(p, g);
+    return cudaGetLastError();
+}
+
+// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp32: theta from the constant bank, runtime chain shape) ----
+struct FkppOps32 {
+    using real = float;
+    static __device__ __forceinline__ float theta(int i) { return c_theta[i]; }
+    static __device__ __forceinline__ int P() { return generic::c_gen.P; }
+    static __device__ __forceinline__ float chain(float x)
+    {
+        float y;
+        generic::chain_fwd<false>(&x, &y, nullptr, nullptr);
+        return y;
+    }
+    static __device__ __forceinline__ float chain_vjp(float x, float dy, float w, float *gw, int lane)
+    {
+        float dx;
+        generic::chain_vjp(&x, &dy, w, &dx, gw, lane);
+        return dx;
+    }
+    static __device__ __forceinline__ void warp_acc(float *gw, int idx, float v, int lane) { generic::warp_acc(gw, idx, v, lane); }
+    static __device__ __forceinline__ void interp(float Th, float *bw) { generic::tsit5_bw_rt(Th, bw); }
+    static __device__ __forceinline__ float btilde(int j) { return generic::tsit5_btilde(j); }
+};
+
+size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes)
+{
+    return std::max(fkpp_adapt::fwd_smem(Nx, real_bytes), fkpp_adapt::adj_smem(Nx, P, real_bytes));
+}
+
+cudaError_t launch_fwd_fkpp_adaptive(const GenericShape &gs, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(gs, st);
+    if (e != cudaSuccess) return e;
+    fkpp_adapt::Fwd<float> q;
+    int th;
+    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
+    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
+    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
+    q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
+    auto kern = fkpp_adapt::forward_kernel<FkppOps32>;
+    const size_t smem = fkpp_adapt::fwd_smem(gs.D, sizeof(float));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<(p.N + q.tpc - 1) / q.tpc, th, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adj_fkpp_adaptive(const GenericShape &gs, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag, cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(gs, st);
+    if (e != cudaSuccess) return e;
+    fkpp_adapt::Adj<float> q;
+    int th;
+    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
+    q.ustep = p.ustep; q.dense = p.dense; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.t0 = ag.t0; q.save_dt = ag.save_dt;
+    auto kern = fkpp_adapt::adjoint_kernel<FkppOps32>;
+    const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + q.tpc - 1) / q.tpc;
+    *rows_out = grid * (th / 32);
+    kern<<<grid, th, smem, st>>>(q);
     return cudaGetLastError();
 }
 

@@ -130,6 +130,10 @@ cudaError_t launch_l2_finish(const float *block_loss, float *loss, cudaStream_t)
 cudaError_t launch_fwd_fkpp(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
 cudaError_t launch_adj_fkpp(const GenericShape &, const ConstTables &, const AdjParams &, cudaStream_t, int *rows_out);
 int adj_rows_fkpp(int N, int Nx);
+// adaptive Tsit5 of the Fisher-KPP UPDE (fkpp_adaptive.cuh): partial rows as adj_rows_fkpp in both precisions
+cudaError_t launch_fwd_fkpp_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
+cudaError_t launch_adj_fkpp_adaptive(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
+size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes);   // per-CTA dynamic shared memory of the larger of the two kernels
 cudaError_t launch_fwd_seir(const Variant &, const ConstTables &, const FwdParams &, cudaStream_t);
 cudaError_t launch_adj_seir(const Variant &, const ConstTables &, const AdjParams &, cudaStream_t, int *rows_out);
 cudaError_t launch_fwd_seir_vern7(const Variant &, const ConstTables &, const FwdParams &, cudaStream_t);
@@ -187,6 +191,8 @@ int adj_rows_f64(int N);
 cudaError_t launch_fwd_f64(const Shape64Host &, const Fwd64Host &, int solver, const Adapt64Host *adaptive_or_null, cudaStream_t);
 cudaError_t launch_adj_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *adaptive_or_null, cudaStream_t, int *rows_out);
 cudaError_t launch_reduce_f64(const double *partial, int nrows, int P1, double *grad, double *loss, cudaStream_t);
+cudaError_t launch_fwd_fkpp_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // adaptive Tsit5 only
+cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot_f64(const Shape64Host &, const double *out, const double *data, double *cot, double *loss, size_t N, int n_save, cudaStream_t);
 
 }  // namespace b200ude
