@@ -38,6 +38,7 @@
  *    bank, so work of DIFFERENT handles of those kinds on one device must be stream-ordered (not concurrent).
  *  - the interpolating adjoint of a Vern7 handle runs over a Tsit5 re-solve from the same u0 with the same step / tolerances
  *    (Vern7's lazy dense output is not available): with the fused L2 entry point the reported loss is that of the re-solve.
+ *    The discrete adjoint of a Vern7 handle differentiates the Vern7 solve itself.
  */
 #ifndef B200UDE_H
 #define B200UDE_H
@@ -56,7 +57,7 @@ extern "C" {
 #define B200UDE_F64 1 /* double precision: EVERY device array of the calls (theta, u0, out, data, dL_dout, grad_theta, grad_u0, loss) is
                         * double.  Runtime-shape kernels for the LV / SEIR / NODE forms, Tsit5 and Vern7, fixed step and adaptive,
                         * and for the Fisher-KPP UPDE with adaptive Tsit5 (fixed-step Fisher-KPP is fp32 only); interpolating
-                        * adjoint -- the precision the reference's scenario 1 / 2, SEIR and Fisher-KPP scripts run in (Float64).  Entry points: create / set_params / get_params / forward / adjoint / adjoint_l2;
+                        * adjoint, and the discrete adjoint of fixed-step Tsit5 / Vern7 and adaptive Vern7 -- the precision the reference's scenario 1 / 2, SEIR and Fisher-KPP scripts run in (Float64).  Entry points: create / set_params / get_params / forward / adjoint / adjoint_l2;
                         * the host-buffer, ADAM and peer entry points return B200UDE_EUNSUPPORTED for such handles. */
 
 /* model kinds: the UDE right-hand sides of the reference */
@@ -86,9 +87,13 @@ extern "C" {
 
 /* sensealg */
 #define B200UDE_INTERPOLATING_ADJOINT 0 /* InterpolatingAdjoint(autojacvec = ReverseDiffVJP())  seir_exposure.jl:71,140 */
-#define B200UDE_DISCRETE_ADJOINT 1      /* exact gradient of the discrete fixed-step scheme by reverse accumulation through the
-                                           stages: the quantity ForwardDiffSensitivity() computes in forward mode
-                                           (scenario_1.jl:86, scenario_2.jl:108, hudson_bay.jl:102); LV chains, Tsit5 fixed step */
+#define B200UDE_DISCRETE_ADJOINT 1      /* exact gradient of the discrete scheme, the accepted step sequence held fixed, by reverse
+                                           accumulation through the stages of every step: the quantity ForwardDiffSensitivity()
+                                           computes in forward mode (scenario_1.jl:84-87, scenario_2.jl:106-108, hudson_bay.jl:99-102).
+                                           Fixed-step Tsit5, fixed-step Vern7 and adaptive Vern7 (save times are tstops) on the
+                                           LV / SEIR / SEIR_NODE / NODE forms, fp32 and fp64; the fused L2 reads the recorded
+                                           step-end states, so the loss reported is that of the solve itself.  Not for adaptive
+                                           Tsit5 (its saveat values come from the interpolant), the Fisher-KPP UPDE or RKC2. */
 
 /* memory space of a pointer argument */
 #define B200UDE_HOST 0

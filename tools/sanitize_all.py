@@ -29,12 +29,28 @@ run("generic", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1)
 run("adaptive", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, adaptive=True, abstol=1e-5, reltol=1e-5, max_steps=200)
 run("vern7", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7())
 run("vern7-adaptive", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7(), adaptive=True, abstol=1e-5, reltol=1e-5, max_steps=200)
+# discrete adjoint (discrete_adjoint.cuh): fp32 through every entry point, fp64 through forward / adjoint_l2
+fd = ude.ForwardDiffSensitivity()
+run("generic-discrete", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, sensealg=fd)
+run("vern7-discrete", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7(), sensealg=fd)
+run("vern7-adaptive-discrete", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7(), adaptive=True, abstol=1e-5, reltol=1e-5,
+    max_steps=200, sensealg=fd)
+for alg, adaptive in ((ude.Tsit5(), False), (ude.Vern7(), False), (ude.Vern7(), True)):
+    s = ude.UDESolver(gen, 0.0, 0.1, 30, 1, max_trajectories=N, alg=alg, adaptive=adaptive, abstol=1e-6, reltol=1e-6, sensealg=fd, dtype=torch.float64)
+    s.set_params(torch.from_numpy(glorot_theta((2, 7, 2), seed=3).astype(np.float64)).cuda())
+    s.forward(torch.from_numpy(u0.astype(np.float64)).cuda())
+    L, g, gu = s.adjoint_l2(torch.from_numpy(y.astype(np.float64)).cuda(), want_grad_u0=True)
+    torch.cuda.synchronize()
+    print("f64-discrete", type(alg).__name__, adaptive, float(L), float(g.abs().sum()))
+    s.close()
 Ns = 300
 S0 = 14e6
 us = np.zeros((7, Ns), np.float32); us[0] = 0.9 * S0; us[1:4] = rng.uniform(0, 50, (3, Ns)); us[4] = S0
 ys = rng.uniform(0, 100, (8, 7, Ns)).astype(np.float32)
 seir = ude.SEIRExposureUDE(ude.FastChain(ude.FastDense(3, 64, ude.tanh), ude.FastDense(64, 64, ude.tanh), ude.FastDense(64, 1)))
 run("seir64", seir, glorot_theta((3, 64, 64, 1), seed=2), us, ys, 0.25, 28, 4, loss_weights=[0, 1, 1, 1, 0, 0, 0])
+run("seir64-vern7-adaptive-discrete", seir, glorot_theta((3, 64, 64, 1), seed=2), us, ys, 1.0, 7, 1, loss_weights=[0, 1, 1, 1, 0, 0, 0], alg=ude.Vern7(),
+    adaptive=True, abstol=1e-4, reltol=1e-4, max_steps=128, sensealg=ude.ForwardDiffSensitivity())
 run("seir64-adaptive-tc", seir, glorot_theta((3, 64, 64, 1), seed=2), us, ys, 1.0, 7, 1, loss_weights=[0, 1, 1, 1, 0, 0, 0], adaptive=True, abstol=1e-4, reltol=1e-4, max_steps=128)
 node = ude.SEIRNeuralODE(ude.FastChain(ude.FastDense(7, 64, ude.tanh), ude.FastDense(64, 64, ude.tanh), ude.FastDense(64, 64, ude.tanh), ude.FastDense(64, 7)))
 run("seir-node", node, 0.3 * glorot_theta((7, 64, 64, 64, 7), seed=6), us[:, :40].copy(), ys[:, :, :40].copy(), 0.25, 28, 4, loss_weights=[0, 1, 1, 1, 0, 0, 0])

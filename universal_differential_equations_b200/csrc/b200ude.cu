@@ -29,7 +29,8 @@ thread_local std::string g_create_error;
 //   K_LV5Px  LV 2 -> 5 -> 5 -> 5 -> 2, per-layer activations, x trainable linear rates
 //            scenario_1.jl:62-73 (x=0), scenario_2.jl:79-98 (x=1), hudson_bay.jl:77-91 (x=2)
 //   K_GENERIC  any LV / SEIR / SEIR_NODE / NODE form with chain widths <= 64 and <= 5 layers (k_generic.cu): functional
-//            coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7 and the adaptive path of untuned chains
+//            coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7, the adaptive path of untuned chains and
+//            the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh)
 //   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126)
 //   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
 //   K_FKPP16   Fisher-KPP UPDE with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu)                BASELINE config 4
@@ -74,6 +75,7 @@ struct b200ude_handle {
     // adaptive stepping
     bool adaptive = false;
     float *d_tgrid = nullptr, *d_cot = nullptr, *d_block_loss = nullptr;
+    float *d_hstep = nullptr;   // discrete-adjoint Vern7: step sizes of the accepted steps
     int *d_nacc = nullptr;
     const float *last_out = nullptr;
     AdaptiveGrid ag{};
@@ -98,7 +100,7 @@ struct b200ude_handle {
     // double-precision path (dtype = B200UDE_F64, kid = K_F64): every device array of the handle and of the callers is double
     Shape64Host sh64{};
     double *q_theta = nullptr, *q_ustep = nullptr, *q_dense = nullptr, *q_partial = nullptr, *q_tgrid = nullptr, *q_cot = nullptr;
-    double *q_u0_keep = nullptr, *q_aux_out = nullptr;
+    double *q_u0_keep = nullptr, *q_aux_out = nullptr, *q_hstep = nullptr;
     const double *q_last_out = nullptr;
     size_t dev_bytes = 0;
     std::string err;
@@ -264,6 +266,18 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
+    if (h->desc.solver == B200UDE_VERN7 && h->var.discrete) {
+        // discrete adjoint: the forward records u_n of every (accepted) step, which the adjoint recomputes the stages from
+        FwdParams p;
+        p.u0 = u0; p.out = out; p.ustep = h->d_ustep; p.dense = nullptr; p.status = status; p.theta = h->d_theta;
+        p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
+        if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
+        else CUDA_TRY(h, launch_fwd_vern7(h->gen, h->tab, p, st));
+        h->last_out = out;
+        h->N = N;
+        h->have_forward = true;
+        return B200UDE_OK;
+    }
     if (h->desc.solver == B200UDE_VERN7) {
         // Vern7 writes the saved states only.  Its lazy dense output is not available (SURVEY.md App. A.3), so the
         // interpolating adjoint of a Vern7 solve runs over a Tsit5 re-solve from the same u0 with the same step /
@@ -320,6 +334,13 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
     p.dt = (float)h->desc.dt;
     cudaError_t e = cudaSuccess;
     int grid = 0;
+    if (h->var.discrete && h->kid == K_GENERIC) {
+        // discrete adjoint of a runtime-shape Tsit5 / Vern7 solve over its recorded steps; the fused L2 reads the recorded step-end states
+        CUDA_TRY(h, launch_adj_discrete(h->gen, h->tab, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &h->ag : nullptr, st, &grid));
+        if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
+        else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
     if (h->adaptive) {
         if (l2) {   // form the cotangent 2 w (out - data) from the interpolated saved states of the last forward
             CUDA_TRY(h, launch_l2_cot(h->tab, h->last_out, cot, h->d_cot, h->d_block_loss, h->D, h->N, h->n_save, st));
@@ -462,7 +483,8 @@ cudaError_t launch_adam(b200ude_handle *h, const b200ude_adam *o, const float *g
 // ---- double-precision path (kid = K_F64) ----------------------------------------------------------------------------------
 Adapt64Host adapt64(const b200ude_handle *h)
 {
-    return Adapt64Host{h->desc.t0, h->desc.dt * h->desc.save_every, h->desc.abstol, h->desc.reltol, h->n_save, h->desc.max_steps, h->q_tgrid, h->d_nacc};
+    return Adapt64Host{h->desc.t0, h->desc.dt * h->desc.save_every, h->desc.abstol, h->desc.reltol, h->n_save, h->desc.max_steps, h->q_tgrid, h->d_nacc,
+                       h->q_hstep};
 }
 
 int32_t tsit5_forward64(b200ude_handle *h, const double *u0, size_t N, double *out, int32_t *status, cudaStream_t st)
@@ -481,6 +503,16 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
+    if (h->desc.solver == B200UDE_VERN7 && h->var.discrete) {
+        // discrete adjoint: u_n of every (accepted) step recorded (as in fp32)
+        Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
+        const Adapt64Host a = adapt64(h);
+        CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
+        h->q_last_out = out;
+        h->N = N;
+        h->have_forward = true;
+        return B200UDE_OK;
+    }
     if (h->desc.solver == B200UDE_VERN7) {
         // saved states only; the interpolating adjoint runs over a Tsit5 re-solve with the same step / tolerances (as in fp32)
         Fwd64Host p{u0, out, nullptr, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
@@ -516,6 +548,12 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
     if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
     Adj64Host p{h->q_ustep, h->q_dense, cot, grad_u0, h->q_partial, (int)h->N, h->desc.n_steps, h->desc.save_every, l2 ? 1 : 0, h->desc.dt};
     int rows = 0;
+    if (h->var.discrete) {   // fixed-step Tsit5 / Vern7, adaptive Vern7 (b200ude_create); the fused L2 reads the recorded step-end states
+        const Adapt64Host a = adapt64(h);
+        CUDA_TRY(h, launch_adj_discrete_f64(h->sh64, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &a : nullptr, st, &rows));
+        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
     if (h->adaptive) {
         const Adapt64Host a = adapt64(h);
         double *loss_l2 = nullptr;
@@ -567,13 +605,21 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (d->n_loss_weights != 0 && d->n_loss_weights != d->state_dim) return fail(nullptr, B200UDE_EINVAL, "create: n_loss_weights must be 0 or state_dim");
     KernelId kid = pick_kernel(*d);
     const bool want64 = d->dtype == B200UDE_F64;
+    const bool disc = d->sensealg == B200UDE_DISCRETE_ADJOINT;
+    // discrete adjoint: the tuned LV kernels (fixed-step Tsit5 on 2-32-32-2 / 2-5-5-5-2, fp32) and the runtime-shape kernels of
+    // discrete_adjoint.cuh.  Adaptive Tsit5 saves through its free interpolant, which an exact discrete adjoint would also have to
+    // differentiate; Fisher-KPP and RKC2 have no such kernels.
+    if (disc && (d->model == B200UDE_MODEL_FKPP || d->solver == B200UDE_RKC2 || (d->adaptive && d->solver == B200UDE_TSIT5)))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: the discrete adjoint (ForwardDiffSensitivity) has kernels for fixed-step Tsit5 and for fixed-step or adaptive Vern7 on the "
+                    "LV / SEIR / SEIR_NODE / NODE forms (chain widths <= 64), fp32 and fp64; not for adaptive Tsit5, the Fisher-KPP UPDE or RKC2");
     if (want64) {
         // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_f64.cuh): LV / SEIR / NODE forms, Tsit5 and Vern7,
-        // fixed step and adaptive, interpolating adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
-        if (!generic_ok(*d) || d->solver == B200UDE_RKC2 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT)
+        // fixed step and adaptive, interpolating or discrete adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
+        if (!generic_ok(*d) || d->solver == B200UDE_RKC2)
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: B200UDE_F64 kernels exist for the LV / SEIR / NODE forms (chain widths <= 64), Tsit5 / Vern7, and the Fisher-KPP UPDE "
-                        "with adaptive Tsit5; interpolating adjoint");
+                        "with adaptive Tsit5 and the interpolating adjoint");
         if (d->model == B200UDE_MODEL_FKPP && (!d->adaptive || d->solver != B200UDE_TSIT5))
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: B200UDE_F64 Fisher-KPP runs adaptive Tsit5 only (adaptive = 1, solver = B200UDE_TSIT5); fixed-step Fisher-KPP is fp32");
@@ -586,7 +632,8 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
             return fail(nullptr, B200UDE_EUNSUPPORTED, "create: Vern7 kernels exist for the LV / SEIR / NODE forms only");
         // fixed-step Vern7 of the SEIR 3-64-64-1 chain runs on the tensor-core kernels (and so does the Tsit5 re-solve its
         // adjoint uses); every other Vern7 configuration on the runtime-shape kernels
-        if (!(kid == K_SEIR64 && !d->adaptive && env_int("B200UDE_SEIR_VERN7_TC", 1))) kid = K_GENERIC;
+        // (the discrete adjoint of a Vern7 solve runs on the runtime-shape kernels only)
+        if (disc || !(kid == K_SEIR64 && !d->adaptive && env_int("B200UDE_SEIR_VERN7_TC", 1))) kid = K_GENERIC;
     }
     if (!want64 && d->adaptive) {
         if (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)
@@ -609,10 +656,9 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: RKC2 has kernels for the Fisher-KPP UPDE with the 1-16-16-1 chain on even grids (fixed step, interpolating adjoint)");
     }
-    if (d->sensealg == B200UDE_DISCRETE_ADJOINT &&
-        (d->adaptive || d->solver != B200UDE_TSIT5 || !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2)))
-        return fail(nullptr, B200UDE_EUNSUPPORTED,
-                    "create: the discrete adjoint has kernels for fixed-step Tsit5 on the LV chains 2-32-32-2 and 2-5-5-5-2 (the scripts that use ForwardDiffSensitivity)");
+    // fixed-step Tsit5 with the discrete adjoint: LV 2-32-32-2 / 2-5-5-5-2 keep their tuned kernels, every other form runs on the
+    // runtime-shape ones (the SEIR tensor-core kernels have no discrete adjoint)
+    if (disc && !want64 && kid != K_NONE && !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2)) kid = K_GENERIC;
     if (kid == K_NONE)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: no sm_90a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");
@@ -682,12 +728,15 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         const size_t N64 = h->cap, D64 = (size_t)h->D;
         const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
         h->partial_blocks = (size_t)(d->model == B200UDE_MODEL_FKPP ? adj_rows_fkpp((int)N64, d->state_dim) : adj_rows_f64((int)N64));
+        // a discrete-adjoint Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead when adaptive
+        const bool disc_vern7 = disc && d->solver == B200UDE_VERN7;
         bool ok64 = dalloc(h, &h->q_theta, (size_t)h->P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D64 * N64) == cudaSuccess &&
-                    dalloc(h, &h->q_dense, (rec * 6 + 1) * D64 * N64) == cudaSuccess &&
+                    (disc_vern7 || dalloc(h, &h->q_dense, (rec * 6 + 1) * D64 * N64) == cudaSuccess) &&
                     dalloc(h, &h->q_partial, h->partial_blocks * (size_t)(h->P + 1)) == cudaSuccess;
         if (h->adaptive)
             ok64 = ok64 && dalloc(h, &h->q_tgrid, (rec + 1) * N64) == cudaSuccess && dalloc(h, &h->d_nacc, N64) == cudaSuccess &&
-                   dalloc(h, &h->q_cot, (size_t)h->n_save * D64 * N64) == cudaSuccess;
+                   dalloc(h, &h->q_cot, (size_t)h->n_save * D64 * N64) == cudaSuccess &&
+                   (!disc_vern7 || dalloc(h, &h->q_hstep, rec * N64) == cudaSuccess);
         if (!ok64) {
             g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
             b200ude_destroy(h);
@@ -716,8 +765,10 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     ok = ok && dalloc(h, &h->d_theta, (size_t)((h->P + 3) / 4) * 4) == cudaSuccess;
     const size_t rec_steps = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;   // capacity of the step record
     ok = ok && dalloc(h, &h->d_ustep, (rec_steps + 1) * D * N) == cudaSuccess;
-    ok = ok && dalloc(h, &h->d_dense, (rec_steps * 6 + 1) * D * N) == cudaSuccess;
+    const bool disc_vern7 = disc && d->solver == B200UDE_VERN7;   // stages recomputed from u_n: no dense record
+    if (!disc_vern7) ok = ok && dalloc(h, &h->d_dense, (rec_steps * 6 + 1) * D * N) == cudaSuccess;
     if (h->adaptive) {
+        if (disc_vern7) ok = ok && dalloc(h, &h->d_hstep, rec_steps * N) == cudaSuccess;
         ok = ok && dalloc(h, &h->d_tgrid, (rec_steps + 1) * N) == cudaSuccess;
         ok = ok && dalloc(h, &h->d_nacc, N) == cudaSuccess;
         ok = ok && dalloc(h, &h->d_cot, (size_t)h->n_save * D * N) == cudaSuccess;
@@ -744,7 +795,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     }
     h->tab.serial = serial;
     h->ag.t0 = (float)d->t0; h->ag.save_dt = (float)(d->dt * d->save_every); h->ag.abstol = (float)d->abstol; h->ag.reltol = (float)d->reltol;
-    h->ag.n_save = h->n_save; h->ag.max_steps = d->max_steps; h->ag.tgrid = h->d_tgrid; h->ag.nacc = h->d_nacc;
+    h->ag.n_save = h->n_save; h->ag.max_steps = d->max_steps; h->ag.tgrid = h->d_tgrid; h->ag.nacc = h->d_nacc; h->ag.hstep = h->d_hstep;
     h->tab.d_theta = h->d_theta;
     h->tab.P = h->P;
     for (int i = 0; i < 16; ++i) {
@@ -766,9 +817,9 @@ void b200ude_destroy(b200ude_handle *h)
     cudaFree(h->d_peer_buf);
     cudaFree(h->d_u0_keep); cudaFree(h->d_aux_out);
     cudaFree(h->d_adam_m); cudaFree(h->d_adam_v); cudaFree(h->d_adam_t); cudaFree(h->d_train_out);
-    cudaFree(h->d_tgrid); cudaFree(h->d_nacc); cudaFree(h->d_cot); cudaFree(h->d_block_loss);
+    cudaFree(h->d_tgrid); cudaFree(h->d_nacc); cudaFree(h->d_cot); cudaFree(h->d_block_loss); cudaFree(h->d_hstep);
     cudaFree(h->q_theta); cudaFree(h->q_ustep); cudaFree(h->q_dense); cudaFree(h->q_partial); cudaFree(h->q_tgrid); cudaFree(h->q_cot);
-    cudaFree(h->q_u0_keep); cudaFree(h->q_aux_out);
+    cudaFree(h->q_u0_keep); cudaFree(h->q_aux_out); cudaFree(h->q_hstep);
     if (h->h_loss) cudaFreeHost(h->h_loss);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);

@@ -1,6 +1,7 @@
 // k_f64.cu -- double-precision kernels (dtype = B200UDE_F64): launchers of ude_f64.cuh + the fp64 reduction / L2 helpers.
 #include "ude_f64.cuh"
 #include "fkpp_adaptive.cuh"
+#include "discrete_adjoint.cuh"
 
 #include "params.h"
 
@@ -49,7 +50,8 @@ static f64::Adj64 adj(const Adj64Host &p)
 }
 static f64::Adapt64 adapt(const Adapt64Host &a, bool record)
 {
-    return f64::Adapt64{a.t0, a.save_dt, a.abstol, a.reltol, a.n_save, a.max_steps, record ? a.tgrid : nullptr, record ? a.nacc : nullptr};
+    return f64::Adapt64{a.t0, a.save_dt, a.abstol, a.reltol, a.n_save, a.max_steps, record ? a.tgrid : nullptr, record ? a.nacc : nullptr,
+                        record ? a.hstep : nullptr};
 }
 
 cudaError_t launch_fwd_f64(const Shape64Host &s, const Fwd64Host &p, int solver, const Adapt64Host *ad, cudaStream_t st)
@@ -57,8 +59,8 @@ cudaError_t launch_fwd_f64(const Shape64Host &s, const Fwd64Host &p, int solver,
     cudaError_t e = upload_shape(s, st);
     if (e != cudaSuccess) return e;
     const int grid = (p.N + F64_BLOCK - 1) / F64_BLOCK;
-    if (solver == 1) {   // Vern7
-        if (ad) f64::vern7_adaptive_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p), adapt(*ad, false));
+    if (solver == 1) {   // Vern7: the step record only for the discrete adjoint (p.ustep set)
+        if (ad) f64::vern7_adaptive_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p), adapt(*ad, p.ustep != nullptr));
         else f64::vern7_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p));
     } else {
         if (ad) f64::adaptive_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p), adapt(*ad, true));
@@ -85,6 +87,41 @@ cudaError_t launch_adj_f64(const Shape64Host &s, const Adj64Host &p, const Adapt
         if (e != cudaSuccess) return e;
         kern<<<grid, F64_BLOCK, smem, st>>>(adj(p));
     }
+    return cudaGetLastError();
+}
+
+// ---- discrete adjoint (discrete_adjoint.cuh in fp64: theta from the handle's device copy) ----
+struct DiscreteOps64 {
+    using real = double;
+    static constexpr int MAXD = f64::MAXD;
+    static __device__ __forceinline__ int D() { return f64::c_gen.D; }
+    static __device__ __forceinline__ int P() { return f64::c_gen.P; }
+    static __device__ __forceinline__ double lossw(int c) { return f64::c_gen.lossw[c]; }
+    static __device__ __forceinline__ void rhs(const double *u, double *du) { f64::model_rhs(u, du); }
+    static __device__ __forceinline__ void vjp(const double *u, const double *g, double lv, double *kl, double *gw, int lane)
+    {
+        f64::model_vjp(u, g, 1.0, lv, kl, gw, lane);
+    }
+};
+
+cudaError_t launch_adj_discrete_f64(const Shape64Host &s, const Adj64Host &p, int solver, const Adapt64Host *ad, cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    discrete::Params<double> q;
+    q.ustep = p.ustep; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.tgrid = ad ? ad->tgrid : nullptr; q.hstep = ad ? ad->hstep : nullptr; q.nacc = ad ? ad->nacc : nullptr;
+    q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
+    q.dt = p.dt; q.t0 = ad ? ad->t0 : 0.0; q.save_dt = ad ? ad->save_dt : 0.0;
+    q.margin = 5e-13;   // half the clipping margin of vern7_adaptive_forward_kernel
+    auto kern = solver == 1 ? discrete::adjoint_kernel<DiscreteOps64, discrete::Vern7Scheme, F64_BLOCK>
+                            : discrete::adjoint_kernel<DiscreteOps64, discrete::Tsit5Scheme, F64_BLOCK>;
+    const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + F64_BLOCK - 1) / F64_BLOCK;
+    *rows_out = grid * (F64_BLOCK / 32);
+    kern<<<grid, F64_BLOCK, smem, st>>>(q);
     return cudaGetLastError();
 }
 

@@ -1,6 +1,7 @@
 // k_generic.cu -- shape-generic UDE kernels (runtime chain widths / activations; LV, SEIR, NODE forms).
 #include "ude_generic.cuh"
 #include "fkpp_adaptive.cuh"
+#include "discrete_adjoint.cuh"
 
 #include <algorithm>
 
@@ -70,8 +71,49 @@ cudaError_t launch_fwd_vern7_adaptive(const GenericShape &g, const ConstTables &
     if (e != cudaSuccess) return e;
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
-    generic::AdaptParams ap{ag.t0, ag.save_dt, ag.abstol, ag.reltol, ag.n_save, ag.max_steps, nullptr, nullptr};   // no step record
+    // the step record only for the discrete adjoint (p.ustep set); the interpolating adjoint re-solves with Tsit5
+    const bool rec = p.ustep != nullptr;
+    generic::AdaptParams ap{ag.t0, ag.save_dt, ag.abstol, ag.reltol, ag.n_save, ag.max_steps, rec ? ag.tgrid : nullptr, rec ? ag.nacc : nullptr,
+                            rec ? ag.hstep : nullptr};
     generic::vern7_adaptive_forward_kernel<GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ap);
+    return cudaGetLastError();
+}
+
+// ---- discrete adjoint (discrete_adjoint.cuh in fp32: theta from the constant bank, runtime chain shape) ----
+struct DiscreteOps32 {
+    using real = float;
+    static constexpr int MAXD = generic::MAXD;
+    static __device__ __forceinline__ int D() { return generic::c_gen.D; }
+    static __device__ __forceinline__ int P() { return generic::c_gen.P; }
+    static __device__ __forceinline__ float lossw(int c) { return c_lossw[c]; }
+    static __device__ __forceinline__ void rhs(const float *u, float *du) { generic::model_rhs(u, du); }
+    static __device__ __forceinline__ void vjp(const float *u, const float *g, float lv, float *kl, float *gw, int lane)
+    {
+        generic::model_vjp(u, g, 1.0f, lv, kl, gw, lane);
+    }
+};
+
+cudaError_t launch_adj_discrete(const GenericShape &g, const ConstTables &t, const AdjParams &p, int solver, const AdaptiveGrid *ag,
+                                cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(g, st);
+    if (e != cudaSuccess) return e;
+    discrete::Params<float> q;
+    q.ustep = p.ustep; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.tgrid = ag ? ag->tgrid : nullptr; q.hstep = ag ? ag->hstep : nullptr; q.nacc = ag ? ag->nacc : nullptr;
+    q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
+    q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
+    q.margin = 5e-7f;   // half the clipping margin of vern7_adaptive_forward_kernel
+    auto kern = solver == 1 ? discrete::adjoint_kernel<DiscreteOps32, discrete::Vern7Scheme, GEN_BLOCK>
+                            : discrete::adjoint_kernel<DiscreteOps32, discrete::Tsit5Scheme, GEN_BLOCK>;
+    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
+    *rows_out = grid * (GEN_BLOCK / 32);
+    kern<<<grid, GEN_BLOCK, smem, st>>>(q);
     return cudaGetLastError();
 }
 

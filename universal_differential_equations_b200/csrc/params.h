@@ -102,6 +102,7 @@ struct AdaptiveGrid {
     int n_save, max_steps;
     float *tgrid;   // [max_steps+1][N]
     int *nacc;      // [N]
+    float *hstep;   // [max_steps][N] step sizes (discrete-adjoint Vern7 handles only, else nullptr)
 };
 constexpr int L2_BLOCKS = 296;
 
@@ -125,6 +126,10 @@ cudaError_t launch_fwd_vern7(const GenericShape &, const ConstTables &, const Fw
 cudaError_t launch_fwd_vern7_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
 cudaError_t launch_fwd_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
 cudaError_t launch_adj_adaptive(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
+// discrete adjoint (discrete_adjoint.cuh) of a runtime-shape Tsit5 (solver 0) / Vern7 (solver 1) solve; ag: the adaptive Vern7
+// record, nullptr on a fixed grid.  Partial rows as adj_rows_generic.
+cudaError_t launch_adj_discrete(const GenericShape &, const ConstTables &, const AdjParams &, int solver, const AdaptiveGrid *ag,
+                                cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot(const ConstTables &, const float *out, const float *data, float *cot, float *block_loss, int D, size_t N, int n_save, cudaStream_t);
 cudaError_t launch_l2_finish(const float *block_loss, float *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
@@ -186,10 +191,13 @@ struct Adapt64Host {
     int n_save, max_steps;
     double *tgrid;
     int *nacc;
+    double *hstep;   // discrete-adjoint Vern7 handles only, else nullptr
 };
 int adj_rows_f64(int N);
 cudaError_t launch_fwd_f64(const Shape64Host &, const Fwd64Host &, int solver, const Adapt64Host *adaptive_or_null, cudaStream_t);
 cudaError_t launch_adj_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *adaptive_or_null, cudaStream_t, int *rows_out);
+// discrete adjoint in fp64 (discrete_adjoint.cuh): solver 0 = Tsit5, 1 = Vern7; ad = adaptive Vern7 record or nullptr
+cudaError_t launch_adj_discrete_f64(const Shape64Host &, const Adj64Host &, int solver, const Adapt64Host *ad, cudaStream_t, int *rows_out);
 cudaError_t launch_reduce_f64(const double *partial, int nrows, int P1, double *grad, double *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // adaptive Tsit5 only
 cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);

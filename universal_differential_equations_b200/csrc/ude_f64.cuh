@@ -49,6 +49,7 @@ struct Adapt64 {
     int n_save, max_steps;
     double *tgrid;   // [max_steps+1][N]
     int *nacc;       // [N]
+    double *hstep;   // [max_steps][N] step sizes of the accepted steps (Vern7 record for the discrete adjoint) or nullptr
 };
 
 constexpr int MAXW = 64;   // max layer width
@@ -185,9 +186,9 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd64 p)
 }
 
 // Vern7 fixed-step forward solve (solve(prob, Vern7(); saveat, adaptive = false)): 9 stages per step, no FSAL.
-// Forward only: the interpolating adjoint of a Vern7 solve needs Vern7's lazy 7th-order dense output, whose
-// coefficients are not recoverable from the reference's artefacts (SURVEY.md App. A.3), so the adjoint call on a
-// Vern7 handle is rejected with B200UDE_EUNSUPPORTED.
+// Vern7's lazy 7th-order dense output is not available (SURVEY.md App. A.3): the interpolating adjoint of a Vern7 solve
+// runs over a Tsit5 re-solve (b200ude.cu).  With p.ustep set (discrete-adjoint handles) u_n of every step is recorded
+// for the discrete adjoint (discrete_adjoint.cuh), which recomputes the stages from it.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(Fwd64 p)
 {
@@ -200,6 +201,8 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(Fwd64 p)
     double u[MAXD], g[MAXD], k[9][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     for (int c = 0; c < D; ++c) p.out[(size_t)c * N + n] = u[c];
+    if (p.ustep)
+        for (int c = 0; c < D; ++c) p.ustep[(size_t)c * N + n] = u[c];
     int isave = 1;
     for (int s = 0; s < p.n_steps; ++s) {
         model_rhs(u, k[0]);
@@ -221,6 +224,8 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(Fwd64 p)
                 if (Vern7::b(j) != 0.0) acc = fma((double)Vern7::b(j), k[j][c], acc);
             u[c] = fma(dt, acc, u[c]);
         }
+        if (p.ustep)
+            for (int c = 0; c < D; ++c) p.ustep[((size_t)(s + 1) * D + c) * N + n] = u[c];
         if ((s + 1) % p.save_every == 0) {
             for (int c = 0; c < D; ++c) p.out[((size_t)isave * D + c) * N + n] = u[c];
             ++isave;
@@ -531,8 +536,9 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd64 p, Ada
 
 // Vern7 with OrdinaryDiffEq's PI controller (abstol / reltol; scenario_1.jl:84-85, seir_exposure.jl:138-139).  The lazy
 // 7th-order interpolant is not available (see above), so the save times are step end points (tstops), exactly as the
-// oracle's Vern7 path does; the step sequence between save points is the controller's own.  Forward solve only: no dense
-// record is written (the gradient of a Vern7 solve is taken over a Tsit5 re-solve, see b200ude.cu).
+// oracle's Vern7 path does; the step sequence between save points is the controller's own.  No dense record is written
+// (the interpolating adjoint of a Vern7 solve is taken over a Tsit5 re-solve, see b200ude.cu).  With ap.tgrid set
+// (discrete-adjoint handles) every accepted step is recorded -- tgrid, ustep, hstep, nacc -- for the discrete adjoint.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(Fwd64 p, Adapt64 ap)
 {
@@ -544,9 +550,14 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(Fwd64 
     const double t0 = ap.t0, t1 = ap.t0 + ap.save_dt * (double)(ap.n_save - 1);
     const double abstol = ap.abstol, reltol = ap.reltol;
     const double gamma = 0.9, qmin = 0.2, qmax = 10.0, beta1 = 7.0 / 70.0, beta2 = 2.0 / 35.0;   // order 7
+    const bool record = ap.tgrid != nullptr;
     double u[MAXD], un[MAXD], g[MAXD], k[10][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     for (int c = 0; c < D; ++c) p.out[(size_t)c * N + n] = u[c];
+    if (record) {
+        ap.tgrid[n] = t0;
+        for (int c = 0; c < D; ++c) p.ustep[(size_t)c * N + n] = u[c];
+    }
     model_rhs(u, k[0]);
     double dt;
     {
@@ -610,6 +621,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(Fwd64 
         double q = fmin(fmax(q11 / pow(qold, beta2) / gamma, 1.0 / qmax), 1.0 / qmin);
         if (EEst <= 1.0) {
             if (nacc >= ap.max_steps) { bad = 2; break; }
+            if (record) ap.hstep[(size_t)nacc * N + n] = h;
             ++nacc;
             if (clipped) {
                 for (int c = 0; c < D; ++c) p.out[((size_t)isave * D + c) * N + n] = un[c];
@@ -620,6 +632,10 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(Fwd64 
             if (!clipped || h >= dt) dt = h / q;
             else dt = fmax(dt, h / q);
             t = clipped ? tend : t + h;
+            if (record) {
+                ap.tgrid[(size_t)nacc * N + n] = t;
+                for (int c = 0; c < D; ++c) p.ustep[((size_t)nacc * D + c) * N + n] = un[c];
+            }
             for (int c = 0; c < D; ++c) u[c] = un[c];
             have_k1 = false;   // not FSAL
         } else {

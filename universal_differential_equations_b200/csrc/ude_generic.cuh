@@ -3,7 +3,8 @@
 // Functional coverage for every recognised UDE form whose chain has no specialised kernel: any dense chain
 // with widths <= 64 and <= 5 layers, models LV (0/1/2 trainable rates), SEIR (7 states, chain on
 // [S/N, I, D/N], SEIR_exposure/seir_exposure.jl:117-130), SEIR_NODE (the script's black-box baseline, :52-64) and NODE;
-// also the adaptive Tsit5 forward / replay-adjoint kernels, the Vern7 forward kernels and the runtime-shape Fisher-KPP kernels.  One trajectory per thread, weights read
+// also the adaptive Tsit5 forward / replay-adjoint kernels, the Vern7 forward kernels and the runtime-shape Fisher-KPP kernels
+// (the discrete adjoint of the Tsit5 / Vern7 solves is in discrete_adjoint.cuh).  One trajectory per thread, weights read
 // from the constant bank with runtime indices, activations in per-thread local arrays, Tsit5 forward with
 // dense output and the interpolating adjoint exactly as in the specialised kernels.  The ensemble-summed
 // parameter gradient is reduced deterministically: every contribution is summed over the warp's lanes with a
@@ -162,9 +163,9 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(FwdParams p)
 }
 
 // Vern7 fixed-step forward solve (solve(prob, Vern7(); saveat, adaptive = false)): 9 stages per step, no FSAL.
-// Forward only: the interpolating adjoint of a Vern7 solve needs Vern7's lazy 7th-order dense output, whose
-// coefficients are not recoverable from the reference's artefacts (SURVEY.md App. A.3), so the adjoint call on a
-// Vern7 handle is rejected with B200UDE_EUNSUPPORTED.
+// Vern7's lazy 7th-order dense output is not available (SURVEY.md App. A.3): the interpolating adjoint of a Vern7 solve
+// runs over a Tsit5 re-solve (b200ude.cu).  With p.ustep set (discrete-adjoint handles) u_n of every step is recorded
+// for the discrete adjoint (discrete_adjoint.cuh), which recomputes the stages from it.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
 {
@@ -177,6 +178,8 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
     float u[MAXD], g[MAXD], k[9][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     for (int c = 0; c < D; ++c) p.out[(size_t)c * N + n] = u[c];
+    if (p.ustep)
+        for (int c = 0; c < D; ++c) p.ustep[(size_t)c * N + n] = u[c];
     int isave = 1;
     for (int s = 0; s < p.n_steps; ++s) {
         model_rhs(u, k[0]);
@@ -198,6 +201,8 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
                 if (Vern7::b(j) != 0.0) acc = fmaf((float)Vern7::b(j), k[j][c], acc);
             u[c] = fmaf(dt, acc, u[c]);
         }
+        if (p.ustep)
+            for (int c = 0; c < D; ++c) p.ustep[((size_t)(s + 1) * D + c) * N + n] = u[c];
         if ((s + 1) % p.save_every == 0) {
             for (int c = 0; c < D; ++c) p.out[((size_t)isave * D + c) * N + n] = u[c];
             ++isave;
@@ -379,6 +384,7 @@ struct AdaptParams {
     int n_save, max_steps;
     float *tgrid;     // [max_steps+1][N]
     int *nacc;        // [N]
+    float *hstep;     // [max_steps][N] step sizes of the accepted steps (Vern7 record for the discrete adjoint) or nullptr
 };
 
 __device__ __forceinline__ void tsit5_bw_rt(float Th, float *bw)
@@ -514,8 +520,9 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
 
 // Vern7 with OrdinaryDiffEq's PI controller (abstol / reltol; scenario_1.jl:84-85, seir_exposure.jl:138-139).  The lazy
 // 7th-order interpolant is not available (see above), so the save times are step end points (tstops), exactly as the
-// oracle's Vern7 path does; the step sequence between save points is the controller's own.  Forward solve only: no dense
-// record is written (the gradient of a Vern7 solve is taken over a Tsit5 re-solve, see b200ude.cu).
+// oracle's Vern7 path does; the step sequence between save points is the controller's own.  No dense record is written
+// (the interpolating adjoint of a Vern7 solve is taken over a Tsit5 re-solve, see b200ude.cu).  With ap.tgrid set
+// (discrete-adjoint handles) every accepted step is recorded -- tgrid, ustep, hstep, nacc -- for the discrete adjoint.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(FwdParams p, AdaptParams ap)
 {
@@ -527,9 +534,14 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(FwdPar
     const float t0 = ap.t0, t1 = ap.t0 + ap.save_dt * (float)(ap.n_save - 1);
     const float abstol = ap.abstol, reltol = ap.reltol;
     const float gamma = 0.9f, qmin = 0.2f, qmax = 10.0f, beta1 = 7.0f / 70.0f, beta2 = 2.0f / 35.0f;   // order 7
+    const bool record = ap.tgrid != nullptr;
     float u[MAXD], un[MAXD], g[MAXD], k[10][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     for (int c = 0; c < D; ++c) p.out[(size_t)c * N + n] = u[c];
+    if (record) {
+        ap.tgrid[n] = t0;
+        for (int c = 0; c < D; ++c) p.ustep[(size_t)c * N + n] = u[c];
+    }
     model_rhs(u, k[0]);
     float dt;
     {
@@ -593,6 +605,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(FwdPar
         float q = fminf(fmaxf(q11 / powf(qold, beta2) / gamma, 1.0f / qmax), 1.0f / qmin);
         if (EEst <= 1.0f) {
             if (nacc >= ap.max_steps) { bad = 2; break; }
+            if (record) ap.hstep[(size_t)nacc * N + n] = h;
             ++nacc;
             if (clipped) {
                 for (int c = 0; c < D; ++c) p.out[((size_t)isave * D + c) * N + n] = un[c];
@@ -603,6 +616,10 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(FwdPar
             if (!clipped || h >= dt) dt = h / q;
             else dt = fmaxf(dt, h / q);
             t = clipped ? tend : t + h;
+            if (record) {
+                ap.tgrid[(size_t)nacc * N + n] = t;
+                for (int c = 0; c < D; ++c) p.ustep[((size_t)nacc * D + c) * N + n] = un[c];
+            }
             for (int c = 0; c < D; ++c) u[c] = un[c];
             have_k1 = false;   // not FSAL
         } else {

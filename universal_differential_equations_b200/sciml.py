@@ -289,10 +289,13 @@ class InterpolatingAdjoint:
 
 
 class ForwardDiffSensitivity:
-    """ForwardDiffSensitivity() of the LV scripts (scenario_1.jl:86, scenario_2.jl:108, hudson_bay.jl:102): the exact
-    derivative of the discrete solver scheme.  The reference pushes dual numbers through the solver (cost O(P) forward
-    solves); here the same quantity comes from reverse accumulation through the Tsit5 stages (one backward sweep,
-    B200UDE_DISCRETE_ADJOINT).  Fixed-step Tsit5 on the LV chains."""
+    """ForwardDiffSensitivity() of the LV scripts (scenario_1.jl:84-87, scenario_2.jl:106-108, hudson_bay.jl:99-102): the exact
+    derivative of the discrete solver scheme with the accepted step sequence held fixed.  The reference pushes dual numbers
+    through the solver (cost O(P) forward solves); here the same quantity comes from reverse accumulation through the stages
+    of every recorded step (one backward sweep, B200UDE_DISCRETE_ADJOINT).  Fixed-step Tsit5, fixed-step Vern7 and adaptive
+    Vern7 (save times are tstops) on the LV / SEIR / SEIR_NODE / NODE forms, float32 and float64; so
+    concrete_solve(prob, Vern7(), p=theta, saveat, abstol=1e-6, reltol=1e-6, sensealg=ForwardDiffSensitivity()) differentiates
+    the Vern7 solve itself.  Not available: adaptive Tsit5, the Fisher-KPP UPDE, RKC2."""
     code = _lib.DISCRETE_ADJOINT
 
 
