@@ -718,7 +718,8 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     // warp-collective mma.sync family (lv32_wm.cuh): -1 = chosen per call from the ensemble size, 0 = off, 1 = always
     h->var.fwd_wm = env_int("B200UDE_FWD_WM", -1);
     h->var.adj_wm = env_int("B200UDE_ADJ_WM", -1);
-    h->var.wm_groups = env_int("B200UDE_WM_G", 1);
+    h->var.wm_groups = env_int("B200UDE_WM_G", 0);
+    h->var.wm_g2_min = h->sm_count * 4 * 2 * 32;   // 33 792 on 132 SMs
     h->var.wm_rows = env_int("B200UDE_WM_R", 0);
     h->var.wm_r1_max = env_int("B200UDE_WM_R1_MAX", h->sm_count * 4 * 8);   // one 8-trajectory warp per scheduler: 4224 on 132 SMs
     h->wm_fwd_max = (size_t)env_int("B200UDE_WM_FWD_MAX", 1 << 26);

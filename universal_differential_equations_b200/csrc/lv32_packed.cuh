@@ -53,8 +53,37 @@ __device__ __forceinline__ float2 tanh2(float2 x)
     }
 }
 
-constexpr float TANH_ZMAX = 30.0f;   // clamp of 2 log2(e) x: tanh is 1.0f beyond x = 9.02, and (2^30 + 1)^4 < FLT_MAX
-// tanh of four values with one reciprocal (TM = 0); tanh.approx (TM = 1)
+// tanh(x) from z = 2 log2(e) x - 1: tanh(x) = 1 - 2 / (1 + 2^(z + 1)) = 1 - 1 / d with d = 2^z + 1/2.  The warp-collective
+// kernels fold the affine map into the weights and biases that produce x, so their tanh takes z directly.
+constexpr float TANH_K = 2.885390081777927f;   // 2 log2(e)
+constexpr float TANH_ZMAX = 29.0f;   // clamp of z: tanh is 1.0f beyond x = 9.02, and (2^29 + 1/2)^4 < FLT_MAX
+// tanh of four values given as z (see above) with one reciprocal (TM = 0); tanh.approx (TM = 1).  22 instructions for TM = 0:
+// 4 FMNMX, 4 MUFU.EX2, 4 FADD, 5 FMUL, 1 MUFU.RCP, 4 FFMA.
+template <int TM>
+__device__ __forceinline__ void tanh_quad_z(float2 &a, float2 &b)
+{
+    if constexpr (TM == 1) {
+        constexpr float ik = 1.0f / TANH_K;
+        a = make_float2(tanh_dev<1>(fmaf(a.x, ik, ik)), tanh_dev<1>(fmaf(a.y, ik, ik)));
+        b = make_float2(tanh_dev<1>(fmaf(b.x, ik, ik)), tanh_dev<1>(fmaf(b.y, ik, ik)));
+    } else {
+        // the clamp keeps a NaN (min.NaN), so a non-finite pre-activation reaches the state and its status word
+        auto ex2c = [](float z) {
+            float e;
+            asm("{\n\t.reg .f32 t;\n\tmin.NaN.f32 t, %1, %2;\n\tex2.approx.ftz.f32 %0, t;\n\t}" : "=f"(e) : "f"(z), "f"(TANH_ZMAX));
+            return e;
+        };
+        float2 ea = make_float2(ex2c(a.x), ex2c(a.y)), eb = make_float2(ex2c(b.x), ex2c(b.y));
+        const float2 da = add2(ea, bc(0.5f)), db = add2(eb, bc(0.5f));   // (1 + e^{2x}) / 2 in [1/2, 2^29 + 1/2]
+        const float2 pp = mul2(da, db);
+        float r;
+        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(pp.x * pp.y));
+        const float2 ip = make_float2(r * pp.y, r * pp.x);   // 1 / (da.x db.x), 1 / (da.y db.y)
+        a = fma2(make_float2(-ip.x, -ip.y), db, bc(1.0f));   // 1 - 1 / da
+        b = fma2(make_float2(-ip.x, -ip.y), da, bc(1.0f));
+    }
+}
+// tanh of four values
 template <int TM>
 __device__ __forceinline__ void tanh_quad(float2 &a, float2 &b)
 {
@@ -62,22 +91,9 @@ __device__ __forceinline__ void tanh_quad(float2 &a, float2 &b)
         a = make_float2(tanh_dev<1>(a.x), tanh_dev<1>(a.y));
         b = make_float2(tanh_dev<1>(b.x), tanh_dev<1>(b.y));
     } else {
-        float2 za = mul2(a, bc(2.885390081777927f)), zb = mul2(b, bc(2.885390081777927f));
-        za.x = fminf(za.x, TANH_ZMAX); za.y = fminf(za.y, TANH_ZMAX);
-        zb.x = fminf(zb.x, TANH_ZMAX); zb.y = fminf(zb.y, TANH_ZMAX);
-        float2 ea, eb;
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ea.x) : "f"(za.x));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ea.y) : "f"(za.y));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(eb.x) : "f"(zb.x));
-        asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(eb.y) : "f"(zb.y));
-        const float2 da = add2(ea, bc(1.0f)), db = add2(eb, bc(1.0f));   // 1 + e^{2x} in [1, 2^30 + 1]
-        const float2 pp = mul2(da, db);
-        float r;
-        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(pp.x * pp.y));
-        const float2 ip = make_float2(r * pp.y, r * pp.x);   // 1 / (da.x db.x), 1 / (da.y db.y)
-        const float2 ia = mul2(ip, db), ib = mul2(ip, da);   // 1 / da, 1 / db
-        a = fma2(bc(-2.0f), ia, bc(1.0f));
-        b = fma2(bc(-2.0f), ib, bc(1.0f));
+        a = fma2(a, bc(TANH_K), bc(-1.0f));
+        b = fma2(b, bc(TANH_K), bc(-1.0f));
+        tanh_quad_z<0>(a, b);
     }
 }
 

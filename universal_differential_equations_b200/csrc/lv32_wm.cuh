@@ -14,7 +14,8 @@
 //     which leaves every lane with the ONE (trajectory, component) pair it owns: the Runge-Kutta state, the stage
 //     derivatives and the adjoint state are kept once per (trajectory, component), not once per lane;
 //   * tanh = 1 - 2 / (1 + 2^(2 log2(e) x)) with ONE reciprocal per four values (Montgomery's batched inversion: the MUFU
-//     pipe -- 16 lanes/clk/SM -- is the scarcest unit of this path): 1.25 MUFU per tanh instead of 2;
+//     pipe -- 16 lanes/clk/SM -- is the scarcest unit of this path): 1.25 MUFU per tanh instead of 2; the affine map to the
+//     exponent is folded into the staged weights (tanh_quad_z);
 //   * adjoint: the ensemble-summed dW2 += q2^T h1 (K = the group's 16 trajectories) is a third 3xTF32 mma.sync product whose
 //     operands are transposed through a per-warp shared-memory tile; thin-layer gradients are per-lane register sums reduced
 //     once at the end of the kernel.
@@ -36,14 +37,18 @@ namespace wm {
 constexpr int WS = 40;    // row stride (floats) of the staged W2 and of the transpose tiles: conflict-free fragment accesses
 constexpr int WSH = 24;   // row stride (32-bit words) of the fp16 copy of W2: 16 words per output unit + 8 padding -> conflict-free LDS.64
 
+// The chain forward computes the pre-activations as z = 2 log2(e) (W x + b) - 1, the argument of tanh_quad_z: layers 1 and 2
+// are staged with that scale and shift folded in (w1a, w1b, b1, b2 and the fp16 copy of W2), which saves the multiply per
+// tanh.  The VJP's weights (W1 in SmemT, W2^T, W3) are staged unscaled.
 struct __align__(16) SmemT {                // adjoint only: operand of W2^T q2, fp16 pairs over the contraction index j
     uint32_t w2t_hi[32 * WSH], w2t_lo[32 * WSH];   // word (i, s, tig, b) = (W2[16 s + 8 b + 2 tig][i], W2[.. + 1][i])
+    float w1a[32], w1b[32];               // W1[f][0], W1[f][1], unscaled
     float w3max;                          // max |W3|: bound of the cotangent rows (scaling of the fp16 product)
 };
 struct __align__(16) SmemW {
-    uint32_t w2h_hi[32 * WSH], w2h_lo[32 * WSH];   // W2[j][.] as fp16 pairs in B-fragment order of mma.m16n8k16 (gemm32h): hi + lo split
-    float w1a[32], w1b[32], b1[32];       // W1[f][0], W1[f][1], b1[f]
-    float b2[32], w3a[32], w3b[32];       // b2[j], W3[0][j], W3[1][j]
+    uint32_t w2h_hi[32 * WSH], w2h_lo[32 * WSH];   // k W2[j][.] as fp16 pairs in B-fragment order of mma.m16n8k16 (gemm32h): hi + lo split
+    float w1a[32], w1b[32], b1[32];       // k W1[f][0], k W1[f][1], k b1[f] - 1   (k = 2 log2(e))
+    float b2[32], w3a[32], w3b[32];       // k b2[j] - 1, W3[0][j], W3[1][j]
     float b3[4];
 };
 
@@ -80,16 +85,20 @@ __device__ __forceinline__ void stage_weights(const float *__restrict__ theta, f
     for (int e = tid; e < 32 * 16; e += nthreads) {
         const int a = e >> 4, r = e & 15, s_ = r >> 3, tg = (r >> 1) & 3, b = r & 1;
         const int c0 = 16 * s_ + 8 * b + 2 * tg;
-        // forward copy: word (j = a, s, tig, b) = (W2[j][c0], W2[j][c0 + 1])
-        pack(raw[OFF_W2 + c0 * 32 + a], raw[OFF_W2 + (c0 + 1) * 32 + a], w.w2h_hi[a * WSH + r], w.w2h_lo[a * WSH + r]);
+        // forward copy: word (j = a, s, tig, b) = k (W2[j][c0], W2[j][c0 + 1])
+        pack(TANH_K * raw[OFF_W2 + c0 * 32 + a], TANH_K * raw[OFF_W2 + (c0 + 1) * 32 + a], w.w2h_hi[a * WSH + r], w.w2h_lo[a * WSH + r]);
         // transposed copy: word (i = a, s, tig, b) = (W2[c0][i], W2[c0 + 1][i])
         if (t) pack(raw[OFF_W2 + a * 32 + c0], raw[OFF_W2 + a * 32 + c0 + 1], t->w2t_hi[a * WSH + r], t->w2t_lo[a * WSH + r]);
     }
     for (int f = tid; f < 32; f += nthreads) {
-        w.w1a[f] = raw[OFF_W1 + f];
-        w.w1b[f] = raw[OFF_W1 + H + f];
-        w.b1[f] = raw[OFF_B1 + f];
-        w.b2[f] = raw[OFF_B2 + f];
+        w.w1a[f] = TANH_K * raw[OFF_W1 + f];
+        w.w1b[f] = TANH_K * raw[OFF_W1 + H + f];
+        w.b1[f] = fmaf(TANH_K, raw[OFF_B1 + f], -1.0f);
+        w.b2[f] = fmaf(TANH_K, raw[OFF_B2 + f], -1.0f);
+        if (t) {
+            t->w1a[f] = raw[OFF_W1 + f];
+            t->w1b[f] = raw[OFF_W1 + H + f];
+        }
         w.w3a[f] = raw[OFF_W3 + 2 * f];
         w.w3b[f] = raw[OFF_W3 + 2 * f + 1];
     }
@@ -179,8 +188,8 @@ __device__ __forceinline__ void layer1(const SmemW &w, const Lane &L, const floa
     for (int g = 0; g < G; ++g)
 #pragma unroll
         for (int r = 0; r < R; ++r) {
-            tanh_quad<TM>(h[g][r][0], h[g][r][1]);
-            tanh_quad<TM>(h[g][r][2], h[g][r][3]);
+            tanh_quad_z<TM>(h[g][r][0], h[g][r][1]);
+            tanh_quad_z<TM>(h[g][r][2], h[g][r][3]);
         }
 }
 
@@ -200,8 +209,9 @@ __device__ __forceinline__ void split_h2(float2 v, uint32_t &hi, uint32_t &lo)
 }
 // d[g][nt] += A[g] B (B fragments from a staged fp16 copy of W2 or W2^T) as a 2-way-split fp16 product (hi hi + lo hi + hi lo:
 // 22-bit operands, fp32 accumulate): half the tensor-pipe time of 3xTF32.  For operands bounded like the tanh outputs
-// (|a| <= 1; the cotangent rows are scaled into that range by the caller) and weights below 65504 (beyond that the fp16
-// copy is inf and the trajectory's status word reports the non-finite result).  A = a[g][r][q]: the D-fragment layout is
+// (|a| <= 1; the cotangent rows are scaled into that range by the caller) and weights below 65504 in the staged copy: the
+// forward copy holds 2 log2(e) W2, so |W2| >= ~22 700 there, |W2| >= 65504 in the W2^T copy (beyond that the fp16 copy is
+// inf, the product NaN, and the trajectory's status word reports the non-finite result).  A = a[g][r][q]: the D-fragment layout is
 // the A-fragment layout under the k permutation (k = 2 tig, 2 tig + 1 <-> units 16 s + 2 tig, + 1; k + 8 <-> units + 8).
 template <int G, int R>
 __device__ __forceinline__ void gemm32h(const uint32_t *__restrict__ bhi, const uint32_t *__restrict__ blo, const Lane &L,
@@ -264,8 +274,8 @@ __device__ __forceinline__ void rhs_wm(const SmemW *wp, float pc, const float (&
             float2 v[4];
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) v[nt] = make_float2(d[g][nt][2 * r], d[g][nt][2 * r + 1]);
-            tanh_quad<TM>(v[0], v[1]);
-            tanh_quad<TM>(v[2], v[3]);
+            tanh_quad_z<TM>(v[0], v[1]);
+            tanh_quad_z<TM>(v[2], v[3]);
             float2 s0 = bc(0.0f), s1 = bc(0.0f);
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) {
@@ -296,7 +306,7 @@ struct Consts {
 
 // ---- forward: fixed-step Tsit5, WPC warps per CTA, G groups of 8 R trajectories per warp -------------------------------
 template <int TM, int G, int R, int WPC>
-__global__ void __launch_bounds__(32 * WPC) forward_kernel(FwdParams p, Consts cs)
+__global__ void __launch_bounds__(32 * WPC, 32 / (WPC * G)) forward_kernel(FwdParams p, Consts cs)
 {
     __shared__ SmemW w;
     extern __shared__ __align__(16) unsigned char s_raw[];
@@ -308,7 +318,7 @@ __global__ void __launch_bounds__(32 * WPC) forward_kernel(FwdParams p, Consts c
     const float dt = p.dt;
     bool live[G];
     size_t idx[G];   // comp * N + n
-    float u[G], k[G][7];
+    float u[G], k[G][6];
 #pragma unroll
     for (int g = 0; g < G; ++g) {
         const long n = (long)(wg * G + g) * (8 * R) + L.fg + (R == 2 ? 8 * L.rsel : 0);
@@ -316,7 +326,7 @@ __global__ void __launch_bounds__(32 * WPC) forward_kernel(FwdParams p, Consts c
         idx[g] = (size_t)L.comp * N + (size_t)(n < (long)N ? n : (long)N - 1);   // padding lanes shadow the last trajectory; stores masked
         u[g] = __ldg(p.u0 + idx[g]);
 #pragma unroll
-        for (int j = 0; j < 7; ++j) k[g][j] = 0.0f;
+        for (int j = 0; j < 6; ++j) k[g][j] = 0.0f;
     }
     auto store = [&](float *base, int row, const float (&v)[G]) {
 #pragma unroll
@@ -330,41 +340,24 @@ __global__ void __launch_bounds__(32 * WPC) forward_kernel(FwdParams p, Consts c
     for (int s = 0; s < p.n_steps; ++s) {
 #pragma unroll 1
         for (int i = (s == 0 ? 0 : 1); i < 7; ++i) {
+            // stage argument from the uniform row a[i][.] (zero beyond the stage's own coefficients: the same sum, in the
+            // same order, as the unrolled stage), the new derivative into its slot by selects: no jump table per stage
             float gv[G];
 #pragma unroll
             for (int g = 0; g < G; ++g) {
                 float a = 0.0f;
-#define B200UDE_WM_COMB(I)                                                                          \
-    case I: {                                                                                       \
-        _Pragma("unroll") for (int j = 0; j < I; ++j) if (Tsit5::a(I, j) != 0.0) a = fmaf((float)Tsit5::a(I, j), k[g][j], a); \
-    } break;
-                switch (i) {
-                    B200UDE_WM_COMB(1)
-                    B200UDE_WM_COMB(2)
-                    B200UDE_WM_COMB(3)
-                    B200UDE_WM_COMB(4)
-                    B200UDE_WM_COMB(5)
-                    B200UDE_WM_COMB(6)
-                default: break;
-                }
-#undef B200UDE_WM_COMB
+#pragma unroll
+                for (int j = 0; j < 6; ++j) a = fmaf(c_a[i][j], k[g][j], a);
                 gv[g] = fmaf(dt, a, u[g]);
-                if (i == 6) u[g] = gv[g];   // stage 7's argument is u_{n+1} (row 7 = b, FSAL)
+                u[g] = i == 6 ? gv[g] : u[g];   // stage 7's argument is u_{n+1} (row 7 = b, FSAL)
             }
             float kk[G];
             rhs_wm<TM, G, R>(&w, pc, gv, kk);
+            const int slot = i == 6 ? 0 : i;   // k_7(s) = k_1(s+1) (FSAL)
 #pragma unroll
-            for (int g = 0; g < G; ++g) {
-                switch (i) {
-                case 0: k[g][0] = kk[g]; break;
-                case 1: k[g][1] = kk[g]; break;
-                case 2: k[g][2] = kk[g]; break;
-                case 3: k[g][3] = kk[g]; break;
-                case 4: k[g][4] = kk[g]; break;
-                case 5: k[g][5] = kk[g]; break;
-                default: k[g][6] = kk[g]; break;
-                }
-            }
+            for (int g = 0; g < G; ++g)
+#pragma unroll
+                for (int j = 0; j < 6; ++j) k[g][j] = slot == j ? kk[g] : k[g][j];
             store(p.dense, s * 6 + i, kk);   // row (s+1)*6 for i = 6: k_7(s) = k_1(s+1)
         }
         store(p.ustep, s + 1, u);
@@ -372,8 +365,6 @@ __global__ void __launch_bounds__(32 * WPC) forward_kernel(FwdParams p, Consts c
             store(p.out, isave, u);
             ++isave;
         }
-#pragma unroll
-        for (int g = 0; g < G; ++g) k[g][0] = k[g][6];
     }
     if (p.status) {
 #pragma unroll
@@ -476,8 +467,8 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
             float2 v[4];
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) v[nt] = make_float2(d[0][nt][2 * r], d[0][nt][2 * r + 1]);
-            tanh_quad<TM>(v[0], v[1]);
-            tanh_quad<TM>(v[2], v[3]);
+            tanh_quad_z<TM>(v[0], v[1]);
+            tanh_quad_z<TM>(v[2], v[3]);
             const float2 s0 = bc(sg[r][0]), s1 = bc(sg[r][1]);
             const uint32_t eb = (__float_as_uint(wt.w3max * (fabsf(sg[r][0]) + fabsf(sg[r][1]))) >> 23) & 0xFFu;   // biased exponent of B_t
             const float2 sc2 = bc(__uint_as_float((254u - eb) << 23));
@@ -537,8 +528,8 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
                 const float2 hh = h1[0][r][nt];
                 const float2 om = mul2(fma2(make_float2(-hh.x, -hh.y), hh, bc(1.0f)), unscale[r]);
                 const float2 q1 = mul2(make_float2(e[0][nt][2 * r], e[0][nt][2 * r + 1]), om);
-                s0 = fma2(lds2(w.w1a + 8 * nt + 2 * L.tig), q1, s0);
-                s1 = fma2(lds2(w.w1b + 8 * nt + 2 * L.tig), q1, s1);
+                s0 = fma2(lds2(wt.w1a + 8 * nt + 2 * L.tig), q1, s0);
+                s1 = fma2(lds2(wt.w1b + 8 * nt + 2 * L.tig), q1, s1);
                 gB1[nt] = add2(gB1[nt], q1);
                 gW1a[nt] = fma2(q1, x0, gW1a[nt]);
                 gW1b[nt] = fma2(q1, x1, gW1b[nt]);

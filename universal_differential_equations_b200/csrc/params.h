@@ -53,7 +53,8 @@ struct Variant {
     int discrete = 0;    // 1: discrete adjoint (exact gradient of the fixed-step scheme) instead of the interpolating adjoint
     int fwd_wm = 0;      // 1: warp-collective mma.sync forward kernel (lv32_wm.cuh)
     int adj_wm = 0;      // 1: warp-collective mma.sync adjoint kernel
-    int wm_groups = 1;   // groups per warp in the warp-collective forward kernel (1 or 2)
+    int wm_groups = 0;   // groups per warp in the warp-collective forward kernel: 1, 2, or 0 = by ensemble size (>= wm_g2_min -> 2)
+    int wm_g2_min = 0;   // two groups per warp once that still leaves two warps per scheduler (SMs x 4 x 2 x 32; b200ude_create)
     int wm_rows = 0;     // trajectories per group / 8: 1, 2, or 0 = by ensemble size (<= wm_r1_max -> 1)
     int wm_r1_max = 0;      // 8 trajectories per warp while that still leaves one warp per scheduler (SMs x 4 x 8; b200ude_create)
 };
