@@ -100,7 +100,11 @@ extern "C" {
 #define B200UDE_DEVICE 1
 
 /* flags */
-#define B200UDE_FLAG_APPROX_TANH 1u /* tanh.approx.f32 (2^-11 rel. error) instead of the ex2/rcp form */
+#define B200UDE_FLAG_APPROX_TANH 1u /* tanh.approx.f32 (2^-11 rel. error) instead of the ex2/rcp form.  Honoured by the kernels
+                                       of the LV 2-32-32-2 chain (warp-collective, tensor-core, packed, adaptive), of the SEIR
+                                       3-64-64-1 chain (fixed-step Tsit5, Vern7, adaptive) and of the Fisher-KPP 1-16-16-1 chain
+                                       (Tsit5, RKC2).  The LV 2-5-5-5-2, runtime-shape and fp64 kernels ignore it: their results
+                                       are bitwise those without the flag. */
 
 /* per-trajectory status words written by b200ude_forward */
 #define B200UDE_TRAJ_OK 0

@@ -710,8 +710,6 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (d->solver == B200UDE_RKC2) rkc2_tables(d->n_stages, &h->rkc);
     // tuning knobs for experiments (defaults are the measured-best variant, see DESIGN.md)
     h->var.fwd_smem = env_int("B200UDE_FWD_SMEM", 0);
-    h->var.fwd_T = env_int("B200UDE_FWD_T", 1) == 2 ? 2 : 1;
-    h->var.adj_smem = env_int("B200UDE_ADJ_SMEM", 0);
     // default: tensor-core (3xTF32 mma.sync) kernels; B200UDE_FWD_TC=0 / B200UDE_ADJ_TC=0 select the packed CUDA-core kernels
     h->var.fwd_tc = env_int("B200UDE_FWD_TC", 1);
     h->var.adj_tc = env_int("B200UDE_ADJ_TC", 2);   // 2: gradient GEMM on mma.sync (3xTF32), 1: on the FMA pipe

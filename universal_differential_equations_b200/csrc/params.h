@@ -44,9 +44,7 @@ struct ConstTables {
 };
 
 struct Variant {
-    int fwd_smem = 0;    // 0: constant-bank weights, 1: shared-memory (TMA-staged) weights
-    int fwd_T = 1;       // trajectories per thread in the forward kernel
-    int adj_smem = 0;
+    int fwd_smem = 0;    // packed LV32 forward: 0 = constant-bank weights, 1 = shared-memory weights
     int approx_tanh = 0;
     int fwd_tc = 0;      // 1: tensor-core (3xTF32 mma.sync) forward kernel
     int adj_tc = 0;      // 1: tensor-core (3xTF32 mma.sync) adjoint kernel, FFMA gradient GEMM; 2: mma.sync gradient GEMM
