@@ -56,8 +56,9 @@ extern "C" {
 #define B200UDE_F32 0
 #define B200UDE_F64 1 /* double precision: EVERY device array of the calls (theta, u0, out, data, dL_dout, grad_theta, grad_u0, loss) is
                         * double.  Runtime-shape kernels for the LV / SEIR / NODE forms, Tsit5 and Vern7, fixed step and adaptive,
-                        * and for the Fisher-KPP UPDE with adaptive Tsit5 (fixed-step Fisher-KPP is fp32 only); interpolating
-                        * adjoint, and the discrete adjoint of fixed-step Tsit5 / Vern7 and adaptive Vern7 -- the precision the reference's scenario 1 / 2, SEIR and Fisher-KPP scripts run in (Float64).  Entry points: create / set_params / get_params / forward / adjoint / adjoint_l2;
+                        * and for the Fisher-KPP UPDE with adaptive Tsit5, or adaptive Vern7 with the discrete adjoint (fixed-step
+                        * Fisher-KPP is fp32 only); interpolating adjoint, and the discrete adjoint of fixed-step Tsit5 / Vern7 and
+                        * adaptive Vern7 -- the precision the reference's scenario 1 / 2, SEIR and Fisher-KPP scripts run in (Float64).  Entry points: create / set_params / get_params / forward / adjoint / adjoint_l2;
                         * the host-buffer, ADAM and peer entry points return B200UDE_EUNSUPPORTED for such handles. */
 
 /* model kinds: the UDE right-hand sides of the reference */
@@ -91,9 +92,10 @@ extern "C" {
                                            accumulation through the stages of every step: the quantity ForwardDiffSensitivity()
                                            computes in forward mode (scenario_1.jl:84-87, scenario_2.jl:106-108, hudson_bay.jl:99-102).
                                            Fixed-step Tsit5, fixed-step Vern7 and adaptive Vern7 (save times are tstops) on the
-                                           LV / SEIR / SEIR_NODE / NODE forms, fp32 and fp64; the fused L2 reads the recorded
-                                           step-end states, so the loss reported is that of the solve itself.  Not for adaptive
-                                           Tsit5 (its saveat values come from the interpolant), the Fisher-KPP UPDE or RKC2. */
+                                           LV / SEIR / SEIR_NODE / NODE forms, and adaptive Vern7 on the Fisher-KPP UPDE
+                                           (scenario_3.jl:121-126), fp32 and fp64; the fused L2 reads the recorded step-end
+                                           states, so the loss reported is that of the solve itself.  Not for adaptive Tsit5 (its
+                                           saveat values come from the interpolant), fixed-step Fisher-KPP or RKC2. */
 
 /* memory space of a pointer argument */
 #define B200UDE_HOST 0
@@ -149,8 +151,9 @@ typedef struct b200ude_desc {
     uint32_t flags;
     int32_t adaptive;   /* 0: fixed step dt (adaptive = false). 1: Tsit5 with OrdinaryDiffEq's PI controller, abstol / reltol;
                            saveat = t0 + i*save_every*dt, i = 0..n_steps/save_every (dt only defines the save grid).
-                           LV / SEIR / NODE forms (Tsit5 or Vern7) and the Fisher-KPP UPDE (Tsit5; its error norm is taken over the
-                           whole grid, as OrdinaryDiffEq's default norm over the state vector), fp32 and fp64 */
+                           LV / SEIR / NODE forms (Tsit5 or Vern7) and the Fisher-KPP UPDE (Tsit5, or Vern7 with the discrete
+                           adjoint; its error norm is taken over the whole grid, as OrdinaryDiffEq's default norm over the state
+                           vector), fp32 and fp64 */
     int32_t max_steps;  /* adaptive: capacity of ACCEPTED steps per trajectory (status 2 when exceeded) */
     int32_t n_stages;   /* B200UDE_RKC2: stages per step (2..64); choose dt * spectral_radius <= 0.65 n_stages^2.  0 otherwise */
 } b200ude_desc;

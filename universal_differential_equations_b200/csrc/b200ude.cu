@@ -31,7 +31,8 @@ thread_local std::string g_create_error;
 //   K_GENERIC  any LV / SEIR / SEIR_NODE / NODE form with chain widths <= 64 and <= 5 layers (k_generic.cu): functional
 //            coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7, the adaptive path of untuned chains and
 //            the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh)
-//   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126)
+//   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126); also
+//            adaptive Tsit5 (fkpp_adaptive.cuh) and adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
 //   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
 //   K_FKPP16   Fisher-KPP UPDE with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu)                BASELINE config 4
 enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_F64 };
@@ -271,7 +272,8 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
         FwdParams p;
         p.u0 = u0; p.out = out; p.ustep = h->d_ustep; p.dense = nullptr; p.status = status; p.theta = h->d_theta;
         p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
-        if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
+        if (h->kid == K_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7(h->gen, h->tab, p, h->ag, st));   // adaptive only (b200ude_create)
+        else if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
         else CUDA_TRY(h, launch_fwd_vern7(h->gen, h->tab, p, st));
         h->last_out = out;
         h->N = N;
@@ -339,6 +341,12 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
         CUDA_TRY(h, launch_adj_discrete(h->gen, h->tab, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &h->ag : nullptr, st, &grid));
         if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
         else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
+    if (h->var.discrete && h->kid == K_FKPP) {
+        // discrete adjoint of an adaptive Vern7 Fisher-KPP solve (grid-per-CTA kernels); adaptive, so never peer (refused above)
+        CUDA_TRY(h, launch_adj_fkpp_vern7(h->gen, h->tab, p, h->ag, st, &grid));
+        CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
         return B200UDE_OK;
     }
     if (h->adaptive) {
@@ -507,7 +515,8 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
         // discrete adjoint: u_n of every (accepted) step recorded (as in fp32)
         Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
         const Adapt64Host a = adapt64(h);
-        CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
+        if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7_f64(h->sh64, p, a, st));   // adaptive only (b200ude_create)
+        else CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
         h->q_last_out = out;
         h->N = N;
         h->have_forward = true;
@@ -550,7 +559,8 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
     int rows = 0;
     if (h->var.discrete) {   // fixed-step Tsit5 / Vern7, adaptive Vern7 (b200ude_create); the fused L2 reads the recorded step-end states
         const Adapt64Host a = adapt64(h);
-        CUDA_TRY(h, launch_adj_discrete_f64(h->sh64, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &a : nullptr, st, &rows));
+        if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_adj_fkpp_vern7_f64(h->sh64, p, a, st, &rows));
+        else CUDA_TRY(h, launch_adj_discrete_f64(h->sh64, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &a : nullptr, st, &rows));
         CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
         return B200UDE_OK;
     }
@@ -606,13 +616,16 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     KernelId kid = pick_kernel(*d);
     const bool want64 = d->dtype == B200UDE_F64;
     const bool disc = d->sensealg == B200UDE_DISCRETE_ADJOINT;
-    // discrete adjoint: the tuned LV kernels (fixed-step Tsit5 on 2-32-32-2 / 2-5-5-5-2, fp32) and the runtime-shape kernels of
-    // discrete_adjoint.cuh.  Adaptive Tsit5 saves through its free interpolant, which an exact discrete adjoint would also have to
-    // differentiate; Fisher-KPP and RKC2 have no such kernels.
-    if (disc && (d->model == B200UDE_MODEL_FKPP || d->solver == B200UDE_RKC2 || (d->adaptive && d->solver == B200UDE_TSIT5)))
+    // discrete adjoint: the tuned LV kernels (fixed-step Tsit5 on 2-32-32-2 / 2-5-5-5-2, fp32), the runtime-shape kernels of
+    // discrete_adjoint.cuh and, for the Fisher-KPP UPDE, the grid-per-CTA adaptive Vern7 kernels of fkpp_vern7_discrete.cuh.
+    // Adaptive Tsit5 saves through its free interpolant, which an exact discrete adjoint would also have to differentiate;
+    // fixed-step Fisher-KPP and RKC2 have no such kernels.
+    const bool fkpp_v7 = d->model == B200UDE_MODEL_FKPP && d->adaptive && d->solver == B200UDE_VERN7;
+    if (disc && ((d->model == B200UDE_MODEL_FKPP && !fkpp_v7) || d->solver == B200UDE_RKC2 || (d->adaptive && d->solver == B200UDE_TSIT5)))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: the discrete adjoint (ForwardDiffSensitivity) has kernels for fixed-step Tsit5 and for fixed-step or adaptive Vern7 on the "
-                    "LV / SEIR / SEIR_NODE / NODE forms (chain widths <= 64), fp32 and fp64; not for adaptive Tsit5, the Fisher-KPP UPDE or RKC2");
+                    "LV / SEIR / SEIR_NODE / NODE forms (chain widths <= 64), and for adaptive Vern7 on the Fisher-KPP UPDE, fp32 and fp64; "
+                    "not for adaptive Tsit5, fixed-step Fisher-KPP or RKC2");
     if (want64) {
         // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_f64.cuh): LV / SEIR / NODE forms, Tsit5 and Vern7,
         // fixed step and adaptive, interpolating or discrete adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
@@ -620,16 +633,18 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: B200UDE_F64 kernels exist for the LV / SEIR / NODE forms (chain widths <= 64), Tsit5 / Vern7, and the Fisher-KPP UPDE "
                         "with adaptive Tsit5 and the interpolating adjoint");
-        if (d->model == B200UDE_MODEL_FKPP && (!d->adaptive || d->solver != B200UDE_TSIT5))
+        if (d->model == B200UDE_MODEL_FKPP && (!d->adaptive || !(d->solver == B200UDE_TSIT5 || (fkpp_v7 && disc))))
             return fail(nullptr, B200UDE_EUNSUPPORTED,
-                        "create: B200UDE_F64 Fisher-KPP runs adaptive Tsit5 only (adaptive = 1, solver = B200UDE_TSIT5); fixed-step Fisher-KPP is fp32");
+                        "create: B200UDE_F64 Fisher-KPP runs adaptive Tsit5 (interpolating adjoint) and adaptive Vern7 with the discrete adjoint "
+                        "only; fixed-step Fisher-KPP is fp32");
         if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1))
             return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
         kid = K_F64;
     }
     if (!want64 && d->solver == B200UDE_VERN7) {
-        if (!generic_ok(*d) || d->model == B200UDE_MODEL_FKPP)
-            return fail(nullptr, B200UDE_EUNSUPPORTED, "create: Vern7 kernels exist for the LV / SEIR / NODE forms only");
+        if (!generic_ok(*d) || (d->model == B200UDE_MODEL_FKPP && !(fkpp_v7 && disc)))
+            return fail(nullptr, B200UDE_EUNSUPPORTED,
+                        "create: Vern7 kernels exist for the LV / SEIR / NODE forms, and for the Fisher-KPP UPDE adaptive with the discrete adjoint");
         // fixed-step Vern7 of the SEIR 3-64-64-1 chain runs on the tensor-core kernels (and so does the Tsit5 re-solve its
         // adjoint uses); every other Vern7 configuration on the runtime-shape kernels
         // (the discrete adjoint of a Vern7 solve runs on the runtime-shape kernels only)
@@ -641,9 +656,11 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         if (!generic_ok(*d))
             return fail(nullptr, B200UDE_EUNSUPPORTED, "create: adaptive stepping is implemented for the LV / SEIR / NODE forms and the Fisher-KPP UPDE (chain widths <= 64)");
         if (d->model == B200UDE_MODEL_FKPP) {
-            // Fisher-KPP: runtime-shape grid-per-CTA kernels (fkpp_adaptive.cuh), the tuned 1-16-16-1 chain included
-            if (d->solver != B200UDE_TSIT5)
-                return fail(nullptr, B200UDE_EUNSUPPORTED, "create: adaptive stepping of the Fisher-KPP UPDE is implemented for Tsit5 only");
+            // Fisher-KPP: runtime-shape grid-per-CTA kernels (fkpp_adaptive.cuh; fkpp_vern7_discrete.cuh for Vern7 with the discrete
+            // adjoint), the tuned 1-16-16-1 chain included
+            if (d->solver != B200UDE_TSIT5 && !(fkpp_v7 && disc))
+                return fail(nullptr, B200UDE_EUNSUPPORTED,
+                            "create: adaptive stepping of the Fisher-KPP UPDE is implemented for Tsit5, and for Vern7 with the discrete adjoint");
             kid = K_FKPP;
         } else if (!((kid == K_LV32 || kid == K_SEIR64) && d->solver == B200UDE_TSIT5 && env_int("B200UDE_ADAPTIVE_TC", 1))) {
             // adaptive solves run on the runtime-shape kernels, except the headline chain (tensor-core kernels with CTA-uniform attempt loops)
@@ -658,7 +675,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     }
     // fixed-step Tsit5 with the discrete adjoint: LV 2-32-32-2 / 2-5-5-5-2 keep their tuned kernels, every other form runs on the
     // runtime-shape ones (the SEIR tensor-core kernels have no discrete adjoint)
-    if (disc && !want64 && kid != K_NONE && !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2)) kid = K_GENERIC;
+    if (disc && !want64 && kid != K_NONE && !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2 || kid == K_FKPP)) kid = K_GENERIC;
     if (kid == K_NONE)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: no sm_90a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");

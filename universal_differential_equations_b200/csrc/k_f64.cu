@@ -2,6 +2,7 @@
 #include "ude_f64.cuh"
 #include "fkpp_adaptive.cuh"
 #include "discrete_adjoint.cuh"
+#include "fkpp_vern7_discrete.cuh"
 
 #include "params.h"
 
@@ -175,6 +176,45 @@ cudaError_t launch_adj_fkpp_f64(const Shape64Host &s, const Adj64Host &p, const 
     q.ustep = p.ustep; q.dense = p.dense; q.tgrid = a.tgrid; q.nacc = a.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.t0 = a.t0; q.save_dt = a.save_dt;
     auto kern = fkpp_adapt::adjoint_kernel<FkppOps64>;
+    const size_t smem = fkpp_adapt::adj_smem(s.D, s.P, sizeof(double));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + q.tpc - 1) / q.tpc;
+    *rows_out = grid * (th / 32);
+    kern<<<grid, th, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+// ---- Fisher-KPP, adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh in fp64) ----
+cudaError_t launch_fwd_fkpp_vern7_f64(const Shape64Host &s, const Fwd64Host &p, const Adapt64Host &a, cudaStream_t st)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    fkpp_vern7::Fwd<double> q;
+    int th;
+    fkpp_adapt::cta_geometry(s.D, &q.tpc, &th);
+    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.hstep = a.hstep; q.status = p.status; q.tgrid = a.tgrid; q.nacc = a.nacc;
+    q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.max_steps = a.max_steps;
+    q.t0 = a.t0; q.save_dt = a.save_dt; q.abstol = a.abstol; q.reltol = a.reltol;
+    auto kern = fkpp_vern7::vern7_forward_kernel<FkppOps64>;
+    const size_t smem = fkpp_adapt::fwd_smem(s.D, sizeof(double));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<(p.N + q.tpc - 1) / q.tpc, th, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adj_fkpp_vern7_f64(const Shape64Host &s, const Adj64Host &p, const Adapt64Host &a, cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    fkpp_vern7::Adj<double> q;
+    int th;
+    fkpp_adapt::cta_geometry(s.D, &q.tpc, &th);
+    q.ustep = p.ustep; q.hstep = a.hstep; q.tgrid = a.tgrid; q.nacc = a.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.fused_l2 = p.fused_l2; q.t0 = a.t0; q.save_dt = a.save_dt;
+    q.margin = 5e-13;   // half the clipping margin of the forward
+    auto kern = fkpp_vern7::discrete_adjoint_kernel<FkppOps64>;
     const size_t smem = fkpp_adapt::adj_smem(s.D, s.P, sizeof(double));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

@@ -2,6 +2,7 @@
 #include "ude_generic.cuh"
 #include "fkpp_adaptive.cuh"
 #include "discrete_adjoint.cuh"
+#include "fkpp_vern7_discrete.cuh"
 
 #include <algorithm>
 
@@ -292,6 +293,49 @@ cudaError_t launch_adj_fkpp_adaptive(const GenericShape &gs, const ConstTables &
     q.ustep = p.ustep; q.dense = p.dense; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.t0 = ag.t0; q.save_dt = ag.save_dt;
     auto kern = fkpp_adapt::adjoint_kernel<FkppOps32>;
+    const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + q.tpc - 1) / q.tpc;
+    *rows_out = grid * (th / 32);
+    kern<<<grid, th, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+// ---- Fisher-KPP, adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh in fp32) ----
+cudaError_t launch_fwd_fkpp_vern7(const GenericShape &gs, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(gs, st);
+    if (e != cudaSuccess) return e;
+    fkpp_vern7::Fwd<float> q;
+    int th;
+    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
+    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.hstep = ag.hstep; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
+    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
+    q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
+    auto kern = fkpp_vern7::vern7_forward_kernel<FkppOps32>;
+    const size_t smem = fkpp_adapt::fwd_smem(gs.D, sizeof(float));
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<(p.N + q.tpc - 1) / q.tpc, th, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adj_fkpp_vern7(const GenericShape &gs, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag, cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(gs, st);
+    if (e != cudaSuccess) return e;
+    fkpp_vern7::Adj<float> q;
+    int th;
+    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
+    q.ustep = p.ustep; q.hstep = ag.hstep; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.fused_l2 = p.fused_l2; q.t0 = ag.t0; q.save_dt = ag.save_dt;
+    q.margin = 5e-7f;   // half the clipping margin of the forward
+    auto kern = fkpp_vern7::discrete_adjoint_kernel<FkppOps32>;
     const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

@@ -138,6 +138,10 @@ int adj_rows_fkpp(int N, int Nx);
 cudaError_t launch_fwd_fkpp_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
 cudaError_t launch_adj_fkpp_adaptive(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
 size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes);   // per-CTA dynamic shared memory of the larger of the two kernels
+// adaptive Vern7 of the Fisher-KPP UPDE with the discrete adjoint (fkpp_vern7_discrete.cuh): same geometry and shared memory as
+// adaptive Tsit5; the record is ustep / ag.tgrid / ag.hstep / ag.nacc; p.fused_l2 reads the recorded step-end states
+cudaError_t launch_fwd_fkpp_vern7(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
+cudaError_t launch_adj_fkpp_vern7(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
 cudaError_t launch_fwd_seir(const Variant &, const ConstTables &, const FwdParams &, cudaStream_t);
 cudaError_t launch_adj_seir(const Variant &, const ConstTables &, const AdjParams &, cudaStream_t, int *rows_out);
 cudaError_t launch_fwd_seir_vern7(const Variant &, const ConstTables &, const FwdParams &, cudaStream_t);
@@ -200,6 +204,8 @@ cudaError_t launch_adj_discrete_f64(const Shape64Host &, const Adj64Host &, int 
 cudaError_t launch_reduce_f64(const double *partial, int nrows, int P1, double *grad, double *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // adaptive Tsit5 only
 cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);
+cudaError_t launch_fwd_fkpp_vern7_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // discrete adjoint handles
+cudaError_t launch_adj_fkpp_vern7_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot_f64(const Shape64Host &, const double *out, const double *data, double *cot, double *loss, size_t N, int n_save, cudaStream_t);
 
 }  // namespace b200ude

@@ -293,10 +293,17 @@ class ForwardDiffSensitivity:
     derivative of the discrete solver scheme with the accepted step sequence held fixed.  The reference pushes dual numbers
     through the solver (cost O(P) forward solves); here the same quantity comes from reverse accumulation through the stages
     of every recorded step (one backward sweep, B200UDE_DISCRETE_ADJOINT).  Fixed-step Tsit5, fixed-step Vern7 and adaptive
-    Vern7 (save times are tstops) on the LV / SEIR / SEIR_NODE / NODE forms, float32 and float64; so
+    Vern7 (save times are tstops) on the LV / SEIR / SEIR_NODE / NODE forms, and adaptive Vern7 on the Fisher-KPP UPDE
+    (scenario_3.jl:121-126), float32 and float64; so
     concrete_solve(prob, Vern7(), p=theta, saveat, abstol=1e-6, reltol=1e-6, sensealg=ForwardDiffSensitivity()) differentiates
-    the Vern7 solve itself.  Not available: adaptive Tsit5, the Fisher-KPP UPDE, RKC2."""
+    the Vern7 solve itself.  Not available: adaptive Tsit5, fixed-step Fisher-KPP, RKC2.
+
+    `convert_tspan` is accepted and ignored: t and dt are never dual numbers here, which is what convert_tspan = false asks for
+    (and what the default does whenever tspan does not depend on the parameters)."""
     code = _lib.DISCRETE_ADJOINT
+
+    def __init__(self, convert_tspan=None):
+        self.convert_tspan = convert_tspan
 
 
 # --------------------------------------------------------------------------- engine
