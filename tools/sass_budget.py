@@ -3,7 +3,8 @@
 
 Compiles k_lv32_wm.cu for sm_90a with the library's flags into a temporary directory (or reads a given object), then for the
 default forward and adjoint instantiations at N = 65 536 prints the registers, the spill traffic, and the opcode counts of
-the stage loop: the smallest loop of the kernel that holds all of its tensor-core instructions.  Loops nested in the stage
+the stage loop: the smallest loop of the kernel that holds all of its tensor-core instructions (HMMA counted by shape:
+m16n8k16 fp16, m16n8k8 fp16, m16n8k8 TF32).  Loops nested in the stage
 loop, and the loop around it (the per-step code), are listed too.  Also counts the instructions of one tanh_quad_z.
 
     python tools/sass_budget.py                   # compile the working tree's k_lv32_wm.cu
@@ -30,8 +31,13 @@ __global__ void tanh_probe(float4 *p) { float4 v = *p; float2 a = make_float2(v.
   b200ude::lv32::tanh_quad_z<0>(a, b); *p = make_float4(a.x, a.y, b.x, b.y); }
 """
 
+# HMMA by shape: m16n8k16 fp16, m16n8k8 fp16, m16n8k8 TF32 (the two m16n8k8 differ only in the .TF32 suffix)
+HMMA_SHAPES = [("16816", "HMMA.16816"), ("1688", "HMMA.1688"), ("1688tf32", "HMMA.1688.F32.TF32")]
 COLUMNS = [
-    ("HMMA", ("HMMA",)),
+    ("16816", ()),
+    ("1688", ()),
+    ("1688tf32", ()),
+    ("MOVM", ("MOVM",)),
     ("MUFU", ("MUFU",)),
     ("FP32", ("FFMA", "FMUL", "FADD", "FMNMX")),
     ("FSEL", ("FSEL",)),
@@ -102,6 +108,9 @@ def count(insns, lo, hi):
         if lo <= addr <= hi:
             n += 1
             base = op.split(".")[0]
+            if base == "HMMA":
+                c[next(col for col, pre in reversed(HMMA_SHAPES) if op.startswith(pre))] += 1
+                continue
             for col, ops in COLUMNS:
                 if base in ops or op in ops or (col == "MOV" and op.startswith("IMAD.MOV")):
                     c[col] += 1

@@ -48,7 +48,7 @@ static cudaError_t launch_adj(const ConstTables &t, const AdjParams &p, int *row
     // single-warp CTAs, no register cap: a 168-register cap (3 warps per scheduler instead of 2) puts spill code in the stage loop
     constexpr int WPC = 1;
     auto kern = lv32::wm::adjoint_kernel<TM, R, WPC, 1>;
-    constexpr size_t smem = lv32::wm::RAW_FLOATS * 4 + sizeof(lv32::wm::WarpTiles<R>) * WPC;
+    constexpr size_t smem = lv32::wm::RAW_FLOATS * 4 + sizeof(lv32::wm::WarpTiles) * WPC;
     static PerDeviceOnce once;
     bool &attr_set = once.flag();
     if (!attr_set) {

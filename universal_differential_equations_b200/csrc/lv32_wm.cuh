@@ -16,9 +16,9 @@
 //   * tanh = 1 - 2 / (1 + 2^(2 log2(e) x)) with ONE reciprocal per four values (Montgomery's batched inversion: the MUFU
 //     pipe -- 16 lanes/clk/SM -- is the scarcest unit of this path): 1.25 MUFU per tanh instead of 2; the affine map to the
 //     exponent is folded into the staged weights (tanh_quad_z);
-//   * adjoint: the ensemble-summed dW2 += q2^T h1 (K = the group's 16 trajectories) is a third 3xTF32 mma.sync product whose
-//     operands are transposed through a per-warp shared-memory tile; thin-layer gradients are per-lane register sums reduced
-//     once at the end of the kernel.
+//   * adjoint: the ensemble-summed dW2 += q2^T h1 (K = the group's 16 trajectories) is a third 2-way-split fp16 mma.sync
+//     product whose operands are the hi/lo words of the two other products, transposed in registers (movmatrix) and scaled
+//     by one power of two per group; thin-layer gradients are per-lane register sums reduced once at the end of the kernel.
 // No CTA-wide barrier inside the time loops; theta is bulk-copied by the TMA from the handle's device copy
 // into shared memory once per CTA (no constant bank: handles are independent, any number can be in flight on a device).
 //
@@ -34,7 +34,6 @@ namespace b200ude {
 namespace lv32 {
 namespace wm {
 
-constexpr int WS = 40;    // row stride (floats) of the staged W2 and of the transpose tiles: conflict-free fragment accesses
 constexpr int WSH = 24;   // row stride (32-bit words) of the fp16 copy of W2: 16 words per output unit + 8 padding -> conflict-free LDS.64
 
 // The chain forward computes the pre-activations as z = 2 log2(e) (W x + b) - 1, the argument of tanh_quad_z: layers 1 and 2
@@ -113,17 +112,6 @@ __device__ __forceinline__ void stage_weights(const float *__restrict__ theta, f
 }
 
 __device__ __forceinline__ float2 lds2(const float *p) { return *reinterpret_cast<const float2 *>(p); }
-
-// D += A B, m16n8k8, TF32 inputs, fp32 accumulate
-__device__ __forceinline__ void mma8(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
-{
-    asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// 3xTF32 split of a run-time operand: the tensor core ignores the low 13 mantissa bits of a .tf32 register, so the value
-// itself is its own "hi" part (truncation) and only the residual has to be formed
-__device__ __forceinline__ uint32_t tf32_lo(float x) { return __float_as_uint(x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u)); }
 
 // per-lane constants of a warp
 struct Lane {
@@ -244,6 +232,58 @@ __device__ __forceinline__ void gemm32h(const uint32_t *__restrict__ bhi, const 
         }
     }
 }
+
+// The adjoint's operands split once and used twice: by gemm32h_w as rows, and transposed by the dW2 product.
+// hi[r][q] / lo[r][q] = split_h2(a[r][q]): one f16x2 word per lane of the 8 x 8 block (rows fg + 8 r, units 8 q + 2 tig, + 1)
+template <int R>
+__device__ __forceinline__ void split_rows(const float2 (&a)[R][4], uint32_t (&hi)[R][4], uint32_t (&lo)[R][4])
+{
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) split_h2(a[r][q], hi[r][q], lo[r][q]);
+}
+// gemm32h<1, R> on words made by split_rows: the same HMMA sequence, so the same result bit for bit
+template <int R>
+__device__ __forceinline__ void gemm32h_w(const uint32_t *__restrict__ bhi, const uint32_t *__restrict__ blo, const Lane &L,
+                                          const uint32_t (&hi)[R][4], const uint32_t (&lo)[R][4], float (&d)[4][4])
+{
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+        const uint32_t ah[4] = {hi[0][2 * s], R == 2 ? hi[R - 1][2 * s] : 0u, hi[0][2 * s + 1], R == 2 ? hi[R - 1][2 * s + 1] : 0u};
+        const uint32_t al[4] = {lo[0][2 * s], R == 2 ? lo[R - 1][2 * s] : 0u, lo[0][2 * s + 1], R == 2 ? lo[R - 1][2 * s + 1] : 0u};
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+            const uint2 bh = *reinterpret_cast<const uint2 *>(bhi + (8 * nt + L.fg) * WSH + 8 * s + 2 * L.tig);
+            const uint2 bl = *reinterpret_cast<const uint2 *>(blo + (8 * nt + L.fg) * WSH + 8 * s + 2 * L.tig);
+            mma16(d[nt], al, bh.x, bh.y);
+            mma16(d[nt], ah, bl.x, bl.y);
+            mma16(d[nt], ah, bh.x, bh.y);
+        }
+    }
+}
+// D += A B, m16n8k8, fp16 inputs, fp32 accumulate
+__device__ __forceinline__ void mma16k8(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t b0)
+{
+    asm("mma.sync.aligned.m16n8k8.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a0), "r"(a1), "r"(b0));
+}
+// transpose of the 8 x 8 fp16 block held one f16x2 word per lane: lane (fg, tig) gets (M[2 tig][fg], M[2 tig + 1][fg])
+__device__ __forceinline__ uint32_t movm_t(uint32_t x)
+{
+    uint32_t y;
+    asm("movmatrix.sync.aligned.m8n8.trans.b16 %0, %1;" : "=r"(y) : "r"(x));
+    return y;
+}
+__device__ __forceinline__ uint32_t hmul2(uint32_t a, uint32_t b)
+{
+    uint32_t y;
+    asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(y) : "r"(a), "r"(b));   // no .ftz: fp16 subnormals are kept
+    return y;
+}
+// 2^(e - 127) for a biased exponent e in [0, 255]: 0 for e = 0, inf for e = 255
+__device__ __forceinline__ float exp2_biased(int e) { return __uint_as_float((uint32_t)e << 23); }
 
 // UDE right-hand side for G groups; gv[g] = this lane's (row, component) of the stage argument, returns the same
 // component of du/dt.  du1 = p1 u1 + NN1(u), du2 = -p4 u2 + NN2(u)  (scenario_1.jl:71-72): pc = p1 / -p4 by component.
@@ -378,12 +418,26 @@ __global__ void __launch_bounds__(32 * WPC, 32 / (WPC * G)) forward_kernel(FwdPa
 }
 
 // ---- adjoint: interpolating adjoint on the fixed grid, one group of 8 R trajectories per warp --------------------------
-template <int R>
 struct __align__(16) WarpTiles {
-    float q2[8 * R * WS];   // q2[t][j] of the current stage (transposed operand of dW2 += q2^T h1)
-    float h1[8 * R * WS];   // h1[t][i]
     float sum[32 * 32];     // running dW2 sums of this warp, element k*32 + lane <-> accumulator register k of that lane
 };
+
+// Backward stage i scales the cotangent by dt b_i, so the dW2 operand of stage i exceeds that of stage 0 by up to
+// max |b_i| / |b_0| = 34.1 (times the change of lambda over the step): the smallest e with 2^e above that ratio (6) is the
+// headroom the first stage of a step leaves in the accumulator's scale, so that the later stages seldom have to rescale it
+constexpr int stage_headroom()
+{
+    double r = 0.0;
+    for (int i = 0; i < 6; ++i) {
+        const double q = Tsit5::b(i) / Tsit5::b(0);
+        r = q > r ? q : (-q > r ? -q : r);
+    }
+    int e = 0;
+    while ((double)(1 << e) <= r) ++e;
+    return e;
+}
+constexpr int STAGE_HEADROOM = stage_headroom();
+static_assert(STAGE_HEADROOM == 6, "Tsit5: max |b_i| / b_0 = 34.1");
 
 template <int TM, int R, int WPC, int MINB>
 __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Consts cs)
@@ -394,7 +448,7 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
     stage_weights(p.theta, reinterpret_cast<float *>(s_raw), w, &wt, threadIdx.x, 32 * WPC);
     const Lane L = make_lane();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    WarpTiles<R> &T = reinterpret_cast<WarpTiles<R> *>(s_raw + RAW_FLOATS * 4)[warp];
+    WarpTiles &T = reinterpret_cast<WarpTiles *>(s_raw + RAW_FLOATS * 4)[warp];
 #pragma unroll
     for (int q = 0; q < 32; ++q) T.sum[q * 32 + lane] = 0.0f;
     __syncwarp();
@@ -410,7 +464,10 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
     const float lw = L.comp ? cs.lw1 : cs.lw0;
     const float dt = p.dt, inv_dt = 1.0f / dt;
 
-    float macc[2][4][4];   // C fragments of dW2 (+)= q2^T h1: tile (mt, nt): rows j = 16 mt + fg (+8), columns i = 8 nt + 2 tig (+1)
+    // C fragments of 2^(127 - e_acc) dW2 (+)= q2^T h1: tile (mt, nt): rows j = 16 mt + fg (+8), columns i = 8 nt + 2 tig (+1).
+    // e_acc (warp-uniform) is the largest row exponent of the cotangent operand since the last flush
+    float macc[2][4][4];
+    int e_acc = 0;
 #pragma unroll
     for (int a = 0; a < 2; ++a)
 #pragma unroll
@@ -436,43 +493,63 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
         }
     };
 
-    // one backward stage: xo = own component of u(t), go = own component of the stage's lambda argument, sc = dt b_i
-    auto eval = [&](float xo, float go, float sc, float isc) -> float {
+    // one backward stage: xo = own component of u(t), go = own component of the stage's lambda argument, sc = dt b_i;
+    // first = the first stage since macc was flushed
+    auto eval = [&](float xo, float go, float sc, float isc, bool first) -> float {
         float x[1][R][2], sg[R][2];
         gather4<R>(L, xo, x[0]);
         const float sgo = lv * sc * go;
         gather4<R>(L, sgo, sg);
         gb3 += sgo;
+        // Every cotangent row q2[t][.] is scaled by a power of two into fp16's range for the W2^T q2 product (|q2[t][j]| <=
+        // max|W3| (|sg_t0| + |sg_t1|) =: B_t; scale 2^(127 - e_t), e_t = biased exponent of B_t, undone on the product -- both exact)
+        uint32_t eb[R];   // e_t
+#pragma unroll
+        for (int r = 0; r < R; ++r) eb[r] = (__float_as_uint(wt.w3max * (fabsf(sg[r][0]) + fabsf(sg[r][1]))) >> 23) & 0xFFu;
+        // dW2 += q2^T h1 (below) sums over rows, so the rows' scales become one per group: the words of row t are
+        // multiplied by 2^(e_t - e_acc) (exact down to fp16's subnormals; below them the error is at most 2^-24 B_max per
+        // element), e_acc >= every e_t since the last flush.  All maxima are over the integer exponents, so an inf/NaN row
+        // (255) poisons the sums as a non-finite q2 does.  Settled here, first in the stage, so that the rest is one block.
+        int e_max = (int)eb[0];
+        if constexpr (R == 2) e_max = max(e_max, (int)eb[1]);
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) e_max = max(e_max, __shfl_xor_sync(0xffffffffu, e_max, o));   // over fg: warp-uniform
+        if (first) {   // macc is zero; room for the larger b_i of the later stages, at most 2^127 for finite rows
+            e_acc = e_max == 255 ? 255 : min(e_max + STAGE_HEADROOM, 254);
+        } else if (e_max > e_acc) {   // above the step's scale so far: rare, lambda changes smoothly over a step
+            const float rs = exp2_biased(max(e_acc - e_max + 127, 0));
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) macc[mt][nt][c] *= rs;
+            e_acc = e_max;
+        }
         float2 h1[1][R][4];
         layer1<TM, 1, R>(w, L, x, h1);
-        // transposed operand of the gradient product: h1 rows
-        __syncwarp();
-#pragma unroll
-        for (int r = 0; r < R; ++r)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) *reinterpret_cast<float2 *>(&T.h1[(L.fg + 8 * r) * WS + 8 * q + 2 * L.tig]) = h1[0][r][q];
-        float d[1][4][4];
+        // h1 split once: A operand of the chain forward, (transposed) B operand of dW2
+        uint32_t h1hi[R][4], h1lo[R][4];
+        split_rows<R>(h1[0], h1hi, h1lo);
+        float d[4][4];
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
             const float2 bias = lds2(w.b2 + 8 * nt + 2 * L.tig);
-            d[0][nt][0] = bias.x; d[0][nt][1] = bias.y; d[0][nt][2] = bias.x; d[0][nt][3] = bias.y;
+            d[nt][0] = bias.x; d[nt][1] = bias.y; d[nt][2] = bias.x; d[nt][3] = bias.y;
         }
-        gemm32h<1, R>(w.w2h_hi, w.w2h_lo, L, h1, d);
-        // h2 = tanh(.), q2 = (W3^T sg) (1 - h2^2); dW3 += sg (x) h2, db2 += q2.  Every cotangent row is also scaled by a power
-        // of two into fp16's range for the W2^T q2 product (|q2[t][j]| <= max|W3| (|sg_t0| + |sg_t1|) =: B_t; scale 2^-e(B_t),
-        // undone on the product -- both exact)
-        float2 q2s[1][R][4], unscale[R];
+        gemm32h_w<R>(w.w2h_hi, w.w2h_lo, L, h1hi, h1lo, d);
+        // h2 = tanh(.), q2 = (W3^T sg) (1 - h2^2); dW3 += sg (x) h2, db2 += q2; the rows scaled by 2^(127 - e_t) (above)
+        float2 q2s[R][4], unscale[R];
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             float2 v[4];
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt) v[nt] = make_float2(d[0][nt][2 * r], d[0][nt][2 * r + 1]);
+            for (int nt = 0; nt < 4; ++nt) v[nt] = make_float2(d[nt][2 * r], d[nt][2 * r + 1]);
             tanh_quad_z<TM>(v[0], v[1]);
             tanh_quad_z<TM>(v[2], v[3]);
             const float2 s0 = bc(sg[r][0]), s1 = bc(sg[r][1]);
-            const uint32_t eb = (__float_as_uint(wt.w3max * (fabsf(sg[r][0]) + fabsf(sg[r][1]))) >> 23) & 0xFFu;   // biased exponent of B_t
-            const float2 sc2 = bc(__uint_as_float((254u - eb) << 23));
-            unscale[r] = bc(__uint_as_float(eb << 23));
+            const float2 sc2 = bc(__uint_as_float((254u - eb[r]) << 23));
+            unscale[r] = bc(__uint_as_float(eb[r] << 23));
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) {
                 const float2 w3a = lds2(w.w3a + 8 * nt + 2 * L.tig), w3b = lds2(w.w3b + 8 * nt + 2 * L.tig);
@@ -481,39 +558,46 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
                 const float2 t = fma2(w3b, s1, mul2(w3a, s0));
                 const float2 om = fma2(make_float2(-v[nt].x, -v[nt].y), v[nt], bc(1.0f));
                 const float2 q2 = mul2(t, om);
-                q2s[0][r][nt] = mul2(q2, sc2);
+                q2s[r][nt] = mul2(q2, sc2);
                 gB2[nt] = add2(gB2[nt], q2);
-                *reinterpret_cast<float2 *>(&T.q2[(L.fg + 8 * r) * WS + 8 * nt + 2 * L.tig]) = q2;
             }
         }
-        __syncwarp();
-        float e[1][4][4];
+        uint32_t q2hi[R][4], q2lo[R][4];
+        split_rows<R>(q2s, q2hi, q2lo);
+        float e[4][4];
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-            for (int c = 0; c < 4; ++c) e[0][nt][c] = 0.0f;
-        gemm32h<1, R>(wt.w2t_hi, wt.w2t_lo, L, q2s, e);
-        // dW2 += q2^T h1 : M = j (2 tiles), N = i (4 tiles), K = the group's trajectories (R k-steps of 8), 3xTF32
+            for (int c = 0; c < 4; ++c) e[nt][c] = 0.0f;
+        gemm32h_w<R>(wt.w2t_hi, wt.w2t_lo, L, q2hi, q2lo, e);
+        // dW2 += q2^T h1: M = j (2 tiles), N = i (4 tiles), K = the group's 8 R trajectories (m16n8k16 for R = 2, m16n8k8 for
+        // R = 1), 2-way split on the words of the two products above, each 8 x 8 block transposed by one movmatrix
+        uint32_t ah[2][2 * R], al[2][2 * R];   // A fragments of q2^T: (mt, 2 r + (nt & 1)) <- block (r, nt) of q2, nt >> 1 = mt
 #pragma unroll
-        for (int ks = 0; ks < R; ++ks) {
-            uint32_t ah[2][4], al[2][4];
-#pragma unroll
-            for (int mt = 0; mt < 2; ++mt) {
-                const float *b0 = T.q2 + (8 * ks + L.tig) * WS + 16 * mt + L.fg;
-                const float v[4] = {b0[0], b0[8], b0[4 * WS], b0[4 * WS + 8]};
-#pragma unroll
-                for (int c = 0; c < 4; ++c) { ah[mt][c] = __float_as_uint(v[c]); al[mt][c] = tf32_lo(v[c]); }
-            }
+        for (int r = 0; r < R; ++r) {
+            uint32_t m2;
+            asm("cvt.rn.f16x2.f32 %0, %1, %1;" : "=r"(m2) : "f"(exp2_biased(max((int)eb[r] - e_acc + 127, 0))));
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) {
-                const float *hb = T.h1 + (8 * ks + L.tig) * WS + 8 * nt + L.fg;
-                const float b0 = hb[0], b1 = hb[4 * WS];
-                const uint32_t bh0 = __float_as_uint(b0), bh1 = __float_as_uint(b1), bl0 = tf32_lo(b0), bl1 = tf32_lo(b1);
+                ah[nt >> 1][2 * r + (nt & 1)] = movm_t(hmul2(q2hi[r][nt], m2));
+                al[nt >> 1][2 * r + (nt & 1)] = movm_t(hmul2(q2lo[r][nt], m2));
+            }
+        }
 #pragma unroll
-                for (int mt = 0; mt < 2; ++mt) {
-                    mma8(macc[mt][nt], al[mt], bh0, bh1);
-                    mma8(macc[mt][nt], ah[mt], bl0, bl1);
-                    mma8(macc[mt][nt], ah[mt], bh0, bh1);
+        for (int nt = 0; nt < 4; ++nt) {
+            uint32_t bh[R], bl[R];   // B fragment of h1: k-step half r <- block (r, nt) of h1
+#pragma unroll
+            for (int r = 0; r < R; ++r) { bh[r] = movm_t(h1hi[r][nt]); bl[r] = movm_t(h1lo[r][nt]); }
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+                if constexpr (R == 2) {
+                    mma16(macc[mt][nt], al[mt], bh[0], bh[1]);
+                    mma16(macc[mt][nt], ah[mt], bl[0], bl[1]);
+                    mma16(macc[mt][nt], ah[mt], bh[0], bh[1]);
+                } else {
+                    mma16k8(macc[mt][nt], al[mt][0], al[mt][1], bh[0]);
+                    mma16k8(macc[mt][nt], ah[mt][0], ah[mt][1], bl[0]);
+                    mma16k8(macc[mt][nt], ah[mt][0], ah[mt][1], bh[0]);
                 }
             }
         }
@@ -527,7 +611,7 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
             for (int nt = 0; nt < 4; ++nt) {
                 const float2 hh = h1[0][r][nt];
                 const float2 om = mul2(fma2(make_float2(-hh.x, -hh.y), hh, bc(1.0f)), unscale[r]);
-                const float2 q1 = mul2(make_float2(e[0][nt][2 * r], e[0][nt][2 * r + 1]), om);
+                const float2 q1 = mul2(make_float2(e[nt][2 * r], e[nt][2 * r + 1]), om);
                 s0 = fma2(lds2(wt.w1a + 8 * nt + 2 * L.tig), q1, s0);
                 s1 = fma2(lds2(wt.w1b + 8 * nt + 2 * L.tig), q1, s1);
                 gB1[nt] = add2(gB1[nt], q1);
@@ -567,7 +651,7 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
             const float go = fmaf(dt, ga, lam);     // lambda argument of backward stage i
             if (stage == 5 && s > 0) load_step(s - 1);
             const float bi = c_a[6][stage];
-            const float kn = eval(xo, go, dt * bi, inv_dt * c_binv[stage]);
+            const float kn = eval(xo, go, dt * bi, inv_dt * c_binv[stage], stage == 0);
 #pragma unroll
             for (int j = 0; j < 6; ++j) kl[j] = (stage == j) ? kn : kl[j];
         }
@@ -577,7 +661,8 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
         lam = fmaf(dt, a, lam);
         if (s % p.save_every == 0) jump(s / p.save_every);
         // the tensor core adds into its accumulator with truncation: keep the chains one step long and add them into
-        // the running sums with round-to-nearest
+        // the running sums with round-to-nearest, undoing the step's scale 2^(127 - e_acc) (exact: a power of two)
+        const float us_acc = exp2_biased(e_acc);
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -585,7 +670,7 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
                     float &slot = T.sum[((mt * 4 + nt) * 4 + c) * 32 + lane];
-                    slot += macc[mt][nt][c];
+                    slot = fmaf(macc[mt][nt][c], us_acc, slot);
                     macc[mt][nt][c] = 0.0f;
                 }
     }
