@@ -302,8 +302,10 @@ int32_t b200ude_bsde_train_adam(b200ude_bsde_handle *h, const b200ude_adam *opt,
                                 void *loss_history, void *u0_history);
 /* device time of the last b200ude_bsde_train_adam call in ms (CUDA events on the handle's stream around all its iterations) */
 double b200ude_bsde_last_train_ms(const b200ude_bsde_handle *h);
-/* fp64 handles with widths <= 112 run fused sweeps (csrc/bsde.cu): ms[0..2] = device time of the forward sweep, the cotangent sweep
- * and the batched weight-gradient GEMMs of the last b200ude_bsde_loss_gradient call (CUDA events on the handle's stream) */
+/* fp64 handles with dim <= 110 and hidden <= 111 run fused sweeps (csrc/bsde.cu; the weight-gradient products on a fused kernel
+ * too when dim and hidden are both even, else on library GEMMs); other handles return B200UDE_EUNSUPPORTED.  ms[0..2] = device time
+ * of the forward sweep, the cotangent sweep and the batched weight-gradient GEMMs of the last b200ude_bsde_loss_gradient call
+ * (CUDA events on the handle's stream) */
 int32_t b200ude_bsde_last_sweep_ms(b200ude_bsde_handle *h, double *ms);
 /* one ADAM update with a caller-supplied DEVICE gradient [P] of the handle's dtype (multi-GPU: b200ude_bsde_loss_gradient on
  * every rank's path shard, all-reduce of the gradient, then this call on every rank) */

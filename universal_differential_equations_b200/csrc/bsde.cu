@@ -9,10 +9,11 @@
 // Here, for the script's family  mu = 0, sigma = s I, f = -lambda |z|^2, g(X) = log(a + b |X|^2)  (Hamilton-Jacobi-Bellman):
 //   * all paths of an iteration advance together; the networks work on [width x paths] column-major activations (a path = a column), so
 //     theta's vec(W) is already the operand of every layer product -- no repacking of the reference's parameter vector;
-//   * fp64 (BASELINE's config 5), widths <= 112: hand-written DMMA kernels -- a fused forward sweep (all layers and all steps in one
-//     launch, two warps per 8-path tile, weights streamed through a TMA slab ring, relu / Euler-Maruyama / residual on the fragments),
-//     a fused cotangent sweep and a fused weight-gradient kernel (see "fused fp64 sweeps" below); Brownian increments from a
-//     counter-based generator (Philox4x32-10 + Box-Muller) in a separate parallel pass;
+//   * fp64 (BASELINE's config 5), dim <= 110 and hidden <= 111 (the augmented rows [X; t; 1] and [h; 1] fit FT unit tiles): hand-written
+//     DMMA kernels -- a fused forward sweep (all layers and all steps in one launch, two warps per 8-path tile, weights streamed through
+//     a TMA slab ring, relu / Euler-Maruyama / residual on the fragments), a fused cotangent sweep and, when dim and hidden are both
+//     even, a fused weight-gradient kernel (see "fused fp64 sweeps" below; odd widths take library GEMMs for [dW | db]); Brownian
+//     increments from a counter-based generator (Philox4x32-10 + Box-Muller) in a separate parallel pass;
 //   * fp32, and wider networks: one library GEMM per layer (cuBLAS) with hand-written kernels between them (fused Euler-Maruyama
 //     with the increments regenerated in place, relu / masks, the loss and its cotangents);
 //   * the backward sweep is the exact reverse-mode derivative of the discretised solve (what Tracker computes through the SDE
@@ -926,7 +927,7 @@ struct b200ude_bsde_handle {
     //   C[k] [n_steps][hls][cap] = cotangents of hidden k
     void *IN = nullptr, *u = nullptr, *H[3] = {}, *Z = nullptr, *Zb = nullptr, *C[3] = {}, *r2 = nullptr, *ubar = nullptr, *ones = nullptr;
     int init_M = 0;   // the constant rows are laid out for this many paths
-    bool fused = false;       // fp64, widths <= 112: the fused DMMA sweeps instead of per-layer library GEMMs
+    bool fused = false;       // fp64, dim <= 110, hidden <= 111: the fused DMMA sweeps instead of per-layer library GEMMs
     void *packed = nullptr;   // zero-padded operand copies of the z network for the fused sweeps
     void *mask = nullptr;     // relu' bits of the hidden layers (fused sweeps)
     void *dW = nullptr;       // Brownian increments of the iteration (fused sweeps)
@@ -1338,7 +1339,7 @@ double b200ude_bsde_last_train_ms(const b200ude_bsde_handle *h) { return h ? (do
 int32_t b200ude_bsde_last_sweep_ms(b200ude_bsde_handle *h, double *ms)
 {
     if (!h || !ms) return B200UDE_EINVAL;
-    if (!h->fused) return bfail(h, B200UDE_EUNSUPPORTED, "bsde_last_sweep_ms: the handle runs on library GEMMs (fp32, or widths above 112)");
+    if (!h->fused) return bfail(h, B200UDE_EUNSUPPORTED, "bsde_last_sweep_ms: the handle runs on library GEMMs (fp32, dim > 110, hidden > 111 or B200UDE_BSDE_FUSED=0)");
     const int pairs[3][2] = {{0, 1}, {2, 3}, {3, 4}};
     for (int i = 0; i < 3; ++i) {
         float t = 0.0f;
