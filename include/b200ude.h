@@ -37,7 +37,9 @@
  *    can be in flight on a device.  The other kernel families read the active handle's theta and tables from the constant
  *    bank, so work of DIFFERENT handles of those kinds on one device must be stream-ordered (not concurrent).
  *  - the interpolating adjoint of a Vern7 handle runs over a Tsit5 re-solve from the same u0 with the same step / tolerances
- *    (Vern7's lazy dense output is not available): with the fused L2 entry point the reported loss is that of the re-solve.
+ *    by default, and an adaptive Vern7 solve treats the save times as tstops: with the fused L2 entry point the reported loss is that of the re-solve.  With B200UDE_FLAG_VERN7_DENSE
+ *    (below) it runs over the Vern7 solve's own lazy 7th-order dense output instead, and an adaptive Vern7 solve fills its
+ *    save times from that interpolant rather than stopping at them -- the call of seir_exposure.jl:137-141 as written.
  *    The discrete adjoint of a Vern7 handle differentiates the Vern7 solve itself.
  */
 #ifndef B200UDE_H
@@ -107,6 +109,18 @@ extern "C" {
                                        3-64-64-1 chain (fixed-step Tsit5, Vern7, adaptive) and of the Fisher-KPP 1-16-16-1 chain
                                        (Tsit5, RKC2).  The LV 2-5-5-5-2, runtime-shape and fp64 kernels ignore it: their results
                                        are bitwise those without the flag. */
+#define B200UDE_FLAG_VERN7_DENSE 2u /* Vern7 with its lazy 7th-order dense output (OrdinaryDiffEq's six extra stages and
+                                       interpolation polynomials), for solver = B200UDE_VERN7 with the interpolating adjoint on the
+                                       LV / SEIR / SEIR_NODE / NODE forms, fp32 and fp64, fixed step and adaptive:
+                                       - adaptive: the steps stop only at the end of tspan; a save time inside a step is evaluated
+                                         with the interpolant, one on a step end takes the step-end state (OrdinaryDiffEq's saveat);
+                                       - fixed step: saves at step ends as without the flag, so the forward output is the same;
+                                       - the interpolating adjoint runs over the Vern7 forward's own dense output (no Tsit5 re-solve):
+                                         b200ude_adjoint_l2 reports the loss of the states b200ude_forward returned.  With adaptive = 1
+                                         `out` must stay valid until the matching adjoint call (the fused L2 reads it).
+                                       Every such handle, the SEIR 3-64-64-1 chain included, runs on the runtime-shape kernels
+                                       (vern7_dense.cuh).  B200UDE_EUNSUPPORTED with the discrete adjoint, Tsit5, RKC2 or the
+                                       Fisher-KPP UPDE. */
 
 /* per-trajectory status words written by b200ude_forward */
 #define B200UDE_TRAJ_OK 0

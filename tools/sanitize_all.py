@@ -29,6 +29,10 @@ run("generic", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1)
 run("adaptive", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, adaptive=True, abstol=1e-5, reltol=1e-5, max_steps=200)
 run("vern7", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7())
 run("vern7-adaptive", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7(), adaptive=True, abstol=1e-5, reltol=1e-5, max_steps=200)
+# Vern7 dense output (vern7_dense.cuh): fixed-step adjoint, adaptive forward and replay adjoint
+run("vern7-dense", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7(dense=True))
+run("vern7-dense-adaptive", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, alg=ude.Vern7(dense=True), adaptive=True, abstol=1e-5,
+    reltol=1e-5, max_steps=200)
 # discrete adjoint (discrete_adjoint.cuh): fp32 through every entry point, fp64 through forward / adjoint_l2
 fd = ude.ForwardDiffSensitivity()
 run("generic-discrete", gen, glorot_theta((2, 7, 2), seed=3), u0, y, 0.1, 30, 1, sensealg=fd)

@@ -95,6 +95,7 @@ struct b200ude_handle {
     // on-device optimiser (b200ude_adam_*, b200ude_train_adam)
     float *d_u0_keep = nullptr, *d_aux_out = nullptr;   // Vern7: u0 of the last forward, saved states of the Tsit5 re-solve
     bool vern7_pending = false;
+    bool vern7_dense = false;   // B200UDE_FLAG_VERN7_DENSE: saveat and the interpolating adjoint through Vern7's own dense output
     float *d_adam_m = nullptr, *d_adam_v = nullptr, *d_train_out = nullptr;
     int *d_adam_t = nullptr;
     int adam_t = 0;   // host mirror of the step counter
@@ -267,12 +268,15 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
-    if (h->desc.solver == B200UDE_VERN7 && h->var.discrete) {
-        // discrete adjoint: the forward records u_n of every (accepted) step, which the adjoint recomputes the stages from
+    if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
+        // discrete adjoint, or the interpolating adjoint over Vern7's dense output: the forward records u_n of every (accepted)
+        // step, which the adjoint recomputes the stages from.  With the dense flag an adaptive solve saves through the
+        // interpolant; a fixed grid saves at step ends either way
         FwdParams p;
         p.u0 = u0; p.out = out; p.ustep = h->d_ustep; p.dense = nullptr; p.status = status; p.theta = h->d_theta;
         p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
         if (h->kid == K_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7(h->gen, h->tab, p, h->ag, st));   // adaptive only (b200ude_create)
+        else if (h->adaptive && h->vern7_dense) CUDA_TRY(h, launch_fwd_vern7_dense(h->gen, h->tab, p, h->ag, st));
         else if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
         else CUDA_TRY(h, launch_fwd_vern7(h->gen, h->tab, p, st));
         h->last_out = out;
@@ -336,6 +340,13 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
     p.dt = (float)h->desc.dt;
     cudaError_t e = cudaSuccess;
     int grid = 0;
+    if (h->vern7_dense) {
+        // interpolating adjoint over the Vern7 solve's own dense output; the fused L2 reads the states the forward returned
+        CUDA_TRY(h, launch_adj_vern7_dense(h->gen, h->tab, p, h->adaptive ? &h->ag : nullptr, h->last_out, st, &grid));
+        if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
+        else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
     if (h->var.discrete && h->kid == K_GENERIC) {
         // discrete adjoint of a runtime-shape Tsit5 / Vern7 solve over its recorded steps; the fused L2 reads the recorded step-end states
         CUDA_TRY(h, launch_adj_discrete(h->gen, h->tab, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &h->ag : nullptr, st, &grid));
@@ -511,11 +522,12 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
-    if (h->desc.solver == B200UDE_VERN7 && h->var.discrete) {
-        // discrete adjoint: u_n of every (accepted) step recorded (as in fp32)
+    if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
+        // discrete adjoint / Vern7 dense output: u_n of every (accepted) step recorded (as in fp32)
         Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
         const Adapt64Host a = adapt64(h);
         if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7_f64(h->sh64, p, a, st));   // adaptive only (b200ude_create)
+        else if (h->adaptive && h->vern7_dense) CUDA_TRY(h, launch_fwd_vern7_dense_f64(h->sh64, p, a, st));
         else CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
         h->q_last_out = out;
         h->N = N;
@@ -557,6 +569,12 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
     if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
     Adj64Host p{h->q_ustep, h->q_dense, cot, grad_u0, h->q_partial, (int)h->N, h->desc.n_steps, h->desc.save_every, l2 ? 1 : 0, h->desc.dt};
     int rows = 0;
+    if (h->vern7_dense) {   // interpolating adjoint over the Vern7 dense output; the fused L2 reads the states the forward returned
+        const Adapt64Host a = adapt64(h);
+        CUDA_TRY(h, launch_adj_vern7_dense_f64(h->sh64, p, h->adaptive ? &a : nullptr, h->q_last_out, st, &rows));
+        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
     if (h->var.discrete) {   // fixed-step Tsit5 / Vern7, adaptive Vern7 (b200ude_create); the fused L2 reads the recorded step-end states
         const Adapt64Host a = adapt64(h);
         if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_adj_fkpp_vern7_f64(h->sh64, p, a, st, &rows));
@@ -626,6 +644,13 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                     "create: the discrete adjoint (ForwardDiffSensitivity) has kernels for fixed-step Tsit5 and for fixed-step or adaptive Vern7 on the "
                     "LV / SEIR / SEIR_NODE / NODE forms (chain widths <= 64), and for adaptive Vern7 on the Fisher-KPP UPDE, fp32 and fp64; "
                     "not for adaptive Tsit5, fixed-step Fisher-KPP or RKC2");
+    // Vern7's lazy dense output (vern7_dense.cuh): saveat through the interpolant and the interpolating adjoint over it.  The
+    // discrete adjoint through an interpolated save would have to differentiate the extra stages: not built
+    const bool v7dense = (d->flags & B200UDE_FLAG_VERN7_DENSE) != 0;
+    if (v7dense && (d->solver != B200UDE_VERN7 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT || d->model == B200UDE_MODEL_FKPP))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_FLAG_VERN7_DENSE applies to Vern7 with the interpolating adjoint on the LV / SEIR / SEIR_NODE / NODE forms; "
+                    "not to the discrete adjoint, Tsit5, RKC2 or the Fisher-KPP UPDE");
     if (want64) {
         // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_f64.cuh): LV / SEIR / NODE forms, Tsit5 and Vern7,
         // fixed step and adaptive, interpolating or discrete adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
@@ -647,8 +672,8 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                         "create: Vern7 kernels exist for the LV / SEIR / NODE forms, and for the Fisher-KPP UPDE adaptive with the discrete adjoint");
         // fixed-step Vern7 of the SEIR 3-64-64-1 chain runs on the tensor-core kernels (and so does the Tsit5 re-solve its
         // adjoint uses); every other Vern7 configuration on the runtime-shape kernels
-        // (the discrete adjoint of a Vern7 solve runs on the runtime-shape kernels only)
-        if (disc || !(kid == K_SEIR64 && !d->adaptive && env_int("B200UDE_SEIR_VERN7_TC", 1))) kid = K_GENERIC;
+        // (the discrete adjoint of a Vern7 solve and the dense-output flag run on the runtime-shape kernels only)
+        if (disc || v7dense || !(kid == K_SEIR64 && !d->adaptive && env_int("B200UDE_SEIR_VERN7_TC", 1))) kid = K_GENERIC;
     }
     if (!want64 && d->adaptive) {
         if (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)
@@ -724,6 +749,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     }
     h->var.approx_tanh = (d->flags & B200UDE_FLAG_APPROX_TANH) ? 1 : 0;
     h->var.discrete = d->sensealg == B200UDE_DISCRETE_ADJOINT ? 1 : 0;
+    h->vern7_dense = v7dense;
     if (d->solver == B200UDE_RKC2) rkc2_tables(d->n_stages, &h->rkc);
     // tuning knobs for experiments (defaults are the measured-best variant, see DESIGN.md)
     h->var.fwd_smem = env_int("B200UDE_FWD_SMEM", 0);
@@ -744,8 +770,9 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         const size_t N64 = h->cap, D64 = (size_t)h->D;
         const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
         h->partial_blocks = (size_t)(d->model == B200UDE_MODEL_FKPP ? adj_rows_fkpp((int)N64, d->state_dim) : adj_rows_f64((int)N64));
-        // a discrete-adjoint Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead when adaptive
-        const bool disc_vern7 = disc && d->solver == B200UDE_VERN7;
+        // a discrete-adjoint or dense-output Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead
+        // when adaptive
+        const bool disc_vern7 = (disc && d->solver == B200UDE_VERN7) || v7dense;
         bool ok64 = dalloc(h, &h->q_theta, (size_t)h->P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D64 * N64) == cudaSuccess &&
                     (disc_vern7 || dalloc(h, &h->q_dense, (rec * 6 + 1) * D64 * N64) == cudaSuccess) &&
                     dalloc(h, &h->q_partial, h->partial_blocks * (size_t)(h->P + 1)) == cudaSuccess;
@@ -781,7 +808,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     ok = ok && dalloc(h, &h->d_theta, (size_t)((h->P + 3) / 4) * 4) == cudaSuccess;
     const size_t rec_steps = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;   // capacity of the step record
     ok = ok && dalloc(h, &h->d_ustep, (rec_steps + 1) * D * N) == cudaSuccess;
-    const bool disc_vern7 = disc && d->solver == B200UDE_VERN7;   // stages recomputed from u_n: no dense record
+    const bool disc_vern7 = (disc && d->solver == B200UDE_VERN7) || v7dense;   // stages recomputed from u_n: no dense record
     if (!disc_vern7) ok = ok && dalloc(h, &h->d_dense, (rec_steps * 6 + 1) * D * N) == cudaSuccess;
     if (h->adaptive) {
         if (disc_vern7) ok = ok && dalloc(h, &h->d_hstep, rec_steps * N) == cudaSuccess;

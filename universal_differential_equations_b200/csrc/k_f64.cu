@@ -3,6 +3,7 @@
 #include "fkpp_adaptive.cuh"
 #include "discrete_adjoint.cuh"
 #include "fkpp_vern7_discrete.cuh"
+#include "vern7_dense.cuh"
 
 #include "params.h"
 
@@ -117,6 +118,46 @@ cudaError_t launch_adj_discrete_f64(const Shape64Host &s, const Adj64Host &p, in
     q.margin = 5e-13;   // half the clipping margin of vern7_adaptive_forward_kernel
     auto kern = solver == 1 ? discrete::adjoint_kernel<DiscreteOps64, discrete::Vern7Scheme, F64_BLOCK>
                             : discrete::adjoint_kernel<DiscreteOps64, discrete::Tsit5Scheme, F64_BLOCK>;
+    const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + F64_BLOCK - 1) / F64_BLOCK;
+    *rows_out = grid * (F64_BLOCK / 32);
+    kern<<<grid, F64_BLOCK, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+// ---- Vern7 with its lazy dense output (vern7_dense.cuh in fp64) ----
+struct DenseOps64 : DiscreteOps64 {
+    static __device__ __forceinline__ void vjp(const double *u, const double *g, double sc, double lv, double *kl, double *gw, int lane)
+    {
+        f64::model_vjp(u, g, sc, lv, kl, gw, lane);
+    }
+};
+
+cudaError_t launch_fwd_vern7_dense_f64(const Shape64Host &s, const Fwd64Host &p, const Adapt64Host &a, cudaStream_t st)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    vern7_dense::Fwd<double> q;
+    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.tgrid = a.tgrid; q.hstep = a.hstep; q.nacc = a.nacc; q.status = p.status;
+    q.N = p.N; q.n_save = a.n_save; q.max_steps = a.max_steps;
+    q.t0 = a.t0; q.save_dt = a.save_dt; q.abstol = a.abstol; q.reltol = a.reltol;
+    vern7_dense::forward_kernel<DenseOps64, F64_BLOCK><<<(p.N + F64_BLOCK - 1) / F64_BLOCK, F64_BLOCK, 0, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adj_vern7_dense_f64(const Shape64Host &s, const Adj64Host &p, const Adapt64Host *ad, const double *saved, cudaStream_t st,
+                                       int *rows_out)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    vern7_dense::Adj<double> q;
+    q.ustep = p.ustep; q.tgrid = ad ? ad->tgrid : nullptr; q.hstep = ad ? ad->hstep : nullptr; q.nacc = ad ? ad->nacc : nullptr;
+    q.cot = p.cot; q.saved = saved; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
+    q.dt = p.dt; q.t0 = ad ? ad->t0 : 0.0; q.save_dt = ad ? ad->save_dt : 0.0;
+    auto kern = vern7_dense::adjoint_kernel<DenseOps64, F64_BLOCK>;
     const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

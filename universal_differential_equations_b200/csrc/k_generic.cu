@@ -3,6 +3,7 @@
 #include "fkpp_adaptive.cuh"
 #include "discrete_adjoint.cuh"
 #include "fkpp_vern7_discrete.cuh"
+#include "vern7_dense.cuh"
 
 #include <algorithm>
 
@@ -109,6 +110,50 @@ cudaError_t launch_adj_discrete(const GenericShape &g, const ConstTables &t, con
     q.margin = 5e-7f;   // half the clipping margin of vern7_adaptive_forward_kernel
     auto kern = solver == 1 ? discrete::adjoint_kernel<DiscreteOps32, discrete::Vern7Scheme, GEN_BLOCK>
                             : discrete::adjoint_kernel<DiscreteOps32, discrete::Tsit5Scheme, GEN_BLOCK>;
+    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
+    *rows_out = grid * (GEN_BLOCK / 32);
+    kern<<<grid, GEN_BLOCK, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+// ---- Vern7 with its lazy dense output (vern7_dense.cuh in fp32) ----
+struct DenseOps32 : DiscreteOps32 {
+    static __device__ __forceinline__ void vjp(const float *u, const float *g, float sc, float lv, float *kl, float *gw, int lane)
+    {
+        generic::model_vjp(u, g, sc, lv, kl, gw, lane);
+    }
+};
+
+cudaError_t launch_fwd_vern7_dense(const GenericShape &g, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(g, st);
+    if (e != cudaSuccess) return e;
+    vern7_dense::Fwd<float> q;
+    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.tgrid = ag.tgrid; q.hstep = ag.hstep; q.nacc = ag.nacc; q.status = p.status;
+    q.N = p.N; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
+    q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
+    vern7_dense::forward_kernel<DenseOps32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adj_vern7_dense(const GenericShape &g, const ConstTables &t, const AdjParams &p, const AdaptiveGrid *ag, const float *saved,
+                                   cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(g, st);
+    if (e != cudaSuccess) return e;
+    vern7_dense::Adj<float> q;
+    q.ustep = p.ustep; q.tgrid = ag ? ag->tgrid : nullptr; q.hstep = ag ? ag->hstep : nullptr; q.nacc = ag ? ag->nacc : nullptr;
+    q.cot = p.cot; q.saved = saved; q.grad_u0 = p.grad_u0; q.partial = p.partial;
+    q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
+    q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
+    auto kern = vern7_dense::adjoint_kernel<DenseOps32, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

@@ -129,6 +129,12 @@ cudaError_t launch_adj_adaptive(const GenericShape &, const ConstTables &, const
 // record, nullptr on a fixed grid.  Partial rows as adj_rows_generic.
 cudaError_t launch_adj_discrete(const GenericShape &, const ConstTables &, const AdjParams &, int solver, const AdaptiveGrid *ag,
                                 cudaStream_t, int *rows_out);
+// Vern7 with its lazy dense output (vern7_dense.cuh, B200UDE_FLAG_VERN7_DENSE): the adaptive forward saving through the interpolant
+// (record: p.ustep, ag.tgrid, ag.hstep, ag.nacc), and the interpolating adjoint over that dense output, ag = nullptr on a fixed grid
+// (record: p.ustep of launch_fwd_vern7).  saved: the forward's `out`, read by the fused L2 on an adaptive grid.  Rows as adj_rows_generic.
+cudaError_t launch_fwd_vern7_dense(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
+cudaError_t launch_adj_vern7_dense(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid *ag, const float *saved,
+                                   cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot(const ConstTables &, const float *out, const float *data, float *cot, float *block_loss, int D, size_t N, int n_save, cudaStream_t);
 cudaError_t launch_l2_finish(const float *block_loss, float *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
@@ -201,6 +207,10 @@ cudaError_t launch_fwd_f64(const Shape64Host &, const Fwd64Host &, int solver, c
 cudaError_t launch_adj_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *adaptive_or_null, cudaStream_t, int *rows_out);
 // discrete adjoint in fp64 (discrete_adjoint.cuh): solver 0 = Tsit5, 1 = Vern7; ad = adaptive Vern7 record or nullptr
 cudaError_t launch_adj_discrete_f64(const Shape64Host &, const Adj64Host &, int solver, const Adapt64Host *ad, cudaStream_t, int *rows_out);
+// Vern7 with its lazy dense output in fp64 (as launch_fwd_vern7_dense / launch_adj_vern7_dense); rows as adj_rows_f64
+cudaError_t launch_fwd_vern7_dense_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);
+cudaError_t launch_adj_vern7_dense_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *ad, const double *saved, cudaStream_t,
+                                       int *rows_out);
 cudaError_t launch_reduce_f64(const double *partial, int nrows, int P1, double *grad, double *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // adaptive Tsit5 only
 cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);

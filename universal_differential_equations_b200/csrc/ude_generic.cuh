@@ -163,8 +163,8 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(FwdParams p)
 }
 
 // Vern7 fixed-step forward solve (solve(prob, Vern7(); saveat, adaptive = false)): 9 stages per step, no FSAL.
-// Vern7's lazy 7th-order dense output is not available (SURVEY.md App. A.3): the interpolating adjoint of a Vern7 solve
-// runs over a Tsit5 re-solve (b200ude.cu).  With p.ustep set (discrete-adjoint handles) u_n of every step is recorded
+// By default the interpolating adjoint of a Vern7 solve runs over a Tsit5 re-solve (b200ude.cu); with B200UDE_FLAG_VERN7_DENSE
+// it runs over Vern7's own dense output (vern7_dense.cuh) from the step record this kernel writes.  With p.ustep set (discrete-adjoint handles) u_n of every step is recorded
 // for the discrete adjoint (discrete_adjoint.cuh), which recomputes the stages from it.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) vern7_forward_kernel(FwdParams p)
@@ -518,9 +518,9 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
     }
 }
 
-// Vern7 with OrdinaryDiffEq's PI controller (abstol / reltol; scenario_1.jl:84-85, seir_exposure.jl:138-139).  The lazy
-// 7th-order interpolant is not available (see above), so the save times are step end points (tstops), exactly as the
-// oracle's Vern7 path does; the step sequence between save points is the controller's own.  No dense record is written
+// Vern7 with OrdinaryDiffEq's PI controller (abstol / reltol; scenario_1.jl:84-85, seir_exposure.jl:138-139).  The save times
+// are step end points (tstops), exactly as the oracle's Vern7 path does (saveat through the lazy 7th-order interpolant:
+// B200UDE_FLAG_VERN7_DENSE, vern7_dense.cuh); the step sequence between save points is the controller's own.  No dense record is written
 // (the interpolating adjoint of a Vern7 solve is taken over a Tsit5 re-solve, see b200ude.cu).  With ap.tgrid set
 // (discrete-adjoint handles) every accepted step is recorded -- tgrid, ustep, hstep, nacc -- for the discrete adjoint.
 template <int BLOCK>

@@ -223,7 +223,13 @@ class Tsit5:
 
 
 class Vern7:
+    """Vern7().  dense=True (B200UDE_FLAG_VERN7_DENSE) runs the reference's Vern7 call as written: an adaptive solve fills saveat
+    from Vern7's lazy 7th-order interpolant instead of stopping at the save times, and the interpolating adjoint runs over
+    that dense output instead of over a Tsit5 re-solve.  Vern7() keeps the default behaviour."""
     code = _lib.VERN7
+
+    def __init__(self, dense=False):
+        self.dense = bool(dense)
 
 
 def _rkc2_beta(s):
@@ -356,7 +362,7 @@ class UDESolver:
             for i, w in enumerate(loss_weights):
                 d.loss_weights[i] = float(w)
         d.max_trajectories = int(max_trajectories)
-        d.flags = _lib.FLAG_APPROX_TANH if approx_tanh else 0
+        d.flags = (_lib.FLAG_APPROX_TANH if approx_tanh else 0) | (_lib.FLAG_VERN7_DENSE if getattr(alg, "dense", False) else 0)
         # adaptive = true: OrdinaryDiffEq's defaults abstol = 1e-6, reltol = 1e-3 when the kwargs are omitted (Fisher-KPP-CNN.jl:136)
         d.adaptive = 1 if adaptive else 0
         d.abstol, d.reltol, d.max_steps = float(abstol), float(reltol), int(max_steps)
@@ -612,7 +618,7 @@ def concrete_solve(prob, alg, u0=None, p=None, *, saveat=None, dt=None, adaptive
     abstol = 1e-6 if abstol is None else abstol
     reltol = 1e-3 if reltol is None else reltol
     key = (id(base.f), t0, dtv, n_steps, save_every, type(alg).__name__, getattr(alg, "stages", None), getattr(alg, "eigen_est", None),
-           type(sensealg).__name__ if sensealg is not None else None, dev.index, tuple(loss_weights) if loss_weights else None,
+           getattr(alg, "dense", None), type(sensealg).__name__ if sensealg is not None else None, dev.index, tuple(loss_weights) if loss_weights else None,
            bool(adaptive), abstol, reltol, max_steps, str(dtype))
     solver = _SOLVERS.get(key)
     if solver is None or solver.capacity < N:
