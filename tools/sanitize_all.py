@@ -68,4 +68,17 @@ for nx, n in ((26, 7), (27, 5), (256, 3)):
     fk2 = ude.FisherKPPUDE(ude.FastChain(ude.FastDense(1, 10, ude.tanh), ude.FastDense(10, 1)), nx)
     th2 = np.concatenate([glorot_theta((1, 10, 1), seed=4), [1.1, -2.3, 0.9, 0.0, 0.01 * (nx - 1) ** 2]])
     run(f"fkpp-generic nx={nx}", fk2, th2, uf, yf, 2.5 / (16 * 0.01 * (nx - 1) ** 2), 40, 8)
+# the largest adjoint footprints of the runtime-shape kernels: fp32 at the 12 288-float constant bank (4 x 12 289 floats of shared
+# memory per CTA), fp64 at 8-64-64-64-64-8 (2 x 13 577 doubles)
+sys.path.insert(0, 'tests')
+import envelope_cases as E
+run("lv_bank", E.ude_form("lv_bank"), E.theta("lv_bank"), u0[:, :130].copy(), y[:, :, :130].copy(), 0.1, 30, 1)
+s = ude.UDESolver(E.ude_form("node8_max"), 0.0, 0.05, 20, 2, max_trajectories=130, dtype=torch.float64)
+s.set_params(torch.from_numpy(E.theta("node8_max")).cuda())
+u8 = torch.from_numpy(E.u0("node8_max", 130)).cuda()
+out8 = s.forward(u8)
+L, g, gu = s.adjoint_l2(out8 + 0.1, want_grad_u0=True)
+torch.cuda.synchronize()
+print("node8_max f64", float(L), float(g.abs().sum()))
+s.close()
 print("ALL DONE")
