@@ -93,11 +93,15 @@ extern "C" {
 #define B200UDE_DISCRETE_ADJOINT 1      /* exact gradient of the discrete scheme, the accepted step sequence held fixed, by reverse
                                            accumulation through the stages of every step: the quantity ForwardDiffSensitivity()
                                            computes in forward mode (scenario_1.jl:84-87, scenario_2.jl:106-108, hudson_bay.jl:99-102).
-                                           Fixed-step Tsit5, fixed-step Vern7 and adaptive Vern7 (save times are tstops) on the
-                                           LV / SEIR / SEIR_NODE / NODE forms, and adaptive Vern7 on the Fisher-KPP UPDE
-                                           (scenario_3.jl:121-126), fp32 and fp64; the fused L2 reads the recorded step-end
-                                           states, so the loss reported is that of the solve itself.  Not for adaptive Tsit5 (its
-                                           saveat values come from the interpolant), fixed-step Fisher-KPP or RKC2. */
+                                           Fixed-step Tsit5, fixed-step Vern7 and adaptive Vern7 on the LV / SEIR / SEIR_NODE /
+                                           NODE forms, and adaptive Vern7 on the Fisher-KPP UPDE (scenario_3.jl:121-126), fp32 and
+                                           fp64.  An adaptive Vern7 solve treats the save times as tstops by default; with
+                                           B200UDE_FLAG_DISCRETE_DENSE (below) it steps freely, fills the save times from Vern7's
+                                           lazy interpolant as OrdinaryDiffEq's saveat does, and the adjoint differentiates the
+                                           interpolated saves too.  The fused L2 reads the saved states of the solve itself
+                                           (recorded step ends, or `out` with the flag), so the loss reported is that solve's.
+                                           Not for adaptive Tsit5 (its saveat values come from the interpolant), fixed-step
+                                           Fisher-KPP or RKC2. */
 
 /* memory space of a pointer argument */
 #define B200UDE_HOST 0
@@ -121,6 +125,20 @@ extern "C" {
                                        Every such handle, the SEIR 3-64-64-1 chain included, runs on the runtime-shape kernels
                                        (vern7_dense.cuh).  B200UDE_EUNSUPPORTED with the discrete adjoint, Tsit5, RKC2 or the
                                        Fisher-KPP UPDE. */
+#define B200UDE_FLAG_DISCRETE_DENSE 4u /* the discrete adjoint through Vern7's interpolated saves, for solver = B200UDE_VERN7 with
+                                       sensealg = B200UDE_DISCRETE_ADJOINT on the LV / SEIR / SEIR_NODE / NODE forms, fp32 and fp64:
+                                       - adaptive: the forward is that of B200UDE_FLAG_VERN7_DENSE (steps stop only at the end of
+                                         tspan, a save time inside a step comes from the interpolant, one on a step end takes the
+                                         step-end state), and the discrete adjoint differentiates exactly that with the accepted
+                                         step sizes held fixed: through the interpolation weights and the six extra stages of every
+                                         step that holds a save time (vern7_dense_discrete.cuh).  This is
+                                         solve(prob, Vern7(); saveat, abstol, reltol, sensealg = ForwardDiffSensitivity()) of
+                                         scenario_1.jl:84-87, scenario_2.jl:106-108, hudson_bay.jl:99-102 as OrdinaryDiffEq steps it.
+                                         `out` must stay valid until the matching adjoint call (the fused L2 reads it);
+                                       - fixed step: saves are step ends; the flag is accepted and the results are bitwise those
+                                         without it.
+                                       B200UDE_EUNSUPPORTED with the interpolating adjoint, together with B200UDE_FLAG_VERN7_DENSE,
+                                       with Tsit5, RKC2 or the Fisher-KPP UPDE. */
 
 /* per-trajectory status words written by b200ude_forward */
 #define B200UDE_TRAJ_OK 0

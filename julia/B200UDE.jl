@@ -31,6 +31,7 @@ const TSIT5, VERN7, RKC2 = Int32.(0:2)
 const INTERPOLATING_ADJOINT, DISCRETE_ADJOINT = Int32(0), Int32(1)
 const HOST, DEVICE = Int32(0), Int32(1)
 const FLAG_VERN7_DENSE = UInt32(2)
+const FLAG_DISCRETE_DENSE = UInt32(4)
 
 Base.@kwdef mutable struct Desc            # mirrors struct b200ude_desc
     struct_size::UInt32 = 0;  device::Int32 = 0;  dtype::Int32 = F32;  model::Int32 = 0
@@ -112,10 +113,14 @@ solver_code(::Vern7) = VERN7
 sens_code(::InterpolatingAdjoint) = INTERPOLATING_ADJOINT
 sens_code(::ForwardDiffSensitivity) = DISCRETE_ADJOINT      # same quantity (exact derivative of the discrete scheme), reverse mode
 sens_code(::Nothing) = INTERPOLATING_ADJOINT
-"""`B200UDE.vern7_dense[] = true`: Vern7 with the interpolating adjoint runs as OrdinaryDiffEq does -- saveat from Vern7's lazy
-dense output, the adjoint over that dense output (B200UDE_FLAG_VERN7_DENSE) -- instead of tstops and a Tsit5 re-solve."""
+"""`B200UDE.vern7_dense[] = true`: Vern7 runs as OrdinaryDiffEq does -- saveat from Vern7's lazy dense output instead of tstops.
+With the interpolating adjoint the adjoint runs over that dense output instead of a Tsit5 re-solve (B200UDE_FLAG_VERN7_DENSE); with
+ForwardDiffSensitivity the discrete adjoint differentiates the interpolated saves (B200UDE_FLAG_DISCRETE_DENSE; the library ignores
+it on a fixed grid, where the saves are step ends).  The Fisher-KPP UPDE with ForwardDiffSensitivity keeps its tstops kernels."""
 const vern7_dense = Ref(false)
-dense_flag(alg, sensealg) = (vern7_dense[] && alg isa Vern7 && sens_code(sensealg) == INTERPOLATING_ADJOINT) ? FLAG_VERN7_DENSE : UInt32(0)
+dense_flag(f, alg, sensealg) = !(vern7_dense[] && alg isa Vern7) ? UInt32(0) :
+                               sens_code(sensealg) != DISCRETE_ADJOINT ? FLAG_VERN7_DENSE :
+                               f.model == MODEL_FKPP ? UInt32(0) : FLAG_DISCRETE_DENSE
 
 function handle_for(f::B200UDEFunction, alg, sensealg, tspan, saveat, dt, abstol, reltol, N)
     ts = saveat isa Number ? collect(tspan[1]:saveat:tspan[2]) : collect(saveat)
@@ -123,7 +128,7 @@ function handle_for(f::B200UDEFunction, alg, sensealg, tspan, saveat, dt, abstol
     all(isapprox.(diff(ts), save_dt; rtol = 1e-9)) || error("B200UDE: uniformly spaced saveat only")
     adaptive = dt === nothing
     step = adaptive ? save_dt : dt
-    key = (objectid(f), typeof(alg), sens_code(sensealg), dense_flag(alg, sensealg), tspan, save_dt, step, adaptive, abstol, reltol)
+    key = (objectid(f), typeof(alg), sens_code(sensealg), dense_flag(f, alg, sensealg), tspan, save_dt, step, adaptive, abstol, reltol)
     h = get(HANDLES, key, nothing)
     (h !== nothing && h.cap >= N) && return h
     nl = length(f.acts)
@@ -134,7 +139,7 @@ function handle_for(f::B200UDEFunction, alg, sensealg, tspan, saveat, dt, abstol
              solver = solver_code(alg), sensealg = sens_code(sensealg), t0 = tspan[1], dt = step,
              n_steps = round(Int32, (tspan[2] - tspan[1]) / step), save_every = round(Int32, save_dt / step),
              adaptive = adaptive ? 1 : 0, abstol = abstol, reltol = reltol, max_steps = adaptive ? 512 : 0, max_trajectories = N,
-             flags = dense_flag(alg, sensealg))
+             flags = dense_flag(f, alg, sensealg))
     HANDLES[key] = Handle(d)
 end
 

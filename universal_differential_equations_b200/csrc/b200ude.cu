@@ -30,7 +30,8 @@ thread_local std::string g_create_error;
 //            scenario_1.jl:62-73 (x=0), scenario_2.jl:79-98 (x=1), hudson_bay.jl:77-91 (x=2)
 //   K_GENERIC  any LV / SEIR / SEIR_NODE / NODE form with chain widths <= 64 and <= 5 layers (k_generic.cu): functional
 //            coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7, the adaptive path of untuned chains and
-//            the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh)
+//            the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh; through Vern7's interpolated
+//            saves: vern7_dense_discrete.cuh)
 //   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126); also
 //            adaptive Tsit5 (fkpp_adaptive.cuh) and adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
 //   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
@@ -96,6 +97,7 @@ struct b200ude_handle {
     float *d_u0_keep = nullptr, *d_aux_out = nullptr;   // Vern7: u0 of the last forward, saved states of the Tsit5 re-solve
     bool vern7_pending = false;
     bool vern7_dense = false;   // B200UDE_FLAG_VERN7_DENSE: saveat and the interpolating adjoint through Vern7's own dense output
+    bool discrete_dense = false;   // B200UDE_FLAG_DISCRETE_DENSE on an adaptive grid: saveat through the interpolant, discrete adjoint through it
     float *d_adam_m = nullptr, *d_adam_v = nullptr, *d_train_out = nullptr;
     int *d_adam_t = nullptr;
     int adam_t = 0;   // host mirror of the step counter
@@ -270,13 +272,13 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
     if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
         // discrete adjoint, or the interpolating adjoint over Vern7's dense output: the forward records u_n of every (accepted)
-        // step, which the adjoint recomputes the stages from.  With the dense flag an adaptive solve saves through the
+        // step, which the adjoint recomputes the stages from.  With either dense flag an adaptive solve saves through the
         // interpolant; a fixed grid saves at step ends either way
         FwdParams p;
         p.u0 = u0; p.out = out; p.ustep = h->d_ustep; p.dense = nullptr; p.status = status; p.theta = h->d_theta;
         p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
         if (h->kid == K_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7(h->gen, h->tab, p, h->ag, st));   // adaptive only (b200ude_create)
-        else if (h->adaptive && h->vern7_dense) CUDA_TRY(h, launch_fwd_vern7_dense(h->gen, h->tab, p, h->ag, st));
+        else if (h->adaptive && (h->vern7_dense || h->discrete_dense)) CUDA_TRY(h, launch_fwd_vern7_dense(h->gen, h->tab, p, h->ag, st));
         else if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
         else CUDA_TRY(h, launch_fwd_vern7(h->gen, h->tab, p, st));
         h->last_out = out;
@@ -345,6 +347,13 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
         CUDA_TRY(h, launch_adj_vern7_dense(h->gen, h->tab, p, h->adaptive ? &h->ag : nullptr, h->last_out, st, &grid));
         if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
         else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
+    if (h->discrete_dense) {
+        // discrete adjoint of the free-stepping Vern7 solve through its interpolated saves; the fused L2 reads the states the forward
+        // returned.  Adaptive, so never peer (refused above)
+        CUDA_TRY(h, launch_adj_vern7_dense_discrete(h->gen, h->tab, p, h->ag, h->last_out, st, &grid));
+        CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
         return B200UDE_OK;
     }
     if (h->var.discrete && h->kid == K_GENERIC) {
@@ -527,7 +536,7 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
         Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
         const Adapt64Host a = adapt64(h);
         if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7_f64(h->sh64, p, a, st));   // adaptive only (b200ude_create)
-        else if (h->adaptive && h->vern7_dense) CUDA_TRY(h, launch_fwd_vern7_dense_f64(h->sh64, p, a, st));
+        else if (h->adaptive && (h->vern7_dense || h->discrete_dense)) CUDA_TRY(h, launch_fwd_vern7_dense_f64(h->sh64, p, a, st));
         else CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
         h->q_last_out = out;
         h->N = N;
@@ -572,6 +581,11 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
     if (h->vern7_dense) {   // interpolating adjoint over the Vern7 dense output; the fused L2 reads the states the forward returned
         const Adapt64Host a = adapt64(h);
         CUDA_TRY(h, launch_adj_vern7_dense_f64(h->sh64, p, h->adaptive ? &a : nullptr, h->q_last_out, st, &rows));
+        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
+        return B200UDE_OK;
+    }
+    if (h->discrete_dense) {   // discrete adjoint through the interpolated saves; the fused L2 reads the states the forward returned
+        CUDA_TRY(h, launch_adj_vern7_dense_discrete_f64(h->sh64, p, adapt64(h), h->q_last_out, st, &rows));
         CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
         return B200UDE_OK;
     }
@@ -638,6 +652,14 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     // discrete_adjoint.cuh and, for the Fisher-KPP UPDE, the grid-per-CTA adaptive Vern7 kernels of fkpp_vern7_discrete.cuh.
     // Adaptive Tsit5 saves through its free interpolant, which an exact discrete adjoint would also have to differentiate;
     // fixed-step Fisher-KPP and RKC2 have no such kernels.
+    // B200UDE_FLAG_DISCRETE_DENSE: the discrete adjoint of the Vern7 solve that saves through its lazy interpolant
+    // (vern7_dense_discrete.cuh); on a fixed grid the saves are step ends and the flag selects nothing
+    const bool disc_dense = (d->flags & B200UDE_FLAG_DISCRETE_DENSE) != 0;
+    if (disc_dense && (d->solver != B200UDE_VERN7 || !disc || d->model == B200UDE_MODEL_FKPP || (d->flags & B200UDE_FLAG_VERN7_DENSE)))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_FLAG_DISCRETE_DENSE applies to Vern7 with the discrete adjoint on the LV / SEIR / SEIR_NODE / NODE forms; "
+                    "not to the interpolating adjoint (B200UDE_FLAG_VERN7_DENSE is its flag, and the two exclude each other), Tsit5, RKC2 or "
+                    "the Fisher-KPP UPDE");
     const bool fkpp_v7 = d->model == B200UDE_MODEL_FKPP && d->adaptive && d->solver == B200UDE_VERN7;
     if (disc && ((d->model == B200UDE_MODEL_FKPP && !fkpp_v7) || d->solver == B200UDE_RKC2 || (d->adaptive && d->solver == B200UDE_TSIT5)))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
@@ -645,7 +667,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                     "LV / SEIR / SEIR_NODE / NODE forms (chain widths <= 64), and for adaptive Vern7 on the Fisher-KPP UPDE, fp32 and fp64; "
                     "not for adaptive Tsit5, fixed-step Fisher-KPP or RKC2");
     // Vern7's lazy dense output (vern7_dense.cuh): saveat through the interpolant and the interpolating adjoint over it.  The
-    // discrete adjoint through an interpolated save would have to differentiate the extra stages: not built
+    // discrete adjoint through an interpolated save has its own flag (above)
     const bool v7dense = (d->flags & B200UDE_FLAG_VERN7_DENSE) != 0;
     if (v7dense && (d->solver != B200UDE_VERN7 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT || d->model == B200UDE_MODEL_FKPP))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
@@ -750,6 +772,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     h->var.approx_tanh = (d->flags & B200UDE_FLAG_APPROX_TANH) ? 1 : 0;
     h->var.discrete = d->sensealg == B200UDE_DISCRETE_ADJOINT ? 1 : 0;
     h->vern7_dense = v7dense;
+    h->discrete_dense = disc_dense && d->adaptive;
     if (d->solver == B200UDE_RKC2) rkc2_tables(d->n_stages, &h->rkc);
     // tuning knobs for experiments (defaults are the measured-best variant, see DESIGN.md)
     h->var.fwd_smem = env_int("B200UDE_FWD_SMEM", 0);

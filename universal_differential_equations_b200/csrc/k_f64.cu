@@ -4,6 +4,7 @@
 #include "discrete_adjoint.cuh"
 #include "fkpp_vern7_discrete.cuh"
 #include "vern7_dense.cuh"
+#include "vern7_dense_discrete.cuh"
 
 #include "params.h"
 
@@ -158,6 +159,26 @@ cudaError_t launch_adj_vern7_dense_f64(const Shape64Host &s, const Adj64Host &p,
     q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
     q.dt = p.dt; q.t0 = ad ? ad->t0 : 0.0; q.save_dt = ad ? ad->save_dt : 0.0;
     auto kern = vern7_dense::adjoint_kernel<DenseOps64, F64_BLOCK>;
+    const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + F64_BLOCK - 1) / F64_BLOCK;
+    *rows_out = grid * (F64_BLOCK / 32);
+    kern<<<grid, F64_BLOCK, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+// ---- discrete adjoint through the interpolated saves of the dense-output forward (vern7_dense_discrete.cuh in fp64) ----
+cudaError_t launch_adj_vern7_dense_discrete_f64(const Shape64Host &s, const Adj64Host &p, const Adapt64Host &a, const double *saved,
+                                                cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_shape(s, st);
+    if (e != cudaSuccess) return e;
+    vern7_dense_discrete::Params<double> q;
+    q.ustep = p.ustep; q.tgrid = a.tgrid; q.hstep = a.hstep; q.nacc = a.nacc; q.cot = p.cot; q.saved = saved;
+    q.grad_u0 = p.grad_u0; q.partial = p.partial; q.N = p.N; q.n_save = a.n_save; q.fused_l2 = p.fused_l2;
+    q.t0 = a.t0; q.save_dt = a.save_dt;
+    auto kern = vern7_dense_discrete::adjoint_kernel<DiscreteOps64, F64_BLOCK>;
     const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

@@ -4,6 +4,7 @@
 #include "discrete_adjoint.cuh"
 #include "fkpp_vern7_discrete.cuh"
 #include "vern7_dense.cuh"
+#include "vern7_dense_discrete.cuh"
 
 #include <algorithm>
 
@@ -154,6 +155,28 @@ cudaError_t launch_adj_vern7_dense(const GenericShape &g, const ConstTables &t, 
     q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
     q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
     auto kern = vern7_dense::adjoint_kernel<DenseOps32, GEN_BLOCK>;
+    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
+    *rows_out = grid * (GEN_BLOCK / 32);
+    kern<<<grid, GEN_BLOCK, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+// ---- discrete adjoint through the interpolated saves of the dense-output forward (vern7_dense_discrete.cuh in fp32) ----
+cudaError_t launch_adj_vern7_dense_discrete(const GenericShape &g, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag,
+                                            const float *saved, cudaStream_t st, int *rows_out)
+{
+    cudaError_t e = upload_tables(t, st);
+    if (e != cudaSuccess) return e;
+    e = upload_gen(g, st);
+    if (e != cudaSuccess) return e;
+    vern7_dense_discrete::Params<float> q;
+    q.ustep = p.ustep; q.tgrid = ag.tgrid; q.hstep = ag.hstep; q.nacc = ag.nacc; q.cot = p.cot; q.saved = saved;
+    q.grad_u0 = p.grad_u0; q.partial = p.partial; q.N = p.N; q.n_save = ag.n_save; q.fused_l2 = p.fused_l2;
+    q.t0 = ag.t0; q.save_dt = ag.save_dt;
+    auto kern = vern7_dense_discrete::adjoint_kernel<DiscreteOps32, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

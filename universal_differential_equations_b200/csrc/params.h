@@ -135,6 +135,10 @@ cudaError_t launch_adj_discrete(const GenericShape &, const ConstTables &, const
 cudaError_t launch_fwd_vern7_dense(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
 cudaError_t launch_adj_vern7_dense(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid *ag, const float *saved,
                                    cudaStream_t, int *rows_out);
+// discrete adjoint of that adaptive forward through its interpolated saves (vern7_dense_discrete.cuh, B200UDE_FLAG_DISCRETE_DENSE):
+// record and `saved` as above, rows as adj_rows_generic
+cudaError_t launch_adj_vern7_dense_discrete(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &,
+                                            const float *saved, cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot(const ConstTables &, const float *out, const float *data, float *cot, float *block_loss, int D, size_t N, int n_save, cudaStream_t);
 cudaError_t launch_l2_finish(const float *block_loss, float *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
@@ -211,6 +215,8 @@ cudaError_t launch_adj_discrete_f64(const Shape64Host &, const Adj64Host &, int 
 cudaError_t launch_fwd_vern7_dense_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);
 cudaError_t launch_adj_vern7_dense_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *ad, const double *saved, cudaStream_t,
                                        int *rows_out);
+cudaError_t launch_adj_vern7_dense_discrete_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, const double *saved,
+                                                cudaStream_t, int *rows_out);   // as launch_adj_vern7_dense_discrete
 cudaError_t launch_reduce_f64(const double *partial, int nrows, int P1, double *grad, double *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // adaptive Tsit5 only
 cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);

@@ -237,10 +237,11 @@ struct Prec<double> {
     static __device__ __forceinline__ double ex(double a) { return exp10(a); }
 };
 
-// stage i of a step from u with step h: g = u + h sum_j a_ij k_j (the expression of the Vern7 forward kernels), k_i = f(g)
+// the point stage i of a step from u with step h is evaluated at: g = u + h sum_j a_ij k_j (the expression of the Vern7 forward
+// kernels)
 template <class Ops, int I>
-__device__ __forceinline__ void stage(const typename Ops::real *u, typename Ops::real h, typename Ops::real (*k)[Ops::MAXD],
-                                      typename Ops::real *g)
+__device__ __forceinline__ void stage_point(const typename Ops::real *u, typename Ops::real h, const typename Ops::real (*k)[Ops::MAXD],
+                                            typename Ops::real *g)
 {
     using R = typename Ops::real;
     const int D = Ops::D();
@@ -254,6 +255,14 @@ __device__ __forceinline__ void stage(const typename Ops::real *u, typename Ops:
         }
         g[c] = fma(h, acc, u[c]);
     }
+}
+
+// stage i of a step from u with step h: k_i = f(g), g its stage point
+template <class Ops, int I>
+__device__ __forceinline__ void stage(const typename Ops::real *u, typename Ops::real h, typename Ops::real (*k)[Ops::MAXD],
+                                      typename Ops::real *g)
+{
+    stage_point<Ops, I>(u, h, k, g);
     Ops::rhs(g, k[I]);
 }
 
@@ -270,13 +279,10 @@ __device__ __forceinline__ void extra_stages(const typename Ops::real *u, typena
     stage<Ops, 15>(u, h, k, g);
 }
 
-// x = u(t_n + th h) = u + h sum_i b_i(th) k_i, b_i by Horner
-template <class Ops>
-__device__ __forceinline__ void interpolate(const typename Ops::real *u, typename Ops::real h, const typename Ops::real (*k)[Ops::MAXD],
-                                            typename Ops::real th, typename Ops::real *x)
+// the interpolation weights b_i(th), i = 0..15, by Horner (zero for the stages without weight)
+template <typename R>
+__device__ __forceinline__ void interp_weights(R th, R *bw)
 {
-    using R = typename Ops::real;
-    R bw[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
         if (!Vern7Dense::weighted(i)) { bw[i] = (R)0; continue; }
@@ -285,6 +291,16 @@ __device__ __forceinline__ void interpolate(const typename Ops::real *u, typenam
         for (int q = 6; q >= 2; --q) acc = fma(acc, th, (R)Vern7Dense::r(i, q));
         bw[i] = i == 0 ? th * fma(acc, th, (R)Vern7Dense::r(0, 1)) : th * th * acc;
     }
+}
+
+// x = u(t_n + th h) = u + h sum_i b_i(th) k_i
+template <class Ops>
+__device__ __forceinline__ void interpolate(const typename Ops::real *u, typename Ops::real h, const typename Ops::real (*k)[Ops::MAXD],
+                                            typename Ops::real th, typename Ops::real *x)
+{
+    using R = typename Ops::real;
+    R bw[16];
+    interp_weights<R>(th, bw);
     const int D = Ops::D();
     for (int c = 0; c < D; ++c) {
         R acc = (R)0;

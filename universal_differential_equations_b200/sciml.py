@@ -223,9 +223,11 @@ class Tsit5:
 
 
 class Vern7:
-    """Vern7().  dense=True (B200UDE_FLAG_VERN7_DENSE) runs the reference's Vern7 call as written: an adaptive solve fills saveat
-    from Vern7's lazy 7th-order interpolant instead of stopping at the save times, and the interpolating adjoint runs over
-    that dense output instead of over a Tsit5 re-solve.  Vern7() keeps the default behaviour."""
+    """Vern7().  dense=True runs the reference's Vern7 calls as written: an adaptive solve fills saveat from Vern7's lazy 7th-order
+    interpolant instead of stopping at the save times.  With InterpolatingAdjoint (B200UDE_FLAG_VERN7_DENSE) the adjoint runs
+    over that dense output instead of over a Tsit5 re-solve; with ForwardDiffSensitivity (B200UDE_FLAG_DISCRETE_DENSE) the discrete
+    adjoint differentiates the interpolated saves, extra stages included.  On a fixed grid the saves are step ends and
+    ForwardDiffSensitivity needs no flag.  Vern7() keeps the default behaviour (save times are tstops)."""
     code = _lib.VERN7
 
     def __init__(self, dense=False):
@@ -299,10 +301,12 @@ class ForwardDiffSensitivity:
     derivative of the discrete solver scheme with the accepted step sequence held fixed.  The reference pushes dual numbers
     through the solver (cost O(P) forward solves); here the same quantity comes from reverse accumulation through the stages
     of every recorded step (one backward sweep, B200UDE_DISCRETE_ADJOINT).  Fixed-step Tsit5, fixed-step Vern7 and adaptive
-    Vern7 (save times are tstops) on the LV / SEIR / SEIR_NODE / NODE forms, and adaptive Vern7 on the Fisher-KPP UPDE
-    (scenario_3.jl:121-126), float32 and float64; so
+    Vern7 on the LV / SEIR / SEIR_NODE / NODE forms, and adaptive Vern7 on the Fisher-KPP UPDE (scenario_3.jl:121-126), float32
+    and float64; so
     concrete_solve(prob, Vern7(), p=theta, saveat, abstol=1e-6, reltol=1e-6, sensealg=ForwardDiffSensitivity()) differentiates
-    the Vern7 solve itself.  Not available: adaptive Tsit5, fixed-step Fisher-KPP, RKC2.
+    the Vern7 solve itself.  With Vern7() that solve stops at the save times; with Vern7(dense=True) it steps freely and fills
+    saveat from the interpolant, as OrdinaryDiffEq does, and the gradient goes through the interpolated saves
+    (B200UDE_FLAG_DISCRETE_DENSE; not on the Fisher-KPP UPDE).  Not available: adaptive Tsit5, fixed-step Fisher-KPP, RKC2.
 
     `convert_tspan` is accepted and ignored: t and dt are never dual numbers here, which is what convert_tspan = false asks for
     (and what the default does whenever tspan does not depend on the parameters)."""
@@ -362,7 +366,13 @@ class UDESolver:
             for i, w in enumerate(loss_weights):
                 d.loss_weights[i] = float(w)
         d.max_trajectories = int(max_trajectories)
-        d.flags = (_lib.FLAG_APPROX_TANH if approx_tanh else 0) | (_lib.FLAG_VERN7_DENSE if getattr(alg, "dense", False) else 0)
+        d.flags = _lib.FLAG_APPROX_TANH if approx_tanh else 0
+        if getattr(alg, "dense", False):
+            # the discrete adjoint has its own flag, and on a fixed grid (saves are step ends) needs none
+            if isinstance(sensealg, ForwardDiffSensitivity):
+                d.flags |= _lib.FLAG_DISCRETE_DENSE if adaptive else 0
+            else:
+                d.flags |= _lib.FLAG_VERN7_DENSE
         # adaptive = true: OrdinaryDiffEq's defaults abstol = 1e-6, reltol = 1e-3 when the kwargs are omitted (Fisher-KPP-CNN.jl:136)
         d.adaptive = 1 if adaptive else 0
         d.abstol, d.reltol, d.max_steps = float(abstol), float(reltol), int(max_steps)
