@@ -99,7 +99,7 @@ u0, y = synthetic_ensemble(N)
 s = ude.UDESolver(ude.LotkaVolterraUDE(chain), 0.0, 0.1, 30, 1, max_trajectories=N, adaptive=True, abstol=1e-6, reltol=1e-6, max_steps=128)
 tf, ta = gpu_time(s, theta, u0, y)
 s.close()
-report("LV 2-32-32-2 ADAPTIVE Tsit5 abstol=reltol=1e-6, N=65536", N, tf, ta, 0.0, None, {"kernels": "lv32::tc::adaptive_forward_kernel / lv32::tc::adjoint_kernel<ADAPT> (B200UDE_ADAPTIVE_TC=0: generic::adaptive_*)"})
+report("LV 2-32-32-2 ADAPTIVE Tsit5 abstol=reltol=1e-6, N=65536", N, tf, ta, 0.0, None, {"kernels": "lv32::tc::adaptive_forward_kernel / lv32::tc::adjoint_kernel<ADAPT> (B200UDE_ADAPTIVE_TC=0: generic::adaptive_*<Ops32, 128>)"})
 
 # ---- SEIR exposure UDE, adaptive Tsit5 abstol = reltol = 1e-4 (fp32 states of magnitude 1e7), saved daily
 N = 65536

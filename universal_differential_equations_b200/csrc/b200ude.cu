@@ -674,7 +674,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                     "create: B200UDE_FLAG_VERN7_DENSE applies to Vern7 with the interpolating adjoint on the LV / SEIR / SEIR_NODE / NODE forms; "
                     "not to the discrete adjoint, Tsit5, RKC2 or the Fisher-KPP UPDE");
     if (want64) {
-        // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_f64.cuh): LV / SEIR / NODE forms, Tsit5 and Vern7,
+        // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_generic.cuh in fp64, k_f64.cu): LV / SEIR / NODE forms, Tsit5 and Vern7,
         // fixed step and adaptive, interpolating or discrete adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
         if (!generic_ok(*d) || d->solver == B200UDE_RKC2)
             return fail(nullptr, B200UDE_EUNSUPPORTED,

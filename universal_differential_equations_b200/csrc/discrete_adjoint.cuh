@@ -20,13 +20,14 @@
 // adaptive mode the warp loops over its longest record; lanes with shorter records shadow step 0 with a zero cotangent, so the
 // shuffles stay convergent and each trajectory's grad_u0 does not depend on its neighbours.
 //
-// `Ops` supplies the precision: real, MAXD, D(), P(), lossw(c), rhs(u, du), vjp(u, g, lv, kl, gw, lane) (kl = J_u^T g;
-// gw += lv J_theta^T g, all lanes participating).  k_generic.cu instantiates it in fp32, k_f64.cu in fp64.
+// `Ops` is the precision of the runtime-shape model layer (ude_generic.cuh): k_generic.cu instantiates it in fp32 (Ops32),
+// k_f64.cu in fp64 (Ops64).  The stage VJPs go through generic::model_vjp with unit quadrature weight (h is inside kbar).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "tsit5.cuh"
+#include "ude_generic.cuh"
 #include "vern7.cuh"
 
 namespace b200ude {
@@ -119,7 +120,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Params<typename Ops::
         for (int c = 0; c < D; ++c) u[c] = p.ustep[((size_t)sr * D + c) * N + n];
         // stages, as the forward kernels evaluate them
         for (int c = 0; c < D; ++c) gs[0][c] = u[c];
-        Ops::rhs(u, k[0]);
+        generic::model_rhs<Ops>(u, k[0]);
 #pragma unroll
         for (int i = 1; i < S; ++i) {
             for (int c = 0; c < D; ++c) {
@@ -129,7 +130,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Params<typename Ops::
                     if (Tab::a(i, j) != 0.0) acc = fma((R)Tab::a(i, j), k[j][c], acc);
                 gs[i][c] = fma(h, acc, u[c]);
             }
-            Ops::rhs(gs[i], k[i]);
+            generic::model_rhs<Ops>(gs[i], k[i]);
         }
         // reverse recurrence through the stages
         const R lv = act ? (R)1 : (R)0;
@@ -142,7 +143,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Params<typename Ops::
                     if (Tab::a(j, i) != 0.0) acc = fma((R)Tab::a(j, i), gb[j][c], acc);
                 kb[c] = act ? h * acc : (R)0;
             }
-            Ops::vjp(gs[i], kb, lv, gb[i], gw, lane);
+            generic::model_vjp<Ops>(gs[i], kb, (R)1, lv, gb[i], gw, lane);
         }
         if (act)
             for (int c = 0; c < D; ++c) {

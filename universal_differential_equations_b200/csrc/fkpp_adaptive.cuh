@@ -3,7 +3,7 @@
 //   du_i = NN(u_i) + D0 * (w1 u_{i-1} + w2 u_i + w3 u_{i+1}),  periodic, theta = [chain | w1 w2 w3 b | D0]
 //   (FisherKPP/Fisher-KPP-CNN.jl:111-126, :136 -- concrete_solve(prob_nn, Tsit5(), ...) with no dt: adaptive, default tolerances).
 //
-// Geometry of the fixed-step Fisher-KPP kernels (ude_generic.cuh): one thread per grid point, `tpc` whole trajectories per CTA,
+// Geometry of the fixed-step Fisher-KPP kernels (k_generic.cu): one thread per grid point, `tpc` whole trajectories per CTA,
 // neighbours through shared memory; the step record (ustep, dense) is point-fastest [row][trajectory][point], the ABI arrays
 // (u0, out, cot, grad_u0) trajectory-fastest [row][point][trajectory]; tgrid [max_steps+1][N] and nacc [N] as in the other
 // adaptive kernels.
@@ -17,18 +17,19 @@
 // any thread of the CTA still has work (__syncthreads_or), so every thread executes the same barrier sequence; a trajectory that
 // has finished keeps stepping with h = 0 on its frozen state and records nothing.
 //
-// `Ops` supplies the precision: real, theta(i), P(), chain(x), chain_vjp(x, dy, w, gw, lane), warp_acc, interp weights, btilde
-// (k_generic.cu: fp32 over the constant bank; k_f64.cu: fp64 over the handle's theta).
+// `Ops` is the precision of the runtime-shape model layer (ude_generic.cuh): k_generic.cu: fp32 over the constant bank (Ops32);
+// k_f64.cu: fp64 over the handle's theta (Ops64).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "tsit5.cuh"
+#include "ude_generic.cuh"
 
 namespace b200ude {
 namespace fkpp_adapt {
 
-// CTA shape of the fixed-step Fisher-KPP kernels (fkpp_geom, k_generic.cu; adj_rows_fkpp sizes the partial rows of both):
+// CTA shape of every Fisher-KPP kernel, fixed step (k_generic.cu) and adaptive (adj_rows_fkpp sizes the partial rows of all):
 // tpc whole trajectories in about 128 threads, a warp multiple
 static inline void cta_geometry(int Nx, int *tpc, int *threads)
 {
@@ -73,6 +74,23 @@ struct Adj {
     R t0, save_dt;
 };
 
+// the chain at one grid point (one input, one output), and its VJP: returns dx, this warp's gradient vector += w (dchain/dtheta)^T dy
+template <class Ops>
+__device__ __forceinline__ typename Ops::real point_chain(typename Ops::real x)
+{
+    typename Ops::real y;
+    generic::chain_fwd<Ops, false>(&x, &y, nullptr, nullptr);
+    return y;
+}
+template <class Ops>
+__device__ __forceinline__ typename Ops::real point_chain_vjp(typename Ops::real x, typename Ops::real dy, typename Ops::real w,
+                                                              typename Ops::real *gw, int lane)
+{
+    typename Ops::real dx;
+    generic::chain_vjp<Ops>(&x, &dy, w, &dx, gw, lane);
+    return dx;
+}
+
 template <typename R>
 __device__ __forceinline__ void exchange(R *sU, int slot, int base, int i, int Nx, bool valid, R v, R &vm, R &vp)
 {
@@ -113,14 +131,14 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol;
     const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)50, beta2 = (R)2 / (R)25;
-    const R ttol = sizeof(R) == 4 ? (R)1e-6 : (R)1e-12;   // relative slack of the clip / save-time tests (as in the one-thread kernels)
-    const R big = sizeof(R) == 4 ? (R)3.0e38 : (R)1.0e300;
+    const R ttol = Prec<R>::clip;   // relative slack of the clip / save-time tests (as in the one-thread kernels)
+    const R big = Prec<R>::huge;
     const int sx = Ops::P() - 5;
     const R w1 = Ops::theta(sx), w2 = Ops::theta(sx + 1), w3 = Ops::theta(sx + 2), D0 = Ops::theta(sx + 4);
     auto rhs = [&](R g) {
         R gm, gp;
         exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
-        const R y = Ops::chain(g);
+        const R y = point_chain<Ops>(g);
         return fma(D0, fma(w1, gm, fma(w2, g, w3 * gp)), y);
     };
     auto rms = [&](R v) { return sqrt(traj_sum(sE, slot, base, Nx, valid, v) / (R)Nx); };
@@ -169,7 +187,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
         }
         R e = (R)0;
 #pragma unroll
-        for (int j = 0; j < 7; ++j) e = fma(Ops::btilde(j), k[j], e);
+        for (int j = 0; j < 7; ++j) e = fma(generic::tsit5_btilde<R>(j), k[j], e);
         e *= h;
         const R sc = abstol + reltol * fmax(fabs(u), fabs(un));
         const R EEst = rms((e / sc) * (e / sc));
@@ -186,7 +204,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
                 const R ts = t0 + p.save_dt * (R)isave;
                 if (ts > tn + ttol * fabs(tn)) break;
                 R bw[7];
-                Ops::interp(fmin((ts - t) / h, (R)1), bw);
+                generic::tsit5_bw_rt(fmin((ts - t) / h, (R)1), bw);
                 R acc = (R)0;
 #pragma unroll
                 for (int j = 0; j < 7; ++j) acc = fma(bw[j], k[j], acc);
@@ -209,7 +227,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
         }
     }
     if (bad && live) {   // failed solve (non-finite error estimate / max_steps): the unreached save points are NaN
-        const R nan = sizeof(R) == 4 ? (R)__int_as_float(0x7fc00000) : (R)__longlong_as_double(0x7ff8000000000000LL);
+        const R nan = Prec<R>::nan();
         for (int is = isave; is < p.n_save; ++is) store_abi(p.out, is, nan);
     }
     if (live && i == 0) p.nacc[n] = nacc;
@@ -238,7 +256,7 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
     const int traj = blockIdx.x * p.tpc + t_loc;
     const bool live = valid && traj < p.N;
     const size_t N = (size_t)p.N, n = (size_t)(live ? traj : p.N - 1);
-    const R eps_rel = sizeof(R) == 4 ? (R)1e-5 : (R)1e-10;   // sub-interval end tests, relative to the step (as in the one-thread kernels)
+    const R eps_rel = Prec<R>::eta;   // sub-interval end tests, relative to the step (as in the one-thread kernels)
     const int sx = P - 5;
     const R w1 = Ops::theta(sx), w2 = Ops::theta(sx + 1), w3 = Ops::theta(sx + 2), D0 = Ops::theta(sx + 4);
     const int nacc = live ? p.nacc[n] : 0;
@@ -274,7 +292,7 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
                 R x = u_n;
                 if (act_s) {
                     R bw[7];
-                    Ops::interp(fmin(fmax((cur - (R)Tsit5::c(st) * h - tn) / hn, (R)0), (R)1), bw);
+                    generic::tsit5_bw_rt(fmin(fmax((cur - (R)Tsit5::c(st) * h - tn) / hn, (R)0), (R)1), bw);
                     R acc = (R)0;
 #pragma unroll
                     for (int j = 0; j < 7; ++j) acc = fma(bw[j], p.dense[((size_t)(sc_ * 6 + j) * N + n) * Nx + i], acc);
@@ -290,12 +308,12 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
                 R xm, xp, gm, gp;
                 exchange(sU, slot, base, i, Nx, valid, x, xm, xp);
                 exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
-                const R dx = Ops::chain_vjp(x, g, w, gw, lane);
+                const R dx = point_chain_vjp<Ops>(x, g, w, gw, lane);
                 kl[st] = dx + D0 * fma(w2, g, fma(w1, gp, w3 * gm));   // (J^T g)_i: w1 couples i+1 -> i, w3 couples i-1 -> i
-                Ops::warp_acc(gw, sx + 0, w * D0 * xm * g, lane);
-                Ops::warp_acc(gw, sx + 1, w * D0 * x * g, lane);
-                Ops::warp_acc(gw, sx + 2, w * D0 * xp * g, lane);
-                Ops::warp_acc(gw, sx + 4, w * fma(w1, xm, fma(w2, x, w3 * xp)) * g, lane);
+                generic::warp_acc(gw, sx + 0, w * D0 * xm * g, lane);
+                generic::warp_acc(gw, sx + 1, w * D0 * x * g, lane);
+                generic::warp_acc(gw, sx + 2, w * D0 * xp * g, lane);
+                generic::warp_acc(gw, sx + 4, w * fma(w1, xm, fma(w2, x, w3 * xp)) * g, lane);
             }
             if (has) {
                 R acc = (R)0;

@@ -10,7 +10,7 @@
 // threads of a trajectory hold the same bits and take the same decisions.  The attempt loop of the forward and the step loop of
 // the adjoint run while any thread of the CTA still has work: every thread executes the same barrier sequence.
 //
-// Forward: the controller of generic::vern7_adaptive_forward_kernel (ude_generic.cuh) and its fp64 twin -- 10 stages, error
+// Forward: the controller of generic::vern7_adaptive_forward_kernel (ude_generic.cuh) -- 10 stages, error
 // from btilde, PI with gamma 0.9, qmin 1/5, qmax 10, beta1 7/70, beta2 2/35, Hairer initial step with the order-7 exponent, no
 // FSAL (k_1 kept after a rejection), save times are tstops: a step is clipped to the next save time and out[isave] is the
 // step-end state.  The record is the one the discrete adjoint needs and nothing more: ustep [nacc+1][N][Nx] (point-fastest),
@@ -24,8 +24,7 @@
 // The CTA loops over its longest record; a trajectory past its own record shadows step 0 with a zero cotangent (h = 0), so its
 // grad_u0 does not depend on its neighbours.
 //
-// `Ops` supplies the precision: real, theta(i), P(), chain(x), chain_vjp(x, dy, w, gw, lane), warp_acc (fkpp_adaptive.cuh's Ops;
-// k_generic.cu: FkppOps32, k_f64.cu: FkppOps64).
+// `Ops` is the precision of the runtime-shape model layer (ude_generic.cuh; k_generic.cu: Ops32, k_f64.cu: Ops64).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -66,7 +65,7 @@ template <class Ops>
 __device__ __forceinline__ typename Ops::real rhs_point(typename Ops::real g, typename Ops::real gm, typename Ops::real gp, typename Ops::real w1,
                                                         typename Ops::real w2, typename Ops::real w3, typename Ops::real D0)
 {
-    return fma(D0, fma(w1, gm, fma(w2, g, w3 * gp)), Ops::chain(g));
+    return fma(D0, fma(w1, gm, fma(w2, g, w3 * gp)), fkpp_adapt::point_chain<Ops>(g));
 }
 
 template <class Ops>
@@ -87,8 +86,8 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol;
     const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)70, beta2 = (R)2 / (R)35;   // order 7
-    const R ttol = sizeof(R) == 4 ? (R)1e-6 : (R)1e-12;   // relative slack of the clip test (as in the one-thread kernels)
-    const R big = sizeof(R) == 4 ? (R)3.0e38 : (R)1.0e300;
+    const R ttol = Prec<R>::clip;   // relative slack of the clip test (as in the one-thread kernels)
+    const R big = Prec<R>::huge;
     const int sx = Ops::P() - 5;
     const R w1 = Ops::theta(sx), w2 = Ops::theta(sx + 1), w3 = Ops::theta(sx + 2), D0 = Ops::theta(sx + 4);
     auto rhs = [&](R g) {
@@ -179,7 +178,7 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
         }
     }
     if (bad && live) {   // failed solve (non-finite error estimate / max_steps): the unreached save points are NaN
-        const R nan = sizeof(R) == 4 ? (R)__int_as_float(0x7fc00000) : (R)__longlong_as_double(0x7ff8000000000000LL);
+        const R nan = Prec<R>::nan();
         for (int is = isave; is < p.n_save; ++is) store_abi(p.out, is, nan);
     }
     if (live && i == 0) p.nacc[n] = nacc;
@@ -225,7 +224,7 @@ __global__ void __launch_bounds__(256) discrete_adjoint_kernel(Adj<typename Ops:
     auto jump = [&](int is, int row) {
         const size_t idx = ((size_t)is * Nx + i) * N + n;
         if (p.fused_l2) {
-            const R nan = sizeof(R) == 4 ? (R)__int_as_float(0x7fc00000) : (R)__longlong_as_double(0x7ff8000000000000LL);
+            const R nan = Prec<R>::nan();
             const R us = row >= 0 ? p.ustep[((size_t)row * N + n) * Nx + i] : nan;
             const R r = us - p.cot[idx];
             loss = fma(r, r, loss);
@@ -274,13 +273,13 @@ __global__ void __launch_bounds__(256) discrete_adjoint_kernel(Adj<typename Ops:
             const R kb = act ? h * acc : (R)0;
             R kbm, kbp;
             fkpp_adapt::exchange(sU, slot, base, i, Nx, valid, kb, kbm, kbp);
-            const R dx = Ops::chain_vjp(gs[st], kb, lv, gw, lane);
+            const R dx = fkpp_adapt::point_chain_vjp<Ops>(gs[st], kb, lv, gw, lane);
             gb[st] = dx + D0 * fma(w2, kb, fma(w1, kbp, w3 * kbm));   // (J^T kb)_i: w1 couples i+1 -> i, w3 couples i-1 -> i
             const R xm = gsm[st], x = gs[st], xp = gsp[st];
-            Ops::warp_acc(gw, sx + 0, D0 * xm * kb, lane);
-            Ops::warp_acc(gw, sx + 1, D0 * x * kb, lane);
-            Ops::warp_acc(gw, sx + 2, D0 * xp * kb, lane);
-            Ops::warp_acc(gw, sx + 4, fma(w1, xm, fma(w2, x, w3 * xp)) * kb, lane);
+            generic::warp_acc(gw, sx + 0, D0 * xm * kb, lane);
+            generic::warp_acc(gw, sx + 1, D0 * x * kb, lane);
+            generic::warp_acc(gw, sx + 2, D0 * xp * kb, lane);
+            generic::warp_acc(gw, sx + 4, fma(w1, xm, fma(w2, x, w3 * xp)) * kb, lane);
         }
         if (act) {
             R acc = lam;

@@ -1,5 +1,6 @@
-// k_f64.cu -- double-precision kernels (dtype = B200UDE_F64): launchers of ude_f64.cuh + the fp64 reduction / L2 helpers.
-#include "ude_f64.cuh"
+// k_f64.cu -- double-precision kernels (dtype = B200UDE_F64): the runtime-shape kernels (ude_generic.cuh and the headers written
+// over its Ops) in fp64 + the fp64 reduction / L2 helpers.
+#include "ude_generic.cuh"
 #include "fkpp_adaptive.cuh"
 #include "discrete_adjoint.cuh"
 #include "fkpp_vern7_discrete.cuh"
@@ -9,6 +10,43 @@
 #include "params.h"
 
 namespace b200ude {
+
+namespace f64 {
+struct Shape64 {
+    uint64_t serial;
+    int model, D, din, dout, n_layers, n_prefix, P;
+    int widths[6];
+    int acts[5];
+    int woff[5];          // offset of layer l's W in theta (column-major, out x in), its bias follows at woff + in*out
+    const double *theta;  // the handle's device copy
+    double consts[16], lossw[16];
+};
+static __constant__ Shape64 c_gen;
+}  // namespace f64
+
+// the fp64 precision of the runtime-shape model layer: shape, constants and loss weights from one small __constant__ struct,
+// theta from the handle's device copy (global memory, L1-resident)
+struct Ops64 {
+    using real = double;
+    using Fwd = Fwd64Host;
+    using Adj = Adj64Host;
+    using Adapt = Adapt64Host;
+    static constexpr int MAXD = generic::MAXD;
+    static __device__ __forceinline__ int model() { return f64::c_gen.model; }
+    static __device__ __forceinline__ int D() { return f64::c_gen.D; }
+    static __device__ __forceinline__ int din() { return f64::c_gen.din; }
+    static __device__ __forceinline__ int dout() { return f64::c_gen.dout; }
+    static __device__ __forceinline__ int n_layers() { return f64::c_gen.n_layers; }
+    static __device__ __forceinline__ int n_prefix() { return f64::c_gen.n_prefix; }
+    static __device__ __forceinline__ int P() { return f64::c_gen.P; }
+    static __device__ __forceinline__ int width(int l) { return f64::c_gen.widths[l]; }
+    static __device__ __forceinline__ int woff(int l) { return f64::c_gen.woff[l]; }
+    static __device__ __forceinline__ int layer_act(int l) { return f64::c_gen.acts[l]; }
+    static __device__ __forceinline__ const double &theta(int i) { return f64::c_gen.theta[i]; }
+    static __device__ __forceinline__ const double &consts(int i) { return f64::c_gen.consts[i]; }
+    static __device__ __forceinline__ const double &lossw(int c) { return f64::c_gen.lossw[c]; }
+    static __device__ __forceinline__ double act(int k, double a) { return k == ACT_TANH ? tanh(a) : (k == ACT_RBF ? exp(-a * a) : a); }
+};
 
 constexpr int F64_BLOCK = 64;   // two warps per CTA: the per-warp gradient vector (P + 1 doubles) lives in shared memory
 
@@ -38,36 +76,17 @@ static cudaError_t upload_shape(const Shape64Host &h, cudaStream_t st)
     return e;
 }
 
-static f64::Fwd64 fwd(const Fwd64Host &p)
-{
-    f64::Fwd64 q;
-    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.dt = p.dt;
-    return q;
-}
-static f64::Adj64 adj(const Adj64Host &p)
-{
-    f64::Adj64 q;
-    q.ustep = p.ustep; q.dense = p.dense; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial; q.N = p.N; q.n_steps = p.n_steps;
-    q.save_every = p.save_every; q.fused_l2 = p.fused_l2; q.dt = p.dt;
-    return q;
-}
-static f64::Adapt64 adapt(const Adapt64Host &a, bool record)
-{
-    return f64::Adapt64{a.t0, a.save_dt, a.abstol, a.reltol, a.n_save, a.max_steps, record ? a.tgrid : nullptr, record ? a.nacc : nullptr,
-                        record ? a.hstep : nullptr};
-}
-
 cudaError_t launch_fwd_f64(const Shape64Host &s, const Fwd64Host &p, int solver, const Adapt64Host *ad, cudaStream_t st)
 {
     cudaError_t e = upload_shape(s, st);
     if (e != cudaSuccess) return e;
     const int grid = (p.N + F64_BLOCK - 1) / F64_BLOCK;
     if (solver == 1) {   // Vern7: the step record only for the discrete adjoint (p.ustep set)
-        if (ad) f64::vern7_adaptive_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p), adapt(*ad, p.ustep != nullptr));
-        else f64::vern7_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p));
+        if (ad) generic::vern7_adaptive_forward_kernel<Ops64, F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(p, *ad);
+        else generic::vern7_forward_kernel<Ops64, F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(p);
     } else {
-        if (ad) f64::adaptive_forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p), adapt(*ad, true));
-        else f64::forward_kernel<F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(fwd(p));
+        if (ad) generic::adaptive_forward_kernel<Ops64, F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(p, *ad);
+        else generic::forward_kernel<Ops64, F64_BLOCK><<<grid, F64_BLOCK, 0, st>>>(p);
     }
     return cudaGetLastError();
 }
@@ -80,32 +99,20 @@ cudaError_t launch_adj_f64(const Shape64Host &s, const Adj64Host &p, const Adapt
     const int grid = (p.N + F64_BLOCK - 1) / F64_BLOCK;
     *rows_out = grid * (F64_BLOCK / 32);
     if (ad) {
-        auto kern = f64::adaptive_adjoint_kernel<F64_BLOCK>;
+        auto kern = generic::adaptive_adjoint_kernel<Ops64, F64_BLOCK>;
         e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        kern<<<grid, F64_BLOCK, smem, st>>>(adj(p), adapt(*ad, true));
+        kern<<<grid, F64_BLOCK, smem, st>>>(p, *ad);
     } else {
-        auto kern = f64::adjoint_kernel<F64_BLOCK>;
+        auto kern = generic::adjoint_kernel<Ops64, F64_BLOCK>;
         e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        kern<<<grid, F64_BLOCK, smem, st>>>(adj(p));
+        kern<<<grid, F64_BLOCK, smem, st>>>(p);
     }
     return cudaGetLastError();
 }
 
-// ---- discrete adjoint (discrete_adjoint.cuh in fp64: theta from the handle's device copy) ----
-struct DiscreteOps64 {
-    using real = double;
-    static constexpr int MAXD = f64::MAXD;
-    static __device__ __forceinline__ int D() { return f64::c_gen.D; }
-    static __device__ __forceinline__ int P() { return f64::c_gen.P; }
-    static __device__ __forceinline__ double lossw(int c) { return f64::c_gen.lossw[c]; }
-    static __device__ __forceinline__ void rhs(const double *u, double *du) { f64::model_rhs(u, du); }
-    static __device__ __forceinline__ void vjp(const double *u, const double *g, double lv, double *kl, double *gw, int lane)
-    {
-        f64::model_vjp(u, g, 1.0, lv, kl, gw, lane);
-    }
-};
+// ---- discrete adjoint (discrete_adjoint.cuh in fp64) ----
 
 cudaError_t launch_adj_discrete_f64(const Shape64Host &s, const Adj64Host &p, int solver, const Adapt64Host *ad, cudaStream_t st, int *rows_out)
 {
@@ -117,8 +124,8 @@ cudaError_t launch_adj_discrete_f64(const Shape64Host &s, const Adj64Host &p, in
     q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
     q.dt = p.dt; q.t0 = ad ? ad->t0 : 0.0; q.save_dt = ad ? ad->save_dt : 0.0;
     q.margin = 5e-13;   // half the clipping margin of vern7_adaptive_forward_kernel
-    auto kern = solver == 1 ? discrete::adjoint_kernel<DiscreteOps64, discrete::Vern7Scheme, F64_BLOCK>
-                            : discrete::adjoint_kernel<DiscreteOps64, discrete::Tsit5Scheme, F64_BLOCK>;
+    auto kern = solver == 1 ? discrete::adjoint_kernel<Ops64, discrete::Vern7Scheme, F64_BLOCK>
+                            : discrete::adjoint_kernel<Ops64, discrete::Tsit5Scheme, F64_BLOCK>;
     const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -129,12 +136,6 @@ cudaError_t launch_adj_discrete_f64(const Shape64Host &s, const Adj64Host &p, in
 }
 
 // ---- Vern7 with its lazy dense output (vern7_dense.cuh in fp64) ----
-struct DenseOps64 : DiscreteOps64 {
-    static __device__ __forceinline__ void vjp(const double *u, const double *g, double sc, double lv, double *kl, double *gw, int lane)
-    {
-        f64::model_vjp(u, g, sc, lv, kl, gw, lane);
-    }
-};
 
 cudaError_t launch_fwd_vern7_dense_f64(const Shape64Host &s, const Fwd64Host &p, const Adapt64Host &a, cudaStream_t st)
 {
@@ -144,7 +145,7 @@ cudaError_t launch_fwd_vern7_dense_f64(const Shape64Host &s, const Fwd64Host &p,
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.tgrid = a.tgrid; q.hstep = a.hstep; q.nacc = a.nacc; q.status = p.status;
     q.N = p.N; q.n_save = a.n_save; q.max_steps = a.max_steps;
     q.t0 = a.t0; q.save_dt = a.save_dt; q.abstol = a.abstol; q.reltol = a.reltol;
-    vern7_dense::forward_kernel<DenseOps64, F64_BLOCK><<<(p.N + F64_BLOCK - 1) / F64_BLOCK, F64_BLOCK, 0, st>>>(q);
+    vern7_dense::forward_kernel<Ops64, F64_BLOCK><<<(p.N + F64_BLOCK - 1) / F64_BLOCK, F64_BLOCK, 0, st>>>(q);
     return cudaGetLastError();
 }
 
@@ -158,7 +159,7 @@ cudaError_t launch_adj_vern7_dense_f64(const Shape64Host &s, const Adj64Host &p,
     q.cot = p.cot; q.saved = saved; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
     q.dt = p.dt; q.t0 = ad ? ad->t0 : 0.0; q.save_dt = ad ? ad->save_dt : 0.0;
-    auto kern = vern7_dense::adjoint_kernel<DenseOps64, F64_BLOCK>;
+    auto kern = vern7_dense::adjoint_kernel<Ops64, F64_BLOCK>;
     const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -178,7 +179,7 @@ cudaError_t launch_adj_vern7_dense_discrete_f64(const Shape64Host &s, const Adj6
     q.ustep = p.ustep; q.tgrid = a.tgrid; q.hstep = a.hstep; q.nacc = a.nacc; q.cot = p.cot; q.saved = saved;
     q.grad_u0 = p.grad_u0; q.partial = p.partial; q.N = p.N; q.n_save = a.n_save; q.fused_l2 = p.fused_l2;
     q.t0 = a.t0; q.save_dt = a.save_dt;
-    auto kern = vern7_dense_discrete::adjoint_kernel<DiscreteOps64, F64_BLOCK>;
+    auto kern = vern7_dense_discrete::adjoint_kernel<Ops64, F64_BLOCK>;
     const size_t smem = sizeof(double) * (size_t)(F64_BLOCK / 32) * (s.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -188,28 +189,7 @@ cudaError_t launch_adj_vern7_dense_discrete_f64(const Shape64Host &s, const Adj6
     return cudaGetLastError();
 }
 
-// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp64: theta from the handle's device copy) ----
-struct FkppOps64 {
-    using real = double;
-    static __device__ __forceinline__ double theta(int i) { return f64::c_gen.theta[i]; }
-    static __device__ __forceinline__ int P() { return f64::c_gen.P; }
-    static __device__ __forceinline__ double chain(double x)
-    {
-        double y;
-        f64::chain_fwd<false>(&x, &y, nullptr, nullptr);
-        return y;
-    }
-    static __device__ __forceinline__ double chain_vjp(double x, double dy, double w, double *gw, int lane)
-    {
-        double dx;
-        f64::chain_vjp(&x, &dy, w, &dx, gw, lane);
-        return dx;
-    }
-    static __device__ __forceinline__ void warp_acc(double *gw, int idx, double v, int lane) { f64::warp_acc(gw, idx, v, lane); }
-    static __device__ __forceinline__ void interp(double Th, double *bw) { f64::tsit5_bw_rt(Th, bw); }
-    static __device__ __forceinline__ double btilde(int j) { return f64::tsit5_btilde(j); }
-};
-
+// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp64) ----
 cudaError_t launch_fwd_fkpp_f64(const Shape64Host &s, const Fwd64Host &p, const Adapt64Host &a, cudaStream_t st)
 {
     cudaError_t e = upload_shape(s, st);
@@ -220,7 +200,7 @@ cudaError_t launch_fwd_fkpp_f64(const Shape64Host &s, const Fwd64Host &p, const 
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.tgrid = a.tgrid; q.nacc = a.nacc;
     q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.max_steps = a.max_steps;
     q.t0 = a.t0; q.save_dt = a.save_dt; q.abstol = a.abstol; q.reltol = a.reltol;
-    auto kern = fkpp_adapt::forward_kernel<FkppOps64>;
+    auto kern = fkpp_adapt::forward_kernel<Ops64>;
     const size_t smem = fkpp_adapt::fwd_smem(s.D, sizeof(double));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -237,7 +217,7 @@ cudaError_t launch_adj_fkpp_f64(const Shape64Host &s, const Adj64Host &p, const 
     fkpp_adapt::cta_geometry(s.D, &q.tpc, &th);
     q.ustep = p.ustep; q.dense = p.dense; q.tgrid = a.tgrid; q.nacc = a.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.t0 = a.t0; q.save_dt = a.save_dt;
-    auto kern = fkpp_adapt::adjoint_kernel<FkppOps64>;
+    auto kern = fkpp_adapt::adjoint_kernel<Ops64>;
     const size_t smem = fkpp_adapt::adj_smem(s.D, s.P, sizeof(double));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -258,7 +238,7 @@ cudaError_t launch_fwd_fkpp_vern7_f64(const Shape64Host &s, const Fwd64Host &p, 
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.hstep = a.hstep; q.status = p.status; q.tgrid = a.tgrid; q.nacc = a.nacc;
     q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.max_steps = a.max_steps;
     q.t0 = a.t0; q.save_dt = a.save_dt; q.abstol = a.abstol; q.reltol = a.reltol;
-    auto kern = fkpp_vern7::vern7_forward_kernel<FkppOps64>;
+    auto kern = fkpp_vern7::vern7_forward_kernel<Ops64>;
     const size_t smem = fkpp_adapt::fwd_smem(s.D, sizeof(double));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -276,7 +256,7 @@ cudaError_t launch_adj_fkpp_vern7_f64(const Shape64Host &s, const Adj64Host &p, 
     q.ustep = p.ustep; q.hstep = a.hstep; q.tgrid = a.tgrid; q.nacc = a.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = s.D; q.n_save = a.n_save; q.fused_l2 = p.fused_l2; q.t0 = a.t0; q.save_dt = a.save_dt;
     q.margin = 5e-13;   // half the clipping margin of the forward
-    auto kern = fkpp_vern7::discrete_adjoint_kernel<FkppOps64>;
+    auto kern = fkpp_vern7::discrete_adjoint_kernel<Ops64>;
     const size_t smem = fkpp_adapt::adj_smem(s.D, s.P, sizeof(double));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

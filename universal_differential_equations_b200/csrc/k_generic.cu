@@ -1,4 +1,6 @@
-// k_generic.cu -- shape-generic UDE kernels (runtime chain widths / activations; LV, SEIR, NODE forms).
+// k_generic.cu -- shape-generic UDE kernels (runtime chain widths / activations; LV, SEIR, NODE forms) in fp32, and the
+// fixed-step Fisher-KPP kernels.
+#include "ude_adjoint.cuh"
 #include "ude_generic.cuh"
 #include "fkpp_adaptive.cuh"
 #include "discrete_adjoint.cuh"
@@ -9,6 +11,40 @@
 #include <algorithm>
 
 namespace b200ude {
+
+namespace generic {
+struct GenDesc {
+    int model, D, din, dout, n_layers, n_prefix, P;
+    int widths[MAXL + 1];
+    int acts[MAXL];
+    int woff[MAXL];   // offset of layer l's W in theta (column-major, out x in), its bias follows at woff + in*out
+};
+static __constant__ GenDesc c_gen;
+}  // namespace generic
+
+// the fp32 precision of the runtime-shape model layer: theta, constants and loss weights from the constant bank, the MUFU
+// activations of the specialised kernels
+struct Ops32 {
+    using real = float;
+    using Fwd = FwdParams;
+    using Adj = AdjParams;
+    using Adapt = AdaptiveGrid;
+    static constexpr int MAXD = generic::MAXD;
+    static __device__ __forceinline__ int model() { return generic::c_gen.model; }
+    static __device__ __forceinline__ int D() { return generic::c_gen.D; }
+    static __device__ __forceinline__ int din() { return generic::c_gen.din; }
+    static __device__ __forceinline__ int dout() { return generic::c_gen.dout; }
+    static __device__ __forceinline__ int n_layers() { return generic::c_gen.n_layers; }
+    static __device__ __forceinline__ int n_prefix() { return generic::c_gen.n_prefix; }
+    static __device__ __forceinline__ int P() { return generic::c_gen.P; }
+    static __device__ __forceinline__ int width(int l) { return generic::c_gen.widths[l]; }
+    static __device__ __forceinline__ int woff(int l) { return generic::c_gen.woff[l]; }
+    static __device__ __forceinline__ int layer_act(int l) { return generic::c_gen.acts[l]; }
+    static __device__ __forceinline__ const float &theta(int i) { return c_theta[i]; }
+    static __device__ __forceinline__ const float &consts(int i) { return c_consts[i]; }
+    static __device__ __forceinline__ const float &lossw(int c) { return c_lossw[c]; }
+    static __device__ __forceinline__ float act(int k, float a) { return k == ACT_TANH ? tanh_dev<0>(a) : (k == ACT_RBF ? rbf_dev(a) : a); }
+};
 
 constexpr int GEN_BLOCK = 128;
 
@@ -38,7 +74,7 @@ cudaError_t launch_fwd_generic(const GenericShape &g, const ConstTables &t, cons
     if (e != cudaSuccess) return e;
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
-    generic::forward_kernel<GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p);
+    generic::forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p);
     return cudaGetLastError();
 }
 
@@ -48,7 +84,7 @@ cudaError_t launch_adj_generic(const GenericShape &g, const ConstTables &t, cons
     if (e != cudaSuccess) return e;
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
-    auto kern = generic::adjoint_kernel<GEN_BLOCK>;
+    auto kern = generic::adjoint_kernel<Ops32, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -64,7 +100,7 @@ cudaError_t launch_fwd_vern7(const GenericShape &g, const ConstTables &t, const 
     if (e != cudaSuccess) return e;
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
-    generic::vern7_forward_kernel<GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p);
+    generic::vern7_forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p);
     return cudaGetLastError();
 }
 
@@ -75,26 +111,11 @@ cudaError_t launch_fwd_vern7_adaptive(const GenericShape &g, const ConstTables &
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
     // the step record only for the discrete adjoint (p.ustep set); the interpolating adjoint re-solves with Tsit5
-    const bool rec = p.ustep != nullptr;
-    generic::AdaptParams ap{ag.t0, ag.save_dt, ag.abstol, ag.reltol, ag.n_save, ag.max_steps, rec ? ag.tgrid : nullptr, rec ? ag.nacc : nullptr,
-                            rec ? ag.hstep : nullptr};
-    generic::vern7_adaptive_forward_kernel<GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ap);
+    generic::vern7_adaptive_forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ag);
     return cudaGetLastError();
 }
 
-// ---- discrete adjoint (discrete_adjoint.cuh in fp32: theta from the constant bank, runtime chain shape) ----
-struct DiscreteOps32 {
-    using real = float;
-    static constexpr int MAXD = generic::MAXD;
-    static __device__ __forceinline__ int D() { return generic::c_gen.D; }
-    static __device__ __forceinline__ int P() { return generic::c_gen.P; }
-    static __device__ __forceinline__ float lossw(int c) { return c_lossw[c]; }
-    static __device__ __forceinline__ void rhs(const float *u, float *du) { generic::model_rhs(u, du); }
-    static __device__ __forceinline__ void vjp(const float *u, const float *g, float lv, float *kl, float *gw, int lane)
-    {
-        generic::model_vjp(u, g, 1.0f, lv, kl, gw, lane);
-    }
-};
+// ---- discrete adjoint (discrete_adjoint.cuh in fp32) ----
 
 cudaError_t launch_adj_discrete(const GenericShape &g, const ConstTables &t, const AdjParams &p, int solver, const AdaptiveGrid *ag,
                                 cudaStream_t st, int *rows_out)
@@ -109,8 +130,8 @@ cudaError_t launch_adj_discrete(const GenericShape &g, const ConstTables &t, con
     q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
     q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
     q.margin = 5e-7f;   // half the clipping margin of vern7_adaptive_forward_kernel
-    auto kern = solver == 1 ? discrete::adjoint_kernel<DiscreteOps32, discrete::Vern7Scheme, GEN_BLOCK>
-                            : discrete::adjoint_kernel<DiscreteOps32, discrete::Tsit5Scheme, GEN_BLOCK>;
+    auto kern = solver == 1 ? discrete::adjoint_kernel<Ops32, discrete::Vern7Scheme, GEN_BLOCK>
+                            : discrete::adjoint_kernel<Ops32, discrete::Tsit5Scheme, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -121,12 +142,6 @@ cudaError_t launch_adj_discrete(const GenericShape &g, const ConstTables &t, con
 }
 
 // ---- Vern7 with its lazy dense output (vern7_dense.cuh in fp32) ----
-struct DenseOps32 : DiscreteOps32 {
-    static __device__ __forceinline__ void vjp(const float *u, const float *g, float sc, float lv, float *kl, float *gw, int lane)
-    {
-        generic::model_vjp(u, g, sc, lv, kl, gw, lane);
-    }
-};
 
 cudaError_t launch_fwd_vern7_dense(const GenericShape &g, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
 {
@@ -138,7 +153,7 @@ cudaError_t launch_fwd_vern7_dense(const GenericShape &g, const ConstTables &t, 
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.tgrid = ag.tgrid; q.hstep = ag.hstep; q.nacc = ag.nacc; q.status = p.status;
     q.N = p.N; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
     q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    vern7_dense::forward_kernel<DenseOps32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(q);
+    vern7_dense::forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(q);
     return cudaGetLastError();
 }
 
@@ -154,7 +169,7 @@ cudaError_t launch_adj_vern7_dense(const GenericShape &g, const ConstTables &t, 
     q.cot = p.cot; q.saved = saved; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
     q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
-    auto kern = vern7_dense::adjoint_kernel<DenseOps32, GEN_BLOCK>;
+    auto kern = vern7_dense::adjoint_kernel<Ops32, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -176,7 +191,7 @@ cudaError_t launch_adj_vern7_dense_discrete(const GenericShape &g, const ConstTa
     q.ustep = p.ustep; q.tgrid = ag.tgrid; q.hstep = ag.hstep; q.nacc = ag.nacc; q.cot = p.cot; q.saved = saved;
     q.grad_u0 = p.grad_u0; q.partial = p.partial; q.N = p.N; q.n_save = ag.n_save; q.fused_l2 = p.fused_l2;
     q.t0 = ag.t0; q.save_dt = ag.save_dt;
-    auto kern = vern7_dense_discrete::adjoint_kernel<DiscreteOps32, GEN_BLOCK>;
+    auto kern = vern7_dense_discrete::adjoint_kernel<Ops32, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -193,8 +208,7 @@ cudaError_t launch_fwd_adaptive(const GenericShape &g, const ConstTables &t, con
     if (e != cudaSuccess) return e;
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
-    generic::AdaptParams ap{ag.t0, ag.save_dt, ag.abstol, ag.reltol, ag.n_save, ag.max_steps, ag.tgrid, ag.nacc};
-    generic::adaptive_forward_kernel<GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ap);
+    generic::adaptive_forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ag);
     return cudaGetLastError();
 }
 
@@ -204,14 +218,13 @@ cudaError_t launch_adj_adaptive(const GenericShape &g, const ConstTables &t, con
     if (e != cudaSuccess) return e;
     e = upload_gen(g, st);
     if (e != cudaSuccess) return e;
-    generic::AdaptParams ap{ag.t0, ag.save_dt, ag.abstol, ag.reltol, ag.n_save, ag.max_steps, ag.tgrid, ag.nacc};
-    auto kern = generic::adaptive_adjoint_kernel<GEN_BLOCK>;
+    auto kern = generic::adaptive_adjoint_kernel<Ops32, GEN_BLOCK>;
     const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
     *rows_out = grid * (GEN_BLOCK / 32);
-    kern<<<grid, GEN_BLOCK, smem, st>>>(p, ap);
+    kern<<<grid, GEN_BLOCK, smem, st>>>(p, ag);
     return cudaGetLastError();
 }
 
@@ -256,19 +269,158 @@ cudaError_t launch_l2_finish(const float *block_loss, float *loss, cudaStream_t 
     return cudaGetLastError();
 }
 
-// ---- Fisher-KPP ----
-static void fkpp_geom(int Nx, generic::FkppGeom *g, int *threads)
+// =====================================================================================================
+// Fisher-KPP UPDE, fixed step (FisherKPP/Fisher-KPP-CNN.jl:111-126, LotkaVolterra/scenario_3.jl:103-114), fp32:
+//   du_i = NN(u_i) + D0 * (w1 u_{i-1} + w2 u_i + w3 u_{i+1}),  periodic, theta = [chain | w1 w2 w3 b | D0].
+// One thread per grid point; a CTA holds `tpc` whole trajectories (tpc * Nx threads, rounded up to a warp
+// multiple: fkpp_adapt::cta_geometry); neighbours are exchanged through shared memory.  The handle's internal stores (ustep,
+// dense) are point-fastest ([row][trajectory][point]) so that every warp access is contiguous; the ABI arrays
+// (u0, out, data, grad_u0) keep the documented trajectory-fastest layout.
+// =====================================================================================================
+static __global__ void fkpp_forward_kernel(FwdParams p, int Nx, int tpc)
 {
-    g->Nx = Nx;
-    g->tpc = Nx >= 128 ? 1 : 128 / Nx;
-    *threads = ((g->tpc * Nx + 31) / 32) * 32;
+    extern __shared__ __align__(16) float s_dyn[];
+    float *sU = s_dyn;
+    const int slots = tpc * Nx;
+    const int slot = threadIdx.x;
+    const bool valid = slot < slots;
+    const int t_loc = valid ? slot / Nx : 0, i = valid ? slot % Nx : 0;
+    const int base = t_loc * Nx;
+    const int traj = blockIdx.x * tpc + t_loc;
+    const bool live = valid && traj < p.N;
+    const size_t N = (size_t)p.N, n = (size_t)(live ? traj : p.N - 1);
+    const float dt = p.dt;
+    const int sx = Ops32::P() - 5;
+    const float w1 = Ops32::theta(sx), w2 = Ops32::theta(sx + 1), w3 = Ops32::theta(sx + 2), D0 = Ops32::theta(sx + 4);
+    float u = __ldg(p.u0 + (size_t)i * N + n);
+    auto rhs = [&](float g) {
+        float gm, gp;
+        fkpp_adapt::exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
+        const float y = fkpp_adapt::point_chain<Ops32>(g);
+        return fmaf(D0, fmaf(w1, gm, fmaf(w2, g, w3 * gp)), y);
+    };
+    auto store_int = [&](float *b, int row, float v) { if (live) b[((size_t)row * N + n) * Nx + i] = v; };
+    auto store_abi = [&](float *b, int row, float v) { if (live) b[((size_t)row * Nx + i) * N + n] = v; };
+    store_abi(p.out, 0, u);
+    store_int(p.ustep, 0, u);
+    float k[7];
+    k[0] = rhs(u);
+    store_int(p.dense, 0, k[0]);
+    int isave = 1;
+    for (int s = 0; s < p.n_steps; ++s) {
+#pragma unroll
+        for (int st = 1; st < 7; ++st) {
+            float acc = 0.0f;
+#pragma unroll
+            for (int j = 0; j < st; ++j)
+                if (Tsit5::a(st, j) != 0.0) acc = fmaf((float)Tsit5::a(st, j), k[j], acc);
+            const float g = fmaf(dt, acc, u);
+            if (st == 6) u = g;
+            k[st] = rhs(g);
+            store_int(p.dense, s * 6 + st, k[st]);
+        }
+        store_int(p.ustep, s + 1, u);
+        if ((s + 1) % p.save_every == 0) { store_abi(p.out, isave, u); ++isave; }
+        k[0] = k[6];
+    }
+    if (p.status) {
+        // a trajectory is flagged when any of its points is non-finite
+        const float big = Prec<float>::huge;
+        const int bad = __syncthreads_or((live && !(fabsf(u) <= big)) ? 1 : 0);   // CTA-wide; refined per trajectory below
+        if (bad) {
+            if (valid) sU[slot] = (fabsf(u) <= big) ? 0.0f : 1.0f;
+            __syncthreads();
+            if (live && i == 0) {
+                float any = 0.0f;
+                for (int q = 0; q < Nx; ++q) any += sU[base + q];
+                p.status[n] = any > 0.0f ? 1 : 0;
+            }
+        } else if (live && i == 0) {
+            p.status[n] = 0;
+        }
+    }
+}
+
+static __global__ void fkpp_adjoint_kernel(AdjParams p, int Nx, int tpc)
+{
+    extern __shared__ __align__(16) float s_dyn[];
+    const int slots = tpc * Nx, P = Ops32::P();
+    float *sU = s_dyn;                                   // [slots] neighbour exchange
+    float *s_g = s_dyn + ((slots + 3) / 4) * 4;          // [nwarps][P+1]
+    const int slot = threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float *gw = s_g + (size_t)warp * (P + 1);
+    for (int q = lane; q < P + 1; q += 32) gw[q] = 0.0f;
+    __syncwarp();
+    const bool valid = slot < slots;
+    const int t_loc = valid ? slot / Nx : 0, i = valid ? slot % Nx : 0;
+    const int base = t_loc * Nx;
+    const int traj = blockIdx.x * tpc + t_loc;
+    const bool live = valid && traj < p.N;
+    const size_t N = (size_t)p.N, n = (size_t)(live ? traj : p.N - 1);
+    const float lv = live ? 1.0f : 0.0f;
+    const float dt = p.dt;
+    const int sx = P - 5;
+    const float w1 = Ops32::theta(sx), w2 = Ops32::theta(sx + 1), w3 = Ops32::theta(sx + 2), D0 = Ops32::theta(sx + 4);
+    float lam = 0.0f, loss = 0.0f, kl[6];
+    auto jump = [&](int isave) {
+        const size_t idx = ((size_t)isave * Nx + i) * N + n;   // ABI layout
+        if (p.fused_l2) {
+            const float r = __ldg(p.ustep + ((size_t)(isave * p.save_every) * N + n) * Nx + i) - __ldg(p.cot + idx);
+            loss = fmaf(r, r, loss);
+            lam = fmaf(2.0f, r, lam);
+        } else {
+            lam += __ldg(p.cot + idx);
+        }
+    };
+    const int n_save = p.n_steps / p.save_every + 1;
+    jump(n_save - 1);
+    for (int s = p.n_steps - 1; s >= 0; --s) {
+#pragma unroll
+        for (int st = 0; st < 6; ++st) {
+            float acc = 0.0f;
+#pragma unroll
+            for (int j = 0; j < 7; ++j)
+                if (Tsit5::bw(st, j) != 0.0)
+                    acc = fmaf((float)Tsit5::bw(st, j), __ldg(p.dense + ((size_t)(s * 6 + j) * N + n) * Nx + i), acc);
+            const float x = fmaf(dt, acc, __ldg(p.ustep + ((size_t)s * N + n) * Nx + i));
+            float a2 = 0.0f;
+#pragma unroll
+            for (int j = 0; j < st; ++j)
+                if (Tsit5::a(st, j) != 0.0) a2 = fmaf((float)Tsit5::a(st, j), kl[j], a2);
+            const float g = fmaf(dt, a2, lam);
+            const float w = dt * (float)Tsit5::b(st) * lv;
+            // neighbours of u (for the stencil-weight gradients) and of lambda (for the transposed stencil)
+            float xm, xp, gm, gp;
+            fkpp_adapt::exchange(sU, slot, base, i, Nx, valid, x, xm, xp);
+            fkpp_adapt::exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
+            const float dx = fkpp_adapt::point_chain_vjp<Ops32>(x, g, w, gw, lane);
+            kl[st] = dx + D0 * fmaf(w2, g, fmaf(w1, gp, w3 * gm));   // (J^T g)_i: w1 couples i+1 -> i, w3 couples i-1 -> i
+            generic::warp_acc(gw, sx + 0, w * D0 * xm * g, lane);
+            generic::warp_acc(gw, sx + 1, w * D0 * x * g, lane);
+            generic::warp_acc(gw, sx + 2, w * D0 * xp * g, lane);
+            generic::warp_acc(gw, sx + 4, w * fmaf(w1, xm, fmaf(w2, x, w3 * xp)) * g, lane);
+        }
+        float acc = 0.0f;
+#pragma unroll
+        for (int j = 0; j < 6; ++j) acc = fmaf((float)Tsit5::b(j), kl[j], acc);
+        lam = fmaf(dt, acc, lam);
+        if (s % p.save_every == 0) jump(s / p.save_every);
+    }
+    if (p.grad_u0 && live) p.grad_u0[(size_t)i * N + n] = lam;
+    loss *= lv;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    if (lane == 0) gw[P] = loss;
+    __syncwarp();
+    float *dst = p.partial + ((size_t)blockIdx.x * (blockDim.x >> 5) + warp) * (P + 1);
+    for (int q = lane; q < P + 1; q += 32) dst[q] = gw[q];
 }
 
 int adj_rows_fkpp(int N, int Nx)
 {
-    generic::FkppGeom g; int th;
-    fkpp_geom(Nx, &g, &th);
-    return ((N + g.tpc - 1) / g.tpc) * (th / 32);
+    int tpc, th;
+    fkpp_adapt::cta_geometry(Nx, &tpc, &th);
+    return ((N + tpc - 1) / tpc) * (th / 32);
 }
 
 cudaError_t launch_fwd_fkpp(const GenericShape &gs, const ConstTables &t, const FwdParams &p, cudaStream_t st)
@@ -277,10 +429,10 @@ cudaError_t launch_fwd_fkpp(const GenericShape &gs, const ConstTables &t, const 
     if (e != cudaSuccess) return e;
     e = upload_gen(gs, st);
     if (e != cudaSuccess) return e;
-    generic::FkppGeom g; int th;
-    fkpp_geom(gs.D, &g, &th);
-    const int grid = (p.N + g.tpc - 1) / g.tpc;
-    generic::fkpp_forward_kernel<0><<<grid, th, sizeof(float) * g.tpc * g.Nx, st>>>(p, g);
+    int tpc, th;
+    fkpp_adapt::cta_geometry(gs.D, &tpc, &th);
+    const int grid = (p.N + tpc - 1) / tpc;
+    fkpp_forward_kernel<<<grid, th, sizeof(float) * tpc * gs.D, st>>>(p, gs.D, tpc);
     return cudaGetLastError();
 }
 
@@ -290,40 +442,18 @@ cudaError_t launch_adj_fkpp(const GenericShape &gs, const ConstTables &t, const 
     if (e != cudaSuccess) return e;
     e = upload_gen(gs, st);
     if (e != cudaSuccess) return e;
-    generic::FkppGeom g; int th;
-    fkpp_geom(gs.D, &g, &th);
-    const int grid = (p.N + g.tpc - 1) / g.tpc;
-    const size_t smem = sizeof(float) * (((g.tpc * g.Nx + 3) / 4) * 4 + (size_t)(th / 32) * (gs.P + 1));
-    auto kern = generic::fkpp_adjoint_kernel<0>;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int tpc, th;
+    fkpp_adapt::cta_geometry(gs.D, &tpc, &th);
+    const int grid = (p.N + tpc - 1) / tpc;
+    const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
+    e = cudaFuncSetAttribute(fkpp_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     *rows_out = grid * (th / 32);
-    kern<<<grid, th, smem, st>>>(p, g);
+    fkpp_adjoint_kernel<<<grid, th, smem, st>>>(p, gs.D, tpc);
     return cudaGetLastError();
 }
 
-// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp32: theta from the constant bank, runtime chain shape) ----
-struct FkppOps32 {
-    using real = float;
-    static __device__ __forceinline__ float theta(int i) { return c_theta[i]; }
-    static __device__ __forceinline__ int P() { return generic::c_gen.P; }
-    static __device__ __forceinline__ float chain(float x)
-    {
-        float y;
-        generic::chain_fwd<false>(&x, &y, nullptr, nullptr);
-        return y;
-    }
-    static __device__ __forceinline__ float chain_vjp(float x, float dy, float w, float *gw, int lane)
-    {
-        float dx;
-        generic::chain_vjp(&x, &dy, w, &dx, gw, lane);
-        return dx;
-    }
-    static __device__ __forceinline__ void warp_acc(float *gw, int idx, float v, int lane) { generic::warp_acc(gw, idx, v, lane); }
-    static __device__ __forceinline__ void interp(float Th, float *bw) { generic::tsit5_bw_rt(Th, bw); }
-    static __device__ __forceinline__ float btilde(int j) { return generic::tsit5_btilde(j); }
-};
-
+// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp32) ----
 size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes)
 {
     return std::max(fkpp_adapt::fwd_smem(Nx, real_bytes), fkpp_adapt::adj_smem(Nx, P, real_bytes));
@@ -341,7 +471,7 @@ cudaError_t launch_fwd_fkpp_adaptive(const GenericShape &gs, const ConstTables &
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
     q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
     q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    auto kern = fkpp_adapt::forward_kernel<FkppOps32>;
+    auto kern = fkpp_adapt::forward_kernel<Ops32>;
     const size_t smem = fkpp_adapt::fwd_smem(gs.D, sizeof(float));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -360,7 +490,7 @@ cudaError_t launch_adj_fkpp_adaptive(const GenericShape &gs, const ConstTables &
     fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
     q.ustep = p.ustep; q.dense = p.dense; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.t0 = ag.t0; q.save_dt = ag.save_dt;
-    auto kern = fkpp_adapt::adjoint_kernel<FkppOps32>;
+    auto kern = fkpp_adapt::adjoint_kernel<Ops32>;
     const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -383,7 +513,7 @@ cudaError_t launch_fwd_fkpp_vern7(const GenericShape &gs, const ConstTables &t, 
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.hstep = ag.hstep; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
     q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
     q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    auto kern = fkpp_vern7::vern7_forward_kernel<FkppOps32>;
+    auto kern = fkpp_vern7::vern7_forward_kernel<Ops32>;
     const size_t smem = fkpp_adapt::fwd_smem(gs.D, sizeof(float));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -403,7 +533,7 @@ cudaError_t launch_adj_fkpp_vern7(const GenericShape &gs, const ConstTables &t, 
     q.ustep = p.ustep; q.hstep = ag.hstep; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.fused_l2 = p.fused_l2; q.t0 = ag.t0; q.save_dt = ag.save_dt;
     q.margin = 5e-7f;   // half the clipping margin of the forward
-    auto kern = fkpp_vern7::discrete_adjoint_kernel<FkppOps32>;
+    auto kern = fkpp_vern7::discrete_adjoint_kernel<Ops32>;
     const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;

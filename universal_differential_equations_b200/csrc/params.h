@@ -7,6 +7,10 @@
 
 namespace b200ude {
 
+// model and activation codes (B200UDE_MODEL_*, B200UDE_ACT_*)
+constexpr int MODEL_LV = 0, MODEL_SEIR = 1, MODEL_FKPP = 2, MODEL_NODE = 3, MODEL_SEIR_NODE = 4;
+constexpr int ACT_IDENTITY = 0, ACT_TANH = 1, ACT_RBF = 2;
+
 struct FwdParams {
     const float *u0;    // [D][N]
     float *out;         // [n_save][D][N]
@@ -178,7 +182,8 @@ struct PeerLinks {
 cudaError_t launch_reduce_exchange(const float *partial, int nblocks, int P1, const PeerLinks &, float *grad, float *loss, cudaStream_t);
 cudaError_t launch_reduce(const float *partial, int nblocks, int P1, float *grad, float *loss, cudaStream_t);
 
-// ---- double-precision path (dtype = B200UDE_F64; k_f64.cu / ude_f64.cuh) ----
+// ---- double-precision path (dtype = B200UDE_F64; k_f64.cu).  Fwd64Host / Adj64Host / Adapt64Host are also the parameters of the
+// fp64 runtime-shape kernels (ude_generic.cuh), as FwdParams / AdjParams / AdaptiveGrid are of the fp32 ones ----
 struct Shape64Host {
     uint64_t serial;
     int model, D, din, dout, n_layers, n_prefix, P;

@@ -29,8 +29,7 @@
 
 namespace b200ude {
 
-constexpr int MODEL_LV = 0, MODEL_SEIR = 1, MODEL_FKPP = 2, MODEL_NODE = 3, MODEL_SEIR_NODE = 4;
-constexpr int ACT_IDENTITY = 0, ACT_TANH = 1, ACT_RBF = 2, ACT_RUNTIME = -1;
+constexpr int ACT_RUNTIME = -1;   // the activation of each layer read from c_acts (the other codes are in params.h)
 constexpr int GRAD_LANE = 0;   // every lane keeps all P partial sums in registers (small chains)
 constexpr int GRAD_WARPGEMM = 1;  // H x H layer via per-warp smem-staged outer-product GEMM
 

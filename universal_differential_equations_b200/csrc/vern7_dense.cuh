@@ -24,12 +24,13 @@
 // grid the warp loops over its longest record, shorter records shadow step 0 with zero weight, and every lane walks its own
 // pieces with a warp-uniform trip count, so a trajectory's results do not depend on its neighbours.
 //
-// `Ops` supplies the precision: real, MAXD, D(), P(), lossw(c), rhs(u, du), vjp(u, g, sc, lv, kl, gw, lane) (kl = J_u^T g;
-// gw += sc lv J_theta^T g, all lanes participating).  k_generic.cu instantiates it in fp32, k_f64.cu in fp64.
+// `Ops` is the precision of the runtime-shape model layer (ude_generic.cuh): k_generic.cu instantiates it in fp32 (Ops32),
+// k_f64.cu in fp64 (Ops64).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ude_generic.cuh"
 #include "vern7.cuh"
 
 namespace b200ude {
@@ -211,32 +212,6 @@ struct Vern7Dense {
 
 namespace vern7_dense {
 
-// per-precision margins and math (the fp32 ones are those of the fp32 Vern7 kernels, the fp64 ones those of the fp64 kernels)
-template <typename R>
-struct Prec;
-template <>
-struct Prec<float> {
-    static constexpr float clip = 1e-6f;   // a step within clip |t1| of the end of tspan is stretched to it
-    static constexpr float eta = 1e-5f;    // a save time within eta h of a step end is that step end
-    static constexpr float huge = 3.0e38f;
-    static __device__ __forceinline__ float nan() { return __int_as_float(0x7fc00000); }
-    static __device__ __forceinline__ float pw(float a, float b) { return powf(a, b); }
-    static __device__ __forceinline__ float sq(float a) { return sqrtf(a); }
-    static __device__ __forceinline__ float lg(float a) { return log10f(a); }
-    static __device__ __forceinline__ float ex(float a) { return exp10f(a); }
-};
-template <>
-struct Prec<double> {
-    static constexpr double clip = 1e-12;
-    static constexpr double eta = 1e-10;
-    static constexpr double huge = 1.0e300;
-    static __device__ __forceinline__ double nan() { return __longlong_as_double(0x7ff8000000000000LL); }
-    static __device__ __forceinline__ double pw(double a, double b) { return pow(a, b); }
-    static __device__ __forceinline__ double sq(double a) { return sqrt(a); }
-    static __device__ __forceinline__ double lg(double a) { return log10(a); }
-    static __device__ __forceinline__ double ex(double a) { return exp10(a); }
-};
-
 // the point stage i of a step from u with step h is evaluated at: g = u + h sum_j a_ij k_j (the expression of the Vern7 forward
 // kernels)
 template <class Ops, int I>
@@ -263,7 +238,7 @@ __device__ __forceinline__ void stage(const typename Ops::real *u, typename Ops:
                                       typename Ops::real *g)
 {
     stage_point<Ops, I>(u, h, k, g);
-    Ops::rhs(g, k[I]);
+    generic::model_rhs<Ops>(g, k[I]);
 }
 
 // the extra stages k_11..k_16 (indices 10..15) of a step whose k_1..k_9 are in k
@@ -347,7 +322,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
         p.ustep[(size_t)c * N + n] = u[c];
     }
     p.tgrid[n] = t0;
-    Ops::rhs(u, k[0]);
+    generic::model_rhs<Ops>(u, k[0]);
     R dt;
     {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
         R d0 = 0, d1 = 0, d2 = 0;
@@ -360,7 +335,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
         R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
         dt0 = fmin(dt0, t1 - t0);
         for (int c = 0; c < D; ++c) g[c] = fma(dt0, k[0][c], u[c]);
-        Ops::rhs(g, un);
+        generic::model_rhs<Ops>(g, un);
         for (int c = 0; c < D; ++c) {
             const R sk = abstol + reltol * fabs(u[c]);
             const R e = (un[c] - k[0][c]) / sk;
@@ -378,7 +353,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
         R h = dt;
         bool clipped = false;
         if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
-        if (!have_k1) Ops::rhs(u, k[0]);
+        if (!have_k1) generic::model_rhs<Ops>(u, k[0]);
         stage<Ops, 1>(u, h, k, g);
         stage<Ops, 2>(u, h, k, g);
         stage<Ops, 3>(u, h, k, g);
@@ -518,7 +493,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Adj<typename Ops::rea
         const R eps = PR::eta * (tn1 - tn);
         for (int c = 0; c < D; ++c) u[c] = p.ustep[((size_t)sr * D + c) * N + n];
         // k_1..k_9 as the forward evaluated them, then the extra stages
-        Ops::rhs(u, k[0]);
+        generic::model_rhs<Ops>(u, k[0]);
         stage<Ops, 1>(u, h, k, g);
         stage<Ops, 2>(u, h, k, g);
         stage<Ops, 3>(u, h, k, g);
@@ -559,7 +534,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Adj<typename Ops::rea
                         if (Vern7::a(i, j) != 0.0) a2 = fma((R)Vern7::a(i, j), kl[j][c], a2);
                     g[c] = fma(hs, a2, lam[c]);
                 }
-                Ops::vjp(x, g, hs * (R)Vern7::b(i), has ? (R)1 : (R)0, kl[i], gw, lane);
+                generic::model_vjp<Ops>(x, g, hs * (R)Vern7::b(i), has ? (R)1 : (R)0, kl[i], gw, lane);
             }
             if (has) {
                 for (int c = 0; c < D; ++c) {

@@ -26,7 +26,7 @@
 // zero cotangent (exact zeros into the sums), so the shuffles stay convergent and a trajectory's grad_u0 does not depend on its
 // neighbours.  The loop over a step's save points holds no collective and runs per lane.
 //
-// `Ops` is discrete_adjoint.cuh's: real, MAXD, D(), P(), lossw(c), rhs(u, du), vjp(u, g, lv, kl, gw, lane).
+// `Ops` is the precision of the runtime-shape model layer (ude_generic.cuh), as in discrete_adjoint.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -71,14 +71,14 @@ __device__ __forceinline__ void back_stage(const typename Ops::real *u, typename
             if (j != 9 && a_all(j, I) != 0.0) acc = fma((R)a_all(j, I), gb[j][c], acc);
         kb[c] = act ? h * acc : (R)0;
     }
-    Ops::vjp(g, kb, act ? (R)1 : (R)0, gb[I], gw, lane);
+    generic::model_vjp<Ops>(g, kb, (R)1, act ? (R)1 : (R)0, gb[I], gw, lane);
 }
 
 template <class Ops, int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Params<typename Ops::real> p)
 {
     using R = typename Ops::real;
-    using PR = vern7_dense::Prec<R>;
+    using PR = Prec<R>;
     constexpr int MAXD = Ops::MAXD;
     extern __shared__ __align__(16) unsigned char s_raw[];
     R *s_g = reinterpret_cast<R *>(s_raw);   // [BLOCK/32][P+1]
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Params<typename Ops::
             }
         const bool extra = __any_sync(0xffffffffu, inner);
         // k_0..k_8 as the forward evaluated them, then the extra stages where a save point needs them
-        Ops::rhs(u, k[0]);
+        generic::model_rhs<Ops>(u, k[0]);
         vern7_dense::stage<Ops, 1>(u, h, k, g);
         vern7_dense::stage<Ops, 2>(u, h, k, g);
         vern7_dense::stage<Ops, 3>(u, h, k, g);
