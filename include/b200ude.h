@@ -74,6 +74,21 @@ extern "C" {
 #define B200UDE_MODEL_NODE 3 /* du = NN(u) */
 #define B200UDE_MODEL_SEIR_NODE 4 /* the SEIR script's black-box baseline dudt_node: dS,dE,dI,dR,dD = first five outputs of
                                      NN([S/N,E,I,R,N,D/N,C]), dN = -mu N, dC = sigma E   seir_exposure.jl:52-64; consts as MODEL_SEIR */
+#define B200UDE_MODEL_FORCED 5 /* forced neural ODE with a readout network (NonNewtonianFluids/FENEP.jl:41-62):
+                                    du = f1([u; gamma(t)]),  readout y = f0([u; gamma(t)]),
+                                    gamma_n(t) = sum_j A_jn cos(w_jn t + phi_jn), per-trajectory coefficients (b200ude_set_forcing).
+                                  Descriptor: state_dim = d; consts[0] = L0 (layers of f0), consts[1] = J (harmonics, 1..4),
+                                  n_consts = 2; n_layers = L0 + L1; widths[0 .. L0] = f0 (d+1 -> ... -> r), then
+                                  widths[L0+1 .. L0+L1+1] = f1 (d+1 -> ... -> d), so L0 + L1 <= 5; acts[] in the same order
+                                  (f0's then f1's).  theta = f0's layers then f1's, each vec(W) column-major then b
+                                  (Flux.params(f0, f1), FENEP.jl:98); n_prefix = n_suffix = 0.  Envelope: widths <= 64, d + 1 <= 8,
+                                  r <= 8, P <= 12288 in fp32.
+                                  Rows: out, data and dL_dout have d + r rows per save, [n_save][d + r][N]: rows 0..d-1 the
+                                  states, rows d..d+r-1 the readout at the saved states; grad_u0 stays [d][N]; n_loss_weights
+                                  is 0 or d + r.  Tsit5, fixed step or adaptive, interpolating adjoint, fp32 and fp64 (the
+                                  interpolating adjoint stands for the reference's Tracker gradient through the solver; the two
+                                  agree to the solve tolerance).  The fused L2 recomputes the readout from the saved state.
+                                  Vern7, RKC2, the discrete adjoint and the dense flags return B200UDE_EUNSUPPORTED. */
 
 /* activations of the dense chain */
 #define B200UDE_ACT_IDENTITY 0
@@ -205,6 +220,12 @@ size_t b200ude_device_bytes(const b200ude_handle *h);
 
 /* theta[P] (float) from host or device memory -> the handle's device copy. */
 int32_t b200ude_set_params(b200ude_handle *h, const void *theta, size_t P, int32_t mem, void *stream);
+
+/* FORCING of a B200UDE_MODEL_FORCED handle: coef [3J][N] in the handle's dtype (host or device memory per `mem`), rows
+ * (A_j, w_j, phi_j) for j = 0..J-1, so that gamma_n(t) = sum_j A_jn cos(w_jn t + phi_jn).  The handle keeps a device copy
+ * (capacity max_trajectories) that forward, solve_host, loss_gradient_host and train_adam read; calling them with more
+ * trajectories than were last set is B200UDE_ESTATE.  Stream-ordered on `stream`.  Any other model: B200UDE_EUNSUPPORTED. */
+int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32_t mem, void *stream);
 
 /* FORWARD  (replaces: the UDE RHS closure + OrdinaryDiffEq perform_step! loop behind
  * concrete_solve(prob, Tsit5(), u0, p; saveat, ...), one trajectory per ensemble member).

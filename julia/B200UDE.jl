@@ -25,7 +25,12 @@ const lib = get(ENV, "B200UDE_LIB", "libb200ude")   # universal_differential_equ
 
 # ---- constants of include/b200ude.h ---------------------------------------------------------------------------------------
 const F32 = Int32(0)
-const MODEL_LV, MODEL_SEIR, MODEL_FKPP, MODEL_NODE, MODEL_SEIR_NODE = Int32.(0:4)
+const MODEL_LV, MODEL_SEIR, MODEL_FKPP, MODEL_NODE, MODEL_SEIR_NODE, MODEL_FORCED = Int32.(0:5)
+
+# forced neural ODE (MODEL_FORCED, FENEP.jl:41-62): per-trajectory forcing coefficients, a Julia Array of size (N, 3J) (the ABI's
+# [3J][N]): columns A_j, ω_j, φ_j
+set_forcing!(h, coef::Matrix{Float32}) =
+    check(h.ptr, ccall((:b200ude_set_forcing, lib), Int32, (Ptr{Cvoid}, Ptr{Float32}, Csize_t, Int32, Ptr{Cvoid}), h.ptr, coef, size(coef, 1), HOST, C_NULL))
 const ACT_IDENTITY, ACT_TANH, ACT_RBF = Int32.(0:2)
 const TSIT5, VERN7, RKC2 = Int32.(0:2)
 const INTERPOLATING_ADJOINT, DISCRETE_ADJOINT = Int32(0), Int32(1)

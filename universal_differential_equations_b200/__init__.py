@@ -7,9 +7,9 @@ mirror of the reference's call surface (sciml.py).  See DESIGN.md.
 """
 from . import _lib  # noqa: F401
 from .sciml import (  # noqa: F401
-    ADAM, BFGS, Chain, Dense, EnsembleProblem, FastChain, FastDense, FisherKPPUDE, ForwardDiffSensitivity,
+    ADAM, BFGS, Chain, Dense, EnsembleProblem, FastChain, FastDense, FisherKPPUDE, ForcedNeuralODE, ForwardDiffSensitivity,
     InterpolatingAdjoint, LotkaVolterraUDE, NeuralODE, ODEProblem, SEIRExposureUDE, SEIRNeuralODE, ReverseDiffVJP, RKC2, ROCK2, Tsit5, UDESolver, Vern7,
-    concrete_solve, identity, initial_params, rbf, remake, sciml_train, sciml_train_l2, solve, tanh,
+    concrete_solve, forcing_coefficients, identity, initial_params, rbf, remake, sciml_train, sciml_train_l2, solve, tanh,
 )
 from . import pde  # noqa: F401
 from . import jld2  # noqa: F401

@@ -36,7 +36,8 @@ thread_local std::string g_create_error;
 //            adaptive Tsit5 (fkpp_adaptive.cuh) and adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
 //   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
 //   K_FKPP16   Fisher-KPP UPDE with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu)                BASELINE config 4
-enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_F64 };
+//   K_FORCED   forced neural ODE with a readout network (FENEP.jl:41-62), fp32 (k_forced.cu; its fp64 handles are K_F64)
+enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_F64, K_FORCED };
 
 int kernel_num_params(KernelId k)
 {
@@ -62,6 +63,7 @@ struct b200ude_handle {
     ConstTables tab;
     GenericShape gen;
     int P = 0, n_save = 0, D = 0;
+    int DR = 0;      // rows per save of out / data / dL_dout: D, or D + r for the forced model
     size_t cap = 0;  // max trajectories
     size_t N = 0;    // trajectories of the last forward
     bool have_forward = false;
@@ -106,6 +108,12 @@ struct b200ude_handle {
     double *q_theta = nullptr, *q_ustep = nullptr, *q_dense = nullptr, *q_partial = nullptr, *q_tgrid = nullptr, *q_cot = nullptr;
     double *q_u0_keep = nullptr, *q_aux_out = nullptr, *q_hstep = nullptr;
     const double *q_last_out = nullptr;
+    // forced neural ODE (B200UDE_MODEL_FORCED, either dtype): shape, the forcing coefficients [3J][cap], the last forward's out
+    bool forced = false;
+    ForcedHost fh{};
+    void *d_forcing = nullptr;
+    size_t forcing_n = 0;   // trajectories of the last b200ude_set_forcing
+    void *d_usave = nullptr;   // adaptive: the saved states of the last forward [n_save][D][cap], read by the replay adjoint
     size_t dev_bytes = 0;
     std::string err;
 };
@@ -227,6 +235,10 @@ KernelId pick_kernel(const b200ude_desc &d)
 }
 
 
+// the forced neural ODE's forward and adjoint (both dtypes; defined with the fp64 path below)
+int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
+int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer);
+
 // Tsit5 forward solve with the dense record (stage derivatives) the interpolating adjoint reads
 int32_t tsit5_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int32_t *status, cudaStream_t st)
 {
@@ -270,6 +282,7 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
+    if (h->forced) return do_forward_forced(h, u0, N, out, status, st);
     if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
         // discrete adjoint, or the interpolating adjoint over Vern7's dense output: the forward records u_n of every (accepted)
         // step, which the adjoint recomputes the stages from.  With either dense flag an adaptive solve saves through the
@@ -335,6 +348,7 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[0], 0));
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[1], 0));
     }
+    if (h->forced) return do_adjoint_forced(h, l2, cot, loss, grad_theta, grad_u0, st, peer);
     AdjParams p;
     p.ustep = h->d_ustep; p.dense = h->d_dense; p.cot = cot; p.grad_u0 = grad_u0; p.partial = h->d_partial;
     p.theta = h->d_theta; p.N = (int)h->N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P;
@@ -531,6 +545,7 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
+    if (h->forced) return do_forward_forced(h, u0, N, out, status, st);
     if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
         // discrete adjoint / Vern7 dense output: u_n of every (accepted) step recorded (as in fp32)
         Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
@@ -566,6 +581,7 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
 int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss, double *grad_theta, double *grad_u0, cudaStream_t st)
 {
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
+    if (h->forced) return do_adjoint_forced(h, l2, cot, loss, grad_theta, grad_u0, st, false);
     if (h->desc.solver == B200UDE_VERN7 && h->vern7_pending) {
         if (!h->q_aux_out && dalloc(h, &h->q_aux_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
             return fail(h, B200UDE_ENOMEM, "adjoint: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -615,6 +631,88 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
     return B200UDE_OK;
 }
 
+// ---- forced neural ODE with a readout network (B200UDE_MODEL_FORCED; k_forced.cu), both dtypes ------------------------------
+int32_t forced_check(const b200ude_desc *d)
+{
+    if (d->solver != B200UDE_TSIT5 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT ||
+        (d->flags & (B200UDE_FLAG_VERN7_DENSE | B200UDE_FLAG_DISCRETE_DENSE)))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_MODEL_FORCED (forced neural ODE with a readout) has kernels for Tsit5, fixed step or adaptive, with the "
+                    "interpolating adjoint; not for Vern7, RKC2, the discrete adjoint, B200UDE_FLAG_VERN7_DENSE or B200UDE_FLAG_DISCRETE_DENSE");
+    const char *why = nullptr;
+    const int D = d->state_dim, NL = d->n_layers;
+    const int L0 = (int)d->consts[0], J = (int)d->consts[1], L1 = NL - L0;
+    if (d->n_consts != 2 || d->consts[0] != (double)L0 || d->consts[1] != (double)J) why = "n_consts must be 2 with consts[0] = L0 (layers of f0) and consts[1] = J (harmonics), both integers";
+    else if (J < 1 || J > 4) why = "J = consts[1] must be 1..4";
+    else if (L0 < 1 || L1 < 1) why = "consts[0] = L0 must leave at least one layer to each of f0 and f1 (n_layers = L0 + L1)";
+    else if (NL > 5) why = "L0 + L1 <= 5 (the widths of both chains take n_layers + 2 <= 7 entries)";
+    else if (D < 1 || D > 7) why = "state_dim must be 1..7 (the chains' input [u; gamma] has <= 8 entries)";
+    else if (d->n_prefix != 0 || d->n_suffix != 0) why = "n_prefix and n_suffix must be 0";
+    if (!why) {
+        for (int l = 0; l <= NL + 1; ++l)
+            if (d->widths[l] < 1 || d->widths[l] > 64) why = "every width must be 1..64";
+        for (int l = 0; l < NL; ++l)
+            if (d->acts[l] < 0 || d->acts[l] > 2) why = "unknown activation";
+    }
+    if (!why) {
+        const int r = d->widths[L0];
+        if (d->widths[0] != D + 1) why = "f0's input widths[0] must be state_dim + 1";
+        else if (r > 8) why = "the readout width widths[L0] must be <= 8";
+        else if (d->widths[L0 + 1] != D + 1) why = "f1's input widths[L0 + 1] must be state_dim + 1";
+        else if (d->widths[NL + 1] != D) why = "f1's output widths[n_layers + 1] must be state_dim";
+        else if (d->n_loss_weights != 0 && d->n_loss_weights != D + r) why = "n_loss_weights must be 0 or state_dim + r";
+        else if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)) why = "adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1";
+    }
+    if (why) return fail(nullptr, B200UDE_EINVAL, "create: B200UDE_MODEL_FORCED: %s", why);
+    return B200UDE_OK;
+}
+
+ForcedRun forced_run(const b200ude_handle *h, size_t N)
+{
+    const bool f64 = h->fh.dtype == 1;
+    ForcedRun r{};
+    r.forcing = h->d_forcing;
+    r.ustep = f64 ? (void *)h->q_ustep : (void *)h->d_ustep;
+    r.dense = f64 ? (void *)h->q_dense : (void *)h->d_dense;
+    r.partial = f64 ? (void *)h->q_partial : (void *)h->d_partial;
+    r.tgrid = f64 ? (void *)h->q_tgrid : (void *)h->d_tgrid;
+    r.nacc = h->d_nacc;
+    r.usave = h->d_usave;
+    r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.adaptive = h->adaptive ? 1 : 0;
+    r.n_save = h->n_save; r.max_steps = h->desc.max_steps; r.fstride = (int)h->cap;
+    r.t0 = h->desc.t0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;
+    return r;
+}
+
+int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st)
+{
+    if (N > h->forcing_n)
+        return fail(h, B200UDE_ESTATE, "forward: B200UDE_MODEL_FORCED needs the forcing of every trajectory (b200ude_set_forcing set %zu, N = %zu)",
+                    h->forcing_n, N);
+    ForcedRun r = forced_run(h, N);
+    r.u0 = u0; r.out = out; r.status = status;
+    CUDA_TRY(h, launch_fwd_forced(h->fh, r, st));
+    h->N = N;
+    h->have_forward = true;
+    return B200UDE_OK;
+}
+
+// fused L2: the loss 2 w (out - data) over all d + r rows, the readout rows recomputed from the saved states
+int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer)
+{
+    if (!h->have_forward) return fail(h, B200UDE_ESTATE, "adjoint: no stored forward solution (call b200ude_forward first)");
+    if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
+    if (h->N > h->forcing_n) return fail(h, B200UDE_ESTATE, "adjoint: the forcing was reset to fewer trajectories than the forward solved");
+    ForcedRun r = forced_run(h, h->N);
+    r.cot = cot; r.saved = h->d_usave; r.grad_u0 = grad_u0; r.fused_l2 = l2 ? 1 : 0;
+    int rows = 0;
+    CUDA_TRY(h, launch_adj_forced(h->fh, r, st, &rows));
+    if (h->fh.dtype == 1) CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, (double *)grad_theta, (double *)loss, st));
+    else if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, rows, h->P + 1, h->peer, (float *)grad_theta, (float *)loss, st));
+    else CUDA_TRY(h, launch_reduce(h->d_partial, rows, h->P + 1, (float *)grad_theta, (float *)loss, st));
+    return B200UDE_OK;
+}
+
 int32_t f64_unsupported(b200ude_handle *h, const char *what)
 {
     return fail(h, B200UDE_EUNSUPPORTED, "%s: not available for B200UDE_F64 handles (device-pointer forward / adjoint entry points only)", what);
@@ -644,7 +742,12 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (!(d->dt > 0) || d->n_steps < 1 || d->save_every < 1 || d->n_steps % d->save_every != 0)
         return fail(nullptr, B200UDE_EINVAL, "create: need dt>0, n_steps>=1, save_every>=1 dividing n_steps");
     if (d->max_trajectories == 0 || d->max_trajectories > (1ull << 26)) return fail(nullptr, B200UDE_EINVAL, "create: max_trajectories out of range");
-    if (d->n_loss_weights != 0 && d->n_loss_weights != d->state_dim) return fail(nullptr, B200UDE_EINVAL, "create: n_loss_weights must be 0 or state_dim");
+    const bool forced = d->model == B200UDE_MODEL_FORCED;
+    if (forced) {
+        const int32_t rc = forced_check(d);
+        if (rc) return rc;
+    }
+    if (!forced && d->n_loss_weights != 0 && d->n_loss_weights != d->state_dim) return fail(nullptr, B200UDE_EINVAL, "create: n_loss_weights must be 0 or state_dim");
     KernelId kid = pick_kernel(*d);
     const bool want64 = d->dtype == B200UDE_F64;
     const bool disc = d->sensealg == B200UDE_DISCRETE_ADJOINT;
@@ -673,7 +776,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: B200UDE_FLAG_VERN7_DENSE applies to Vern7 with the interpolating adjoint on the LV / SEIR / SEIR_NODE / NODE forms; "
                     "not to the discrete adjoint, Tsit5, RKC2 or the Fisher-KPP UPDE");
-    if (want64) {
+    if (want64 && !forced) {
         // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_generic.cuh in fp64, k_f64.cu): LV / SEIR / NODE forms, Tsit5 and Vern7,
         // fixed step and adaptive, interpolating or discrete adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
         if (!generic_ok(*d) || d->solver == B200UDE_RKC2)
@@ -697,7 +800,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         // (the discrete adjoint of a Vern7 solve and the dense-output flag run on the runtime-shape kernels only)
         if (disc || v7dense || !(kid == K_SEIR64 && !d->adaptive && env_int("B200UDE_SEIR_VERN7_TC", 1))) kid = K_GENERIC;
     }
-    if (!want64 && d->adaptive) {
+    if (!want64 && d->adaptive && !forced) {
         if (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)
             return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
         if (!generic_ok(*d))
@@ -723,6 +826,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     // fixed-step Tsit5 with the discrete adjoint: LV 2-32-32-2 / 2-5-5-5-2 keep their tuned kernels, every other form runs on the
     // runtime-shape ones (the SEIR tensor-core kernels have no discrete adjoint)
     if (disc && !want64 && kid != K_NONE && !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2 || kid == K_FKPP)) kid = K_GENERIC;
+    if (forced) kid = want64 ? K_F64 : K_FORCED;
     if (kid == K_NONE)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: no sm_90a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");
@@ -754,6 +858,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     h->desc = *d;
     h->kid = kid;
     h->D = d->state_dim;
+    h->DR = d->state_dim;
     h->n_save = d->n_steps / d->save_every + 1;
     h->cap = (size_t)d->max_trajectories;
     h->sm_count = prop.multiProcessorCount;
@@ -768,6 +873,63 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         h->gen.n_layers = d->n_layers; h->gen.n_prefix = d->n_prefix; h->gen.P = P;
         for (int l = 0; l < 8; ++l) { h->gen.widths[l] = l <= d->n_layers ? d->widths[l] : 0; h->gen.acts[l] = l < d->n_layers ? d->acts[l] : 0; }
         if (kid != K_F64 && P > 12288) { delete h; return fail(nullptr, B200UDE_EUNSUPPORTED, "create: %d parameters exceed the constant-bank budget", P); }
+    }
+    if (forced) {
+        // both chains back to back; P as the layer list says
+        const int L0 = (int)d->consts[0], L1 = d->n_layers - L0;
+        int P = 0;
+        for (int l = 0; l < L0 + L1; ++l) {
+            const int a = l < L0 ? l : l + 1;
+            P += d->widths[a] * d->widths[a + 1] + d->widths[a + 1];
+        }
+        if (!want64 && P > 12288) { delete h; return fail(nullptr, B200UDE_EUNSUPPORTED, "create: %d parameters exceed the constant-bank budget", P); }
+        h->P = P;
+        h->forced = true;
+        h->DR = d->state_dim + d->widths[L0];
+        ForcedHost &f = h->fh;
+        f.serial = serial; f.dtype = want64 ? 1 : 0; f.D = d->state_dim; f.R = d->widths[L0]; f.J = (int)d->consts[1]; f.L0 = L0; f.L1 = L1; f.P = P;
+        for (int l = 0; l < 8; ++l) {
+            f.widths[l] = l <= d->n_layers + 1 ? d->widths[l] : 0;
+            f.acts[l] = l < d->n_layers ? d->acts[l] : 0;
+        }
+        for (int i = 0; i < 16; ++i) f.lossw[i] = d->n_loss_weights > 0 ? (i < d->n_loss_weights ? d->loss_weights[i] : 0.0) : 1.0;
+        const size_t N = h->cap, D = (size_t)h->D, es = want64 ? sizeof(double) : sizeof(float);
+        const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
+        h->partial_blocks = (size_t)adj_rows_forced((int)N, f.dtype);
+        bool ok = true;
+        if (want64) {
+            ok = dalloc(h, &h->q_theta, (size_t)P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D * N) == cudaSuccess &&
+                 dalloc(h, &h->q_dense, (rec * 6 + 1) * D * N) == cudaSuccess && dalloc(h, &h->q_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess;
+            if (h->adaptive) ok = ok && dalloc(h, &h->q_tgrid, (rec + 1) * N) == cudaSuccess;
+            f.theta = h->q_theta;
+        } else {
+            ok = dalloc(h, &h->d_theta, (size_t)P + 1) == cudaSuccess && dalloc(h, &h->d_ustep, (rec + 1) * D * N) == cudaSuccess &&
+                 dalloc(h, &h->d_dense, (rec * 6 + 1) * D * N) == cudaSuccess && dalloc(h, &h->d_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess &&
+                 dalloc(h, &h->d_grad, (size_t)P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
+            if (h->adaptive) ok = ok && dalloc(h, &h->d_tgrid, (rec + 1) * N) == cudaSuccess;
+            f.theta = h->d_theta;
+        }
+        if (h->adaptive)
+            ok = ok && dalloc(h, &h->d_nacc, N) == cudaSuccess &&
+                 dalloc(h, (unsigned char **)&h->d_usave, es * (size_t)h->n_save * D * N) == cudaSuccess;
+        ok = ok && dalloc(h, (unsigned char **)&h->d_forcing, es * 3 * (size_t)f.J * N) == cudaSuccess;
+        if (ok) ok = cudaMemset(want64 ? (void *)h->q_theta : (void *)h->d_theta, 0, es * ((size_t)P + 1)) == cudaSuccess;
+        if (!ok) {
+            g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
+            b200ude_destroy(h);
+            return B200UDE_ENOMEM;
+        }
+        if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaEventCreateWithFlags(&h->data_ready, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&h->data_ready2, cudaEventDisableTiming) != cudaSuccess ||
+            (!want64 && cudaMallocHost((void **)&h->h_loss, sizeof(float)) != cudaSuccess)) {
+            g_create_error = "create: stream / pinned allocation failed";
+            b200ude_destroy(h);
+            return B200UDE_ENOMEM;
+        }
+        *out = h;
+        return B200UDE_OK;
     }
     h->var.approx_tanh = (d->flags & B200UDE_FLAG_APPROX_TANH) ? 1 : 0;
     h->var.discrete = d->sensealg == B200UDE_DISCRETE_ADJOINT ? 1 : 0;
@@ -886,6 +1048,7 @@ void b200ude_destroy(b200ude_handle *h)
     cudaFree(h->d_tgrid); cudaFree(h->d_nacc); cudaFree(h->d_cot); cudaFree(h->d_block_loss); cudaFree(h->d_hstep);
     cudaFree(h->q_theta); cudaFree(h->q_ustep); cudaFree(h->q_dense); cudaFree(h->q_partial); cudaFree(h->q_tgrid); cudaFree(h->q_cot);
     cudaFree(h->q_u0_keep); cudaFree(h->q_aux_out); cudaFree(h->q_hstep);
+    cudaFree(h->d_forcing); cudaFree(h->d_usave);
     if (h->h_loss) cudaFreeHost(h->h_loss);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
@@ -909,6 +1072,19 @@ int32_t b200ude_set_params(b200ude_handle *h, const void *theta, size_t P, int32
     CUDA_TRY(h, cudaMemcpyAsync(h->d_theta, theta, sizeof(float) * P,
                                 mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     h->have_theta = true;
+    return B200UDE_OK;
+}
+
+int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32_t mem, void *stream)
+{
+    if (!h) return B200UDE_EINVAL;
+    if (!h->forced) return fail(h, B200UDE_EUNSUPPORTED, "set_forcing: only B200UDE_MODEL_FORCED handles take a forcing (this handle: model %d)", h->desc.model);
+    if (!coef || N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "set_forcing: null pointer or N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
+    CUDA_TRY(h, cudaSetDevice(h->desc.device));
+    const size_t es = h->fh.dtype == 1 ? sizeof(double) : sizeof(float);
+    CUDA_TRY(h, cudaMemcpy2DAsync(h->d_forcing, es * h->cap, coef, es * N, es * N, (size_t)3 * h->fh.J,
+                                  mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    h->forcing_n = N;
     return B200UDE_OK;
 }
 
@@ -942,8 +1118,8 @@ static int32_t ensure_host_path(b200ude_handle *h)
     const size_t N = h->cap, D = (size_t)h->D;
     bool ok = true;
     ok = ok && dalloc(h, &h->d_u0, D * N) == cudaSuccess;
-    ok = ok && dalloc(h, &h->d_out, (size_t)h->n_save * D * N) == cudaSuccess;
-    ok = ok && dalloc(h, &h->d_data, (size_t)h->n_save * D * N) == cudaSuccess;
+    ok = ok && dalloc(h, &h->d_out, (size_t)h->n_save * h->DR * N) == cudaSuccess;
+    ok = ok && dalloc(h, &h->d_data, (size_t)h->n_save * h->DR * N) == cudaSuccess;
     ok = ok && dalloc(h, &h->d_gu0, D * N) == cudaSuccess;
     ok = ok && dalloc(h, &h->d_status, N) == cudaSuccess;
     if (!ok) return fail(h, B200UDE_ENOMEM, "host path: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -965,7 +1141,7 @@ int32_t b200ude_solve_host(b200ude_handle *h, const void *theta, const void *u0,
     CUDA_TRY(h, cudaMemcpyAsync(h->d_u0, u0, sizeof(float) * D * N, cudaMemcpyHostToDevice, st));
     rc = do_forward(h, h->d_u0, N, h->d_out, status ? h->d_status : nullptr, st);
     if (rc) return rc;
-    CUDA_TRY(h, cudaMemcpyAsync(out, h->d_out, sizeof(float) * (size_t)h->n_save * D * N, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(h, cudaMemcpyAsync(out, h->d_out, sizeof(float) * (size_t)h->n_save * h->DR * N, cudaMemcpyDeviceToHost, st));
     if (status) CUDA_TRY(h, cudaMemcpyAsync(status, h->d_status, sizeof(int32_t) * N, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(h, cudaStreamSynchronize(st));
     return B200UDE_OK;
@@ -990,7 +1166,7 @@ int32_t b200ude_loss_gradient_host(b200ude_handle *h, const void *theta, const v
     // ... in two halves of the trajectories (strided copies: the layout is trajectory-fastest), so that the adjoint of the first half
     // can start under the second half's upload when the link is slower than the forward kernel
     const size_t half = N >= 8192 ? ((N / 2 + 15) / 16) * 16 : N;
-    const size_t rows = (size_t)h->n_save * D;
+    const size_t rows = (size_t)h->n_save * h->DR;
     CUDA_TRY(h, cudaMemcpy2DAsync(h->d_data, sizeof(float) * N, data, sizeof(float) * N, sizeof(float) * half, rows, cudaMemcpyHostToDevice, h->copy_stream));
     CUDA_TRY(h, cudaEventRecord(h->data_ready, h->copy_stream));
     if (half < N)
@@ -1057,7 +1233,7 @@ int32_t b200ude_train_adam(b200ude_handle *h, const b200ude_adam *opt, const voi
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "train_adam: N=%zu outside (0, %zu]", N, h->cap);
     int32_t rc = check_adam(h, opt);
     if (rc) return rc;
-    if (!h->d_train_out && dalloc(h, &h->d_train_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
+    if (!h->d_train_out && dalloc(h, &h->d_train_out, (size_t)h->n_save * (size_t)h->DR * h->cap) != cudaSuccess)
         return fail(h, B200UDE_ENOMEM, "train_adam: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
     cudaStream_t st = stream ? (cudaStream_t)stream : h->own_stream;   // the legacy default stream cannot be captured
     if (!stream) {

@@ -8,7 +8,7 @@
 namespace b200ude {
 
 // model and activation codes (B200UDE_MODEL_*, B200UDE_ACT_*)
-constexpr int MODEL_LV = 0, MODEL_SEIR = 1, MODEL_FKPP = 2, MODEL_NODE = 3, MODEL_SEIR_NODE = 4;
+constexpr int MODEL_LV = 0, MODEL_SEIR = 1, MODEL_FKPP = 2, MODEL_NODE = 3, MODEL_SEIR_NODE = 4, MODEL_FORCED = 5;
 constexpr int ACT_IDENTITY = 0, ACT_TANH = 1, ACT_RBF = 2;
 
 struct FwdParams {
@@ -228,5 +228,26 @@ cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Ad
 cudaError_t launch_fwd_fkpp_vern7_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // discrete adjoint handles
 cudaError_t launch_adj_fkpp_vern7_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot_f64(const Shape64Host &, const double *out, const double *data, double *cot, double *loss, size_t N, int n_save, cudaStream_t);
+
+// ---- forced neural ODE with a readout network (B200UDE_MODEL_FORCED; forced.cuh, k_forced.cu), fp32 and fp64 ----
+struct ForcedHost {
+    uint64_t serial;
+    int dtype;               // 0 = float, 1 = double: every pointer below and in ForcedRun
+    int D, R, J, L0, L1, P;  // states, readout outputs, harmonics, layers of f0 / f1, parameters
+    int widths[8], acts[8];  // the descriptor's back-to-back lists
+    double lossw[16];        // d + r weights
+    const void *theta;       // the handle's device copy
+};
+struct ForcedRun {
+    const void *u0, *forcing, *cot, *saved;   // saved: the recorded saved states of an adaptive forward (= usave)
+    void *out, *ustep, *dense, *usave, *grad_u0, *partial, *tgrid;
+    int32_t *status;
+    int *nacc;
+    int N, n_steps, save_every, fused_l2, adaptive, n_save, max_steps, fstride;
+    double t0, dt, save_dt, abstol, reltol;
+};
+int adj_rows_forced(int N, int dtype);
+cudaError_t launch_fwd_forced(const ForcedHost &, const ForcedRun &, cudaStream_t);
+cudaError_t launch_adj_forced(const ForcedHost &, const ForcedRun &, cudaStream_t, int *rows_out);
 
 }  // namespace b200ude

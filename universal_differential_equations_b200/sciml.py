@@ -197,6 +197,56 @@ class SEIRNeuralODE:
         return self.chain.num_params()
 
 
+@dataclass(frozen=True)
+class ForcedNeuralODE:
+    """A neural ODE driven by a per-trajectory cosine forcing, with a readout network inside the loss
+    (NonNewtonianFluids/FENEP.jl:41-62):
+
+        du = dynamics([u; gamma(t)]),   y = readout([u; gamma(t)]),   gamma_n(t) = sum_j A_jn cos(w_jn t + phi_jn).
+
+    dynamics: d + 1 -> ... -> d, readout: d + 1 -> ... -> r.  theta = [readout; dynamics] (Flux.params(f0, f1), FENEP.jl:98).
+    The solver's outputs have d + r rows per save (the states, then the readout at the saved states); the forcing is a
+    [3 * harmonics, N] array with rows (A_j, w_j, phi_j), given per call (`concrete_solve(..., forcing=)`) or per solver
+    (`UDESolver.set_forcing`)."""
+    dynamics: FastChain
+    readout: FastChain
+    harmonics: int = 1
+
+    model = _lib.MODEL_FORCED
+
+    @property
+    def state_dim(self):
+        return self.dynamics.widths[-1]
+
+    @property
+    def readout_dim(self):
+        return self.readout.widths[-1]
+
+    @property
+    def chain(self):
+        return self.dynamics
+
+    def desc_layers(self):
+        """(n_layers, widths, acts) of the descriptor: the readout's list, then the dynamics' (b200ude.h, B200UDE_MODEL_FORCED)."""
+        return (len(self.readout.layers) + len(self.dynamics.layers), self.readout.widths + self.dynamics.widths,
+                self.readout.acts + self.dynamics.acts)
+
+    def consts(self):
+        return (float(len(self.readout.layers)), float(self.harmonics))
+
+    def num_params(self):
+        return self.readout.num_params() + self.dynamics.num_params()
+
+
+def forcing_coefficients(amplitude, omega, phase=None) -> np.ndarray:
+    """[3J, N] coefficient rows (A_j, w_j, phi_j) from arrays of shape [J, N] (or [N] for J = 1): gamma(t) = sum_j A cos(w t + phi)."""
+    A = np.atleast_2d(np.asarray(amplitude, dtype=np.float64))
+    W = np.atleast_2d(np.asarray(omega, dtype=np.float64))
+    F = np.zeros_like(W) if phase is None else np.atleast_2d(np.asarray(phase, dtype=np.float64))
+    A, W, F = np.broadcast_arrays(A, W, F)
+    return np.stack([A, W, F], axis=1).reshape(-1, A.shape[1])
+
+
 # --------------------------------------------------------------------------- problem / algorithm types
 @dataclass
 class ODEProblem:
@@ -345,11 +395,14 @@ class UDESolver:
         d.dtype = _lib.F64 if dtype == torch.float64 else _lib.F32
         d.model = f.model
         d.state_dim = f.state_dim
-        chain = f.chain
-        d.n_layers = len(chain.layers)
-        for i, w in enumerate(chain.widths):
+        if hasattr(f, "desc_layers"):   # the forced model: readout and dynamics back to back
+            n_layers, widths, acts = f.desc_layers()
+        else:
+            n_layers, widths, acts = len(f.chain.layers), f.chain.widths, f.chain.acts
+        d.n_layers = n_layers
+        for i, w in enumerate(widths):
             d.widths[i] = w
-        for i, a in enumerate(chain.acts):
+        for i, a in enumerate(acts):
             d.acts[i] = _ACT_CODE[a]
         d.n_prefix = getattr(f, "trainable_rates", 0)
         d.n_suffix = getattr(f, "n_suffix", 0)
@@ -385,6 +438,8 @@ class UDESolver:
         self.P = int(self._L.b200ude_num_params(h))
         self.n_save = int(self._L.b200ude_num_save(h))
         self.d = f.state_dim
+        self.rows = f.state_dim + getattr(f, "readout_dim", 0)   # rows per save of out / data / dL_dout
+        self._forcing = None
         self.capacity = int(max_trajectories)
         self.adaptive, self.max_steps = bool(adaptive), int(max_steps)
         self.generation = 0   # bumped by every set_params / forward: identifies the forward record the handle holds
@@ -414,13 +469,25 @@ class UDESolver:
         self._theta_keepalive = theta
         self.generation += 1
 
+    def set_forcing(self, coef):
+        """Forced model: the forcing coefficients [3J, N] (rows A_j, w_j, phi_j), host or device, in the solver's dtype."""
+        coef = torch.as_tensor(coef).to(self.dtype).contiguous() if not isinstance(coef, torch.Tensor) else coef.detach().to(self.dtype).contiguous()
+        if coef.dim() != 2:
+            raise ValueError("forcing must be [3J, N]")
+        mem = _lib.DEVICE if coef.is_cuda else _lib.HOST
+        _lib.check(self._h, self._L.b200ude_set_forcing(self._h, coef.data_ptr(), coef.shape[1], mem, _stream_ptr(self.device)))
+        if not coef.is_cuda:
+            torch.cuda.current_stream(self.device).synchronize()   # the host copy is read by the stream-ordered upload
+        self._forcing = coef
+        self.generation += 1
+
     def forward(self, u0: torch.Tensor, out: Optional[torch.Tensor] = None, status: Optional[torch.Tensor] = None):
-        """u0[d, N] (cuda, the solver's dtype) -> out[n_save, d, N]."""
+        """u0[d, N] (cuda, the solver's dtype) -> out[n_save, rows, N] (rows = d, or d + r for the forced model)."""
         assert u0.is_cuda and u0.dtype == self.dtype and u0.dim() == 2 and u0.shape[0] == self.d
         u0 = u0.contiguous()
         N = u0.shape[1]
         if out is None:
-            out = torch.empty((self.n_save, self.d, N), device=u0.device, dtype=self.dtype)
+            out = torch.empty((self.n_save, self.rows, N), device=u0.device, dtype=self.dtype)
         sp = status.data_ptr() if status is not None else None
         _lib.check(self._h, self._L.b200ude_forward(self._h, u0.data_ptr(), N, out.data_ptr(), sp, _stream_ptr(self.device)))
         self.generation += 1
@@ -456,7 +523,7 @@ class UDESolver:
         theta = np.ascontiguousarray(theta, np.float32)
         u0 = np.ascontiguousarray(u0, np.float32)
         N = u0.shape[1]
-        out = np.empty((self.n_save, self.d, N), np.float32)
+        out = np.empty((self.n_save, self.rows, N), np.float32)
         status = np.empty(N, np.int32)
         self.generation += 1
         _lib.check(self._h, self._L.b200ude_solve_host(self._h, theta.ctypes.data, u0.ctypes.data, N, out.ctypes.data, status.ctypes.data))
@@ -558,6 +625,7 @@ class _SolveFn(torch.autograd.Function):
         # the forward record (step states, stage derivatives, theta) lives in the handle, which later calls with the same
         # key reuse: remember which forward it holds and what produced it, so that backward can restore it
         ctx.solver = solver
+        ctx.forcing = solver._forcing
         ctx.gen = solver.generation
         ctx.theta, ctx.u0 = theta.detach(), u0.detach()
         ctx.need_u0 = u0.requires_grad
@@ -570,6 +638,8 @@ class _SolveFn(torch.autograd.Function):
             # another forward / set_params used the handle since (two predictions in one loss, multiple shooting,
             # mini-batches): re-run this call's forward so that the adjoint reads its own record and theta
             solver.set_params(ctx.theta)
+            if ctx.forcing is not None:
+                solver.set_forcing(ctx.forcing)
             solver.forward(ctx.u0)
         gth, gu0 = solver.adjoint(gout, want_grad_u0=True)
         return gth, (gu0 if ctx.need_u0 else None), None
@@ -602,13 +672,14 @@ def _grid_from(tspan, saveat, dt):
 
 
 def concrete_solve(prob, alg, u0=None, p=None, *, saveat=None, dt=None, adaptive=None, abstol=None, reltol=None,
-                   sensealg=None, loss_weights=None, max_steps=512, dtype=torch.float32):
+                   sensealg=None, loss_weights=None, max_steps=512, dtype=torch.float32, forcing=None):
     """Array(concrete_solve(prob, Tsit5(), u0, p; saveat, sensealg=InterpolatingAdjoint(...))).
 
     `prob` may be an ODEProblem (u0[d] -> d x n_save, like Julia's Array(sol)) or an
     EnsembleProblem (u0s[d, N] -> n_save x d x N).  Differentiable w.r.t. p and u0.
     adaptive defaults to true when no dt is given (as in OrdinaryDiffEq): Tsit5 with the PI controller and
     abstol / reltol (defaults 1e-6 / 1e-3); pass dt= for adaptive=false.
+    A ForcedNeuralODE takes its forcing coefficients [3J, N] as `forcing` and returns d + r rows per save.
     """
     ens = isinstance(prob, EnsembleProblem)
     base = prob.prob if ens else prob
@@ -637,6 +708,10 @@ def concrete_solve(prob, alg, u0=None, p=None, *, saveat=None, dt=None, adaptive
         solver = UDESolver(base.f, t0, dtv, n_steps, save_every, max_trajectories=max(N, 1), device=dev, alg=alg,
                            sensealg=sensealg, loss_weights=loss_weights, adaptive=adaptive, abstol=abstol, reltol=reltol, max_steps=max_steps, dtype=dtype)
         _SOLVERS[key] = solver
+    if forcing is not None:
+        solver.set_forcing(forcing)
+    elif getattr(base.f, "model", None) == _lib.MODEL_FORCED:
+        raise ValueError("concrete_solve: a ForcedNeuralODE needs forcing=[3J, N]")
     out = _SolveFn.apply(pt, u0t, solver)
     return out if ens else out[:, :, 0].transpose(0, 1)
 
