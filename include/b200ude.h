@@ -89,6 +89,15 @@ extern "C" {
                                   interpolating adjoint stands for the reference's Tracker gradient through the solver; the two
                                   agree to the solve tolerance).  The fused L2 recomputes the readout from the saved state.
                                   Vern7, RKC2, the discrete adjoint and the dense flags return B200UDE_EUNSUPPORTED. */
+#define B200UDE_MODEL_OPERATOR 6 /* wide-state operator UDE (Climate/NeuralPDE/npde.jl:75-78):  du = D1 * NN(u) + D2 * u,
+                                    NN: widths[0] = d -> ... -> widths[n_layers] = m; D1 (d x m) and D2 (d x d) fixed, column-major,
+                                    set by b200ude_set_operators.  Envelope: d 1..64, every width 1..64, 1..5 layers, activations
+                                    identity / tanh / rbf; n_prefix = n_suffix = n_consts = 0; n_loss_weights 0, or d when d <= 16.
+                                    theta = per layer vec(W) then b (Flux.destructure).  A warp integrates one trajectory.
+                                    Tsit5 fixed step or adaptive, RKC2 fixed step (2..64 stages), interpolating adjoint, fp32 and
+                                    fp64.  Vern7, the discrete adjoint and the dense flags return B200UDE_EUNSUPPORTED;
+                                    B200UDE_FLAG_APPROX_TANH is accepted and ignored.  create returns B200UDE_EUNSUPPORTED when the
+                                    staged operators, theta and one warp's gradient vector exceed the device's shared memory. */
 
 /* activations of the dense chain */
 #define B200UDE_ACT_IDENTITY 0
@@ -226,6 +235,12 @@ int32_t b200ude_set_params(b200ude_handle *h, const void *theta, size_t P, int32
  * (capacity max_trajectories) that forward, solve_host, loss_gradient_host and train_adam read; calling them with more
  * trajectories than were last set is B200UDE_ESTATE.  Stream-ordered on `stream`.  Any other model: B200UDE_EUNSUPPORTED. */
 int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32_t mem, void *stream);
+
+/* OPERATORS of a B200UDE_MODEL_OPERATOR handle: D1 [d x m] and D2 [d x d], column-major, in the handle's dtype (host or device
+ * memory per `mem`).  D2 = NULL is a zero D2 (D1 = I, D2 = NULL: a plain wide neural ODE).  The handle keeps its own padded
+ * device copies; forward or adjoint before the first call is B200UDE_ESTATE.  Stream-ordered on `stream`.  Any other model:
+ * B200UDE_EUNSUPPORTED. */
+int32_t b200ude_set_operators(b200ude_handle *h, const void *D1, const void *D2, int32_t mem, void *stream);
 
 /* FORWARD  (replaces: the UDE RHS closure + OrdinaryDiffEq perform_step! loop behind
  * concrete_solve(prob, Tsit5(), u0, p; saveat, ...), one trajectory per ensemble member).

@@ -25,7 +25,13 @@ const lib = get(ENV, "B200UDE_LIB", "libb200ude")   # universal_differential_equ
 
 # ---- constants of include/b200ude.h ---------------------------------------------------------------------------------------
 const F32 = Int32(0)
-const MODEL_LV, MODEL_SEIR, MODEL_FKPP, MODEL_NODE, MODEL_SEIR_NODE, MODEL_FORCED = Int32.(0:5)
+const MODEL_LV, MODEL_SEIR, MODEL_FKPP, MODEL_NODE, MODEL_SEIR_NODE, MODEL_FORCED, MODEL_OPERATOR = Int32.(0:6)
+
+# operator UDE (MODEL_OPERATOR, npde.jl:75-78): du = D1 * re(p)(u) + D2 * u with fixed Julia matrices (column-major, as the ABI
+# takes them); D2 = nothing is a zero D2
+set_operators!(h, D1::Matrix{Float32}, D2::Union{Matrix{Float32},Nothing}=nothing) =
+    check(h.ptr, ccall((:b200ude_set_operators, lib), Int32, (Ptr{Cvoid}, Ptr{Float32}, Ptr{Float32}, Int32, Ptr{Cvoid}),
+                       h.ptr, D1, D2 === nothing ? Ptr{Float32}(C_NULL) : D2, HOST, C_NULL))
 
 # forced neural ODE (MODEL_FORCED, FENEP.jl:41-62): per-trajectory forcing coefficients, a Julia Array of size (N, 3J) (the ABI's
 # [3J][N]): columns A_j, ω_j, φ_j

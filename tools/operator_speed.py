@@ -1,0 +1,81 @@
+"""Time one training iteration of the operator UDE (npde.jl's 30-8-30 tanh closure): forward, fused-L2 adjoint and reduce.
+
+Adaptive Tsit5 at (1e-6, 1e-3) against fixed-step RKC2 at the save spacing with the stage count from eigen_est = rho(D2),
+fp32 and fp64, for N = 1 (the script's case) and ensembles of initial bumps.  CUDA events; the configurations alternate
+round by round, and the median and the spread over rounds are printed with the GPU's name and power limit.
+Usage: python tools/operator_speed.py [--rounds 7] [--iters 20] [--sizes 1,4096,65536]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import universal_differential_equations_b200 as ude  # noqa: E402
+import operator_ref as R  # noqa: E402
+
+
+def bumps(N, rng):
+    z = R.npde_grid()[1:31]
+    c = rng.uniform(0.2, 0.8, N) if N > 1 else np.array([0.75])
+    return np.exp(-200.0 * (z[:, None] - c[None, :]) ** 2)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=7)
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--sizes", default="1,4096,65536")
+    a = ap.parse_args()
+    D1, D2 = R.npde_ops()
+    saveat = np.linspace(0, 1.5, 30)
+    chain = ude.FastChain(ude.FastDense(30, 8, ude.tanh), ude.FastDense(8, 30, ude.tanh))
+    f = ude.OperatorUDE(chain, D1, D2)
+    th = R.glorot([30, 8, 30], np.random.default_rng(0))
+    rng = np.random.default_rng(1)
+    stages = ude.RKC2(eigen_est=191.7).n_stages(saveat[1])
+    cfgs = []
+    for N in [int(x) for x in a.sizes.split(",")]:
+        u0 = bumps(N, rng)
+        for dt in (torch.float32, torch.float64):
+            for solver in ("tsit5_adaptive", "rkc2"):
+                kw = dict(adaptive=True, abstol=1e-6, reltol=1e-3, max_steps=400) if solver == "tsit5_adaptive" else dict(alg=ude.RKC2(stages=stages))
+                s = ude.UDESolver(f, 0.0, saveat[1], 29, 1, max_trajectories=N, device="cuda:0", dtype=dt, **kw)
+                s.set_params(torch.tensor(th, dtype=dt, device="cuda"))
+                u = torch.tensor(u0, dtype=dt, device="cuda")
+                out = s.forward(u)
+                data = (out * 1.01).contiguous()
+                cfgs.append(dict(N=N, dtype=str(dt).split(".")[-1], solver=solver, s=s, u=u, data=data, times=[]))
+
+    def step(c):
+        c["s"].forward(c["u"])
+        c["s"].adjoint_l2(c["data"])
+
+    for c in cfgs:   # warm-up
+        for _ in range(3):
+            step(c)
+    torch.cuda.synchronize()
+    for _ in range(a.rounds):
+        for c in cfgs:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(a.iters):
+                step(c)
+            e1.record()
+            e1.synchronize()
+            c["times"].append(e0.elapsed_time(e1) / a.iters)
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"# GPU: {q}; RKC2 stages = {stages}; ms per iteration (forward + fused-L2 adjoint + reduce), median [min, max] over {a.rounds} rounds")
+    for c in cfgs:
+        t = np.array(c["times"])
+        print(json.dumps(dict(N=c["N"], dtype=c["dtype"], solver=c["solver"], ms_median=round(float(np.median(t)), 4),
+                              ms_min=round(float(t.min()), 4), ms_max=round(float(t.max()), 4))))
+
+
+if __name__ == "__main__":
+    main()

@@ -8,7 +8,7 @@ mirror of the reference's call surface (sciml.py).  See DESIGN.md.
 from . import _lib  # noqa: F401
 from .sciml import (  # noqa: F401
     ADAM, BFGS, Chain, Dense, EnsembleProblem, FastChain, FastDense, FisherKPPUDE, ForcedNeuralODE, ForwardDiffSensitivity,
-    InterpolatingAdjoint, LotkaVolterraUDE, NeuralODE, ODEProblem, SEIRExposureUDE, SEIRNeuralODE, ReverseDiffVJP, RKC2, ROCK2, Tsit5, UDESolver, Vern7,
+    InterpolatingAdjoint, LotkaVolterraUDE, NeuralODE, ODEProblem, OperatorUDE, SEIRExposureUDE, SEIRNeuralODE, ReverseDiffVJP, RKC2, ROCK2, Tsit5, UDESolver, Vern7,
     concrete_solve, forcing_coefficients, identity, initial_params, rbf, remake, sciml_train, sciml_train_l2, solve, tanh,
 )
 from . import pde  # noqa: F401

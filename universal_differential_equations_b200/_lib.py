@@ -15,7 +15,7 @@ SO_PATH = os.path.join(CSRC, "libb200ude.so")
 # ---- constants mirrored from include/b200ude.h -------------------------------
 ABI_VERSION = 1
 F32, F64 = 0, 1
-MODEL_LV, MODEL_SEIR, MODEL_FKPP, MODEL_NODE, MODEL_SEIR_NODE, MODEL_FORCED = 0, 1, 2, 3, 4, 5
+MODEL_LV, MODEL_SEIR, MODEL_FKPP, MODEL_NODE, MODEL_SEIR_NODE, MODEL_FORCED, MODEL_OPERATOR = 0, 1, 2, 3, 4, 5, 6
 ACT_IDENTITY, ACT_TANH, ACT_RBF = 0, 1, 2
 TSIT5, VERN7, RKC2 = 0, 1, 2
 INTERPOLATING_ADJOINT, DISCRETE_ADJOINT = 0, 1
@@ -28,7 +28,7 @@ MAX_LAYERS = 6
 
 EXPORTS = [
     "b200ude_version", "b200ude_last_error", "b200ude_create", "b200ude_destroy",
-    "b200ude_num_params", "b200ude_num_save", "b200ude_device_bytes", "b200ude_set_params", "b200ude_set_forcing",
+    "b200ude_num_params", "b200ude_num_save", "b200ude_device_bytes", "b200ude_set_params", "b200ude_set_forcing", "b200ude_set_operators",
     "b200ude_forward", "b200ude_adjoint", "b200ude_adjoint_l2", "b200ude_solve_host",
     "b200ude_loss_gradient_host", "b200ude_get_params", "b200ude_adam_reset", "b200ude_adam_step", "b200ude_train_adam",
     "b200ude_peer_export", "b200ude_peer_attach", "b200ude_peer_detach", "b200ude_adjoint_l2_allreduce", "b200ude_selftest_tanh",
@@ -114,6 +114,8 @@ def lib():
     L.b200ude_set_params.argtypes = [vp, vp, sz, i32, vp]
     L.b200ude_set_forcing.restype = i32
     L.b200ude_set_forcing.argtypes = [vp, vp, sz, i32, vp]
+    L.b200ude_set_operators.restype = i32
+    L.b200ude_set_operators.argtypes = [vp, vp, vp, i32, vp]
     L.b200ude_forward.restype = i32
     L.b200ude_forward.argtypes = [vp, vp, sz, vp, vp, vp]
     L.b200ude_adjoint.restype = i32

@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <atomic>
 #include <string>
+#include <vector>
 
 #include "params.h"
 
@@ -37,7 +38,9 @@ thread_local std::string g_create_error;
 //   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
 //   K_FKPP16   Fisher-KPP UPDE with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu)                BASELINE config 4
 //   K_FORCED   forced neural ODE with a readout network (FENEP.jl:41-62), fp32 (k_forced.cu; its fp64 handles are K_F64)
-enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_F64, K_FORCED };
+//   K_OPERATOR wide-state operator UDE du = D1 NN(u) + D2 u (npde.jl:75-78), warp per trajectory, fp32 (k_operator.cu; its fp64
+//            handles are K_F64)
+enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_F64, K_FORCED, K_OPERATOR };
 
 int kernel_num_params(KernelId k)
 {
@@ -114,6 +117,12 @@ struct b200ude_handle {
     void *d_forcing = nullptr;
     size_t forcing_n = 0;   // trajectories of the last b200ude_set_forcing
     void *d_usave = nullptr;   // adaptive: the saved states of the last forward [n_save][D][cap], read by the replay adjoint
+    // operator UDE (B200UDE_MODEL_OPERATOR, either dtype): shape, the padded operator block, the RKC2 tables (handle dtype);
+    // it shares d_usave (as [n_save][cap][D]) and the record buffers with the forced model
+    bool op = false;
+    bool ops_set = false;
+    OperatorHost oh{};
+    void *d_ops = nullptr, *d_rkc = nullptr;
     size_t dev_bytes = 0;
     std::string err;
 };
@@ -150,10 +159,12 @@ cudaError_t dalloc(b200ude_handle *h, T **p, size_t count)
 
 // RKC2 (Sommeijer, Shampine, Verwer 1998) recurrence coefficients, stage abscissae and the quadrature weights of the stage
 // integrands (from running the recurrence on unit impulses)
-void rkc2_tables(int s, RkcHost *out)
+// in double: mt1, then mu, nu, mt, ga, c, w with 65 entries each
+void rkc2_tables64(int s, double &mt1, double *mu, double *nu, double *mt, double *ga, double *c, double *w)
 {
     const double eps = 2.0 / 13.0, w0 = 1.0 + eps / ((double)s * s);
-    double T[65], dT[65], d2T[65], b[65] = {0}, mu[65] = {0}, nu[65] = {0}, mt[65] = {0}, ga[65] = {0}, c[65] = {0};
+    double T[65], dT[65], d2T[65], b[65] = {0};
+    for (int j = 0; j < 65; ++j) mu[j] = nu[j] = mt[j] = ga[j] = c[j] = w[j] = 0;
     double W[65][65];   // 33 KB of stack, host side only
     T[0] = 1; T[1] = w0; dT[0] = 0; dT[1] = 1; d2T[0] = 0; d2T[1] = 0;
     for (int j = 2; j <= s; ++j) {
@@ -164,7 +175,7 @@ void rkc2_tables(int s, RkcHost *out)
     const double w1 = dT[s] / d2T[s];
     for (int j = 2; j <= s; ++j) b[j] = d2T[j] / (dT[j] * dT[j]);
     b[0] = b[1] = b[2];
-    const double mt1 = b[1] * w1;
+    mt1 = b[1] * w1;
     for (int j = 2; j <= s; ++j) {
         mu[j] = 2 * b[j] * w0 / b[j - 1];
         nu[j] = -b[j] / b[j - 2];
@@ -179,12 +190,31 @@ void rkc2_tables(int s, RkcHost *out)
         W[j][j - 1] += mt[j];
         W[j][0] += ga[j];
     }
+    for (int j = 0; j < s; ++j) w[j] = W[s][j];
+}
+
+void rkc2_tables(int s, RkcHost *out)
+{
+    double mt1, mu[65], nu[65], mt[65], ga[65], c[65], w[65];
+    rkc2_tables64(s, mt1, mu, nu, mt, ga, c, w);
     *out = RkcHost();
     out->s = s; out->mt1 = (float)mt1;
     for (int j = 0; j <= s; ++j) {
         out->mu[j] = (float)mu[j]; out->nu[j] = (float)nu[j]; out->mt[j] = (float)mt[j]; out->ga[j] = (float)ga[j]; out->c[j] = (float)c[j];
-        out->w[j] = j < s ? (float)W[s][j] : 0.0f;
+        out->w[j] = j < s ? (float)w[j] : 0.0f;
     }
+}
+
+// operator UDE RKC2 table layout (operator.cuh: mt1, then c, w, mu, nu, mt, ga with 65 entries each); k = 0..5 in that order
+constexpr int op_rkc_len() { return 1 + 6 * 65; }
+constexpr int op_rkc_off(int k) { return 1 + 65 * k; }
+
+// n doubles -> dst (device) in the handle's dtype, synchronously
+cudaError_t upload_as(void *dst, const double *src, size_t n, bool f64)
+{
+    if (f64) return cudaMemcpy(dst, src, n * sizeof(double), cudaMemcpyHostToDevice);
+    std::vector<float> v(src, src + n);
+    return cudaMemcpy(dst, v.data(), n * sizeof(float), cudaMemcpyHostToDevice);
 }
 
 int env_int(const char *name, int dflt)
@@ -238,6 +268,9 @@ KernelId pick_kernel(const b200ude_desc &d)
 // the forced neural ODE's forward and adjoint (both dtypes; defined with the fp64 path below)
 int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
 int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer);
+// the operator UDE's forward and adjoint (both dtypes; defined with the fp64 path below)
+int32_t do_forward_operator(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
+int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer);
 
 // Tsit5 forward solve with the dense record (stage derivatives) the interpolating adjoint reads
 int32_t tsit5_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int32_t *status, cudaStream_t st)
@@ -283,6 +316,7 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
     if (h->forced) return do_forward_forced(h, u0, N, out, status, st);
+    if (h->op) return do_forward_operator(h, u0, N, out, status, st);
     if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
         // discrete adjoint, or the interpolating adjoint over Vern7's dense output: the forward records u_n of every (accepted)
         // step, which the adjoint recomputes the stages from.  With either dense flag an adaptive solve saves through the
@@ -349,6 +383,7 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[1], 0));
     }
     if (h->forced) return do_adjoint_forced(h, l2, cot, loss, grad_theta, grad_u0, st, peer);
+    if (h->op) return do_adjoint_operator(h, l2, cot, loss, grad_theta, grad_u0, st, peer);
     AdjParams p;
     p.ustep = h->d_ustep; p.dense = h->d_dense; p.cot = cot; p.grad_u0 = grad_u0; p.partial = h->d_partial;
     p.theta = h->d_theta; p.N = (int)h->N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P;
@@ -546,6 +581,7 @@ int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out,
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
     if (h->forced) return do_forward_forced(h, u0, N, out, status, st);
+    if (h->op) return do_forward_operator(h, u0, N, out, status, st);
     if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
         // discrete adjoint / Vern7 dense output: u_n of every (accepted) step recorded (as in fp32)
         Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
@@ -582,6 +618,7 @@ int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss
 {
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
     if (h->forced) return do_adjoint_forced(h, l2, cot, loss, grad_theta, grad_u0, st, false);
+    if (h->op) return do_adjoint_operator(h, l2, cot, loss, grad_theta, grad_u0, st, false);
     if (h->desc.solver == B200UDE_VERN7 && h->vern7_pending) {
         if (!h->q_aux_out && dalloc(h, &h->q_aux_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
             return fail(h, B200UDE_ENOMEM, "adjoint: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -713,6 +750,180 @@ int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *los
     return B200UDE_OK;
 }
 
+// ---- wide-state operator UDE du = D1 NN(u) + D2 u (B200UDE_MODEL_OPERATOR; k_operator.cu), both dtypes ---------------------------
+int32_t operator_check(const b200ude_desc *d)
+{
+    if (d->solver == B200UDE_VERN7 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT ||
+        (d->flags & (B200UDE_FLAG_VERN7_DENSE | B200UDE_FLAG_DISCRETE_DENSE)))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_MODEL_OPERATOR (operator UDE du = D1 NN(u) + D2 u) has kernels for Tsit5, fixed step or adaptive, and "
+                    "fixed-step RKC2, with the interpolating adjoint; not for Vern7, the discrete adjoint, B200UDE_FLAG_VERN7_DENSE or "
+                    "B200UDE_FLAG_DISCRETE_DENSE");
+    const char *why = nullptr;
+    const int D = d->state_dim, NL = d->n_layers;
+    if (D < 1 || D > 64) why = "state_dim must be 1..64";
+    else if (NL > 5) why = "n_layers must be 1..5";
+    else if (d->n_prefix != 0 || d->n_suffix != 0 || d->n_consts != 0) why = "n_prefix, n_suffix and n_consts must be 0";
+    if (!why) {
+        for (int l = 0; l <= NL; ++l)
+            if (d->widths[l] < 1 || d->widths[l] > 64) why = "every width must be 1..64";
+        for (int l = 0; l < NL; ++l)
+            if (d->acts[l] < 0 || d->acts[l] > 2) why = "unknown activation";
+    }
+    if (!why) {
+        if (d->widths[0] != D) why = "the chain's input widths[0] must be state_dim";
+        else if (d->n_loss_weights != 0 && (d->n_loss_weights != D || D > 16)) why = "n_loss_weights must be 0, or state_dim when state_dim <= 16";
+        else if (d->solver == B200UDE_RKC2 && (d->n_stages < 2 || d->n_stages > 64)) why = "RKC2 needs 2 <= n_stages <= 64";
+        else if (d->solver == B200UDE_RKC2 && d->adaptive) why = "RKC2 runs with a fixed step (adaptive = 0)";
+        else if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)) why = "adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1";
+    }
+    if (why) return fail(nullptr, B200UDE_EINVAL, "create: B200UDE_MODEL_OPERATOR: %s", why);
+    return B200UDE_OK;
+}
+
+OperatorRun operator_run(const b200ude_handle *h, size_t N)
+{
+    const bool f64 = h->oh.dtype == 1;
+    OperatorRun r{};
+    r.ustep = f64 ? (void *)h->q_ustep : (void *)h->d_ustep;
+    r.dense = f64 ? (void *)h->q_dense : (void *)h->d_dense;
+    r.partial = f64 ? (void *)h->q_partial : (void *)h->d_partial;
+    r.tgrid = f64 ? (void *)h->q_tgrid : (void *)h->d_tgrid;
+    r.usave = h->d_usave;
+    r.nacc = h->d_nacc;
+    r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.n_save = h->n_save; r.max_steps = h->desc.max_steps;
+    r.adaptive = h->adaptive ? 1 : 0;
+    r.t0 = h->desc.t0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;
+    return r;
+}
+
+int32_t do_forward_operator(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st)
+{
+    if (!h->ops_set) return fail(h, B200UDE_ESTATE, "forward: B200UDE_MODEL_OPERATOR needs its operators (call b200ude_set_operators first)");
+    OperatorRun r = operator_run(h, N);
+    r.u0 = u0; r.out = out; r.status = status;
+    CUDA_TRY(h, launch_fwd_operator(h->oh, r, st));
+    h->N = N;
+    h->have_forward = true;
+    return B200UDE_OK;
+}
+
+int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer)
+{
+    if (!h->ops_set) return fail(h, B200UDE_ESTATE, "adjoint: B200UDE_MODEL_OPERATOR needs its operators (call b200ude_set_operators first)");
+    if (!h->have_forward) return fail(h, B200UDE_ESTATE, "adjoint: no stored forward solution (call b200ude_forward first)");
+    if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
+    OperatorRun r = operator_run(h, h->N);
+    r.cot = cot; r.grad_u0 = grad_u0; r.fused_l2 = l2 ? 1 : 0;
+    int rows = 0;
+    CUDA_TRY(h, launch_adj_operator(h->oh, r, st, &rows));
+    if (h->oh.dtype == 1) CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, (double *)grad_theta, (double *)loss, st));
+    else if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, rows, h->P + 1, h->peer, (float *)grad_theta, (float *)loss, st));
+    else CUDA_TRY(h, launch_reduce(h->d_partial, rows, h->P + 1, (float *)grad_theta, (float *)loss, st));
+    return B200UDE_OK;
+}
+
+// create for B200UDE_MODEL_OPERATOR (the descriptor is validated before the device check, so that it is testable without a GPU)
+int32_t create_operator(const b200ude_desc *d, b200ude_handle **out)
+{
+    int32_t rc = operator_check(d);
+    if (rc) return rc;
+    const bool want64 = d->dtype == B200UDE_F64;
+    OperatorHost oh{};
+    oh.dtype = want64 ? 1 : 0; oh.D = d->state_dim; oh.M = d->widths[d->n_layers]; oh.L = d->n_layers;
+    for (int l = 0; l < 6; ++l) oh.widths[l] = l <= d->n_layers ? d->widths[l] : 0;
+    for (int l = 0; l < 5; ++l) oh.acts[l] = l < d->n_layers ? d->acts[l] : 0;
+    oh.rkc2 = d->solver == B200UDE_RKC2 ? 1 : 0;
+    oh.S = oh.rkc2 ? d->n_stages : 0;
+    operator_layout(oh);
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0) return fail(nullptr, B200UDE_ENODEVICE, "create: no CUDA device (%s)", cudaGetErrorString(e));
+    if (d->device < 0 || d->device >= ndev) return fail(nullptr, B200UDE_EINVAL, "create: device %d of %d", d->device, ndev);
+    cudaDeviceProp prop;
+    e = cudaGetDeviceProperties(&prop, d->device);
+    if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaGetDeviceProperties: %s", cudaGetErrorString(e));
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_90a code only", d->device, prop.major, prop.minor);
+    e = cudaSetDevice(d->device);
+    if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaSetDevice: %s", cudaGetErrorString(e));
+    // four warps (trajectories) per CTA, fewer when their gradient vectors do not fit next to the kernels' static shared memory
+    size_t stat = 0;
+    e = operator_static_smem(oh.dtype, &stat);
+    if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaFuncGetAttributes: %s", cudaGetErrorString(e));
+    oh.dyn_cap = (int)(prop.sharedMemPerBlockOptin - stat);
+    oh.warps = 4;
+    while (oh.warps > 0 && operator_smem(oh, oh.warps) > (size_t)oh.dyn_cap) --oh.warps;
+    if (oh.warps == 0)
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_MODEL_OPERATOR with d = %d, m = %d and %d parameters needs %zu B of shared memory for one warp "
+                    "(%zu B dynamic + %zu B static; device limit %zu B)",
+                    oh.D, oh.M, oh.P, operator_smem(oh, 1) + stat, operator_smem(oh, 1), stat, (size_t)prop.sharedMemPerBlockOptin);
+    b200ude_handle *h = new (std::nothrow) b200ude_handle();
+    if (!h) return fail(nullptr, B200UDE_ENOMEM, "create: out of host memory");
+    h->desc = *d;
+    h->kid = want64 ? K_F64 : K_OPERATOR;
+    h->op = true;
+    h->D = h->DR = d->state_dim;
+    h->n_save = d->n_steps / d->save_every + 1;
+    h->cap = (size_t)d->max_trajectories;
+    h->sm_count = prop.multiProcessorCount;
+    h->adaptive = d->adaptive != 0;
+    h->P = oh.P;
+    const size_t N = h->cap, D = (size_t)h->D, P = (size_t)oh.P, es = want64 ? sizeof(double) : sizeof(float);
+    const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
+    const size_t dense_rows = oh.rkc2 ? rec + 1 : rec * 6 + 1;   // RKC2: f(u_n); Tsit5: the stages
+    h->partial_blocks = (size_t)adj_rows_operator((int)N, oh.warps);
+    bool ok = true;
+    if (want64) {
+        ok = dalloc(h, &h->q_theta, P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D * N) == cudaSuccess &&
+             dalloc(h, &h->q_dense, dense_rows * D * N) == cudaSuccess && dalloc(h, &h->q_partial, h->partial_blocks * (P + 1)) == cudaSuccess;
+        if (h->adaptive) ok = ok && dalloc(h, &h->q_tgrid, (rec + 1) * N) == cudaSuccess;
+        oh.theta = h->q_theta;
+    } else {
+        ok = dalloc(h, &h->d_theta, P + 1) == cudaSuccess && dalloc(h, &h->d_ustep, (rec + 1) * D * N) == cudaSuccess &&
+             dalloc(h, &h->d_dense, dense_rows * D * N) == cudaSuccess && dalloc(h, &h->d_partial, h->partial_blocks * (P + 1)) == cudaSuccess &&
+             dalloc(h, &h->d_grad, P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
+        if (h->adaptive) ok = ok && dalloc(h, &h->d_tgrid, (rec + 1) * N) == cudaSuccess;
+        oh.theta = h->d_theta;
+    }
+    if (h->adaptive)
+        ok = ok && dalloc(h, &h->d_nacc, N) == cudaSuccess && dalloc(h, (unsigned char **)&h->d_usave, es * (size_t)h->n_save * D * N) == cudaSuccess;
+    ok = ok && dalloc(h, (unsigned char **)&h->d_ops, es * (size_t)oh.ops_elems) == cudaSuccess;
+    if (oh.rkc2) ok = ok && dalloc(h, (unsigned char **)&h->d_rkc, es * (size_t)op_rkc_len()) == cudaSuccess;
+    if (ok) {
+        // the loss weights in front of the operator block; the operators follow in b200ude_set_operators
+        std::vector<double> w64(oh.ops_elems, 0.0);
+        for (int c = 0; c < 64; ++c) w64[c] = c < oh.D ? (d->n_loss_weights > 0 ? d->loss_weights[c] : 1.0) : 0.0;
+        ok = upload_as(h->d_ops, w64.data(), w64.size(), want64) == cudaSuccess &&
+             cudaMemset(want64 ? (void *)h->q_theta : (void *)h->d_theta, 0, es * (P + 1)) == cudaSuccess;
+        if (ok && oh.rkc2) {
+            std::vector<double> t(op_rkc_len(), 0.0);
+            rkc2_tables64(oh.S, t[0], &t[op_rkc_off(2)], &t[op_rkc_off(3)], &t[op_rkc_off(4)], &t[op_rkc_off(5)], &t[op_rkc_off(0)], &t[op_rkc_off(1)]);
+            ok = upload_as(h->d_rkc, t.data(), t.size(), want64) == cudaSuccess;
+        }
+    }
+    if (!ok) {
+        g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
+        b200ude_destroy(h);
+        return B200UDE_ENOMEM;
+    }
+    oh.ops = h->d_ops;
+    oh.rkc = h->d_rkc;
+    h->oh = oh;
+    if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->data_ready, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->data_ready2, cudaEventDisableTiming) != cudaSuccess ||
+        (!want64 && cudaMallocHost((void **)&h->h_loss, sizeof(float)) != cudaSuccess)) {
+        g_create_error = "create: stream / pinned allocation failed";
+        b200ude_destroy(h);
+        return B200UDE_ENOMEM;
+    }
+    *out = h;
+    return B200UDE_OK;
+}
+
 int32_t f64_unsupported(b200ude_handle *h, const char *what)
 {
     return fail(h, B200UDE_EUNSUPPORTED, "%s: not available for B200UDE_F64 handles (device-pointer forward / adjoint entry points only)", what);
@@ -742,6 +953,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (!(d->dt > 0) || d->n_steps < 1 || d->save_every < 1 || d->n_steps % d->save_every != 0)
         return fail(nullptr, B200UDE_EINVAL, "create: need dt>0, n_steps>=1, save_every>=1 dividing n_steps");
     if (d->max_trajectories == 0 || d->max_trajectories > (1ull << 26)) return fail(nullptr, B200UDE_EINVAL, "create: max_trajectories out of range");
+    if (d->model == B200UDE_MODEL_OPERATOR) return create_operator(d, out);
     const bool forced = d->model == B200UDE_MODEL_FORCED;
     if (forced) {
         const int32_t rc = forced_check(d);
@@ -1049,6 +1261,7 @@ void b200ude_destroy(b200ude_handle *h)
     cudaFree(h->q_theta); cudaFree(h->q_ustep); cudaFree(h->q_dense); cudaFree(h->q_partial); cudaFree(h->q_tgrid); cudaFree(h->q_cot);
     cudaFree(h->q_u0_keep); cudaFree(h->q_aux_out); cudaFree(h->q_hstep);
     cudaFree(h->d_forcing); cudaFree(h->d_usave);
+    cudaFree(h->d_ops); cudaFree(h->d_rkc);
     if (h->h_loss) cudaFreeHost(h->h_loss);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
@@ -1085,6 +1298,25 @@ int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32
     CUDA_TRY(h, cudaMemcpy2DAsync(h->d_forcing, es * h->cap, coef, es * N, es * N, (size_t)3 * h->fh.J,
                                   mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, (cudaStream_t)stream));
     h->forcing_n = N;
+    return B200UDE_OK;
+}
+
+int32_t b200ude_set_operators(b200ude_handle *h, const void *D1, const void *D2, int32_t mem, void *stream)
+{
+    if (!h) return B200UDE_EINVAL;
+    if (!h->op) return fail(h, B200UDE_EUNSUPPORTED, "set_operators: only B200UDE_MODEL_OPERATOR handles take operators (this handle: model %d)", h->desc.model);
+    if (!D1) return fail(h, B200UDE_EINVAL, "set_operators: D1 is a null pointer");
+    CUDA_TRY(h, cudaSetDevice(h->desc.device));
+    const OperatorHost &o = h->oh;
+    const size_t es = o.dtype == 1 ? sizeof(double) : sizeof(float);
+    const cudaMemcpyKind kind = mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    // column-major d x m and d x d into the padded block: column k at (64 + k ld) elements
+    unsigned char *base = (unsigned char *)h->d_ops + es * 64;
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_TRY(h, cudaMemcpy2DAsync(base, es * o.ld1, D1, es * o.D, es * o.D, (size_t)o.M, kind, st));
+    if (D2) CUDA_TRY(h, cudaMemcpy2DAsync(base + es * o.ld1 * o.M, es * o.ld2, D2, es * o.D, es * o.D, (size_t)o.D, kind, st));
+    h->oh.has_d2 = D2 ? 1 : 0;
+    h->ops_set = true;
     return B200UDE_OK;
 }
 

@@ -1,0 +1,651 @@
+// operator.cuh -- wide-state operator UDEs (B200UDE_MODEL_OPERATOR), written once over the real type:
+//
+//     du/dt = D1 · NN(u) + D2 · u,     NN: d -> ... -> m,  D1 (d x m), D2 (d x d) fixed, column-major
+//
+// (Climate/NeuralPDE/npde.jl:75-78: dudt_(u, p, t) = ops.D1 * re(p)(u) + ops.D2 * u, a method-of-lines PDE with a learned
+// closure).  d and every width go up to 64, so one thread per trajectory would hold u and the Tsit5 stages on its stack and
+// run ~2 d^2 dependent FMAs per right-hand side.  Here a WARP integrates one trajectory:
+//
+//   - lane l holds state component l and l + 32 (the second slot only when d > 32); each layer's units follow the same rule.
+//     Runge-Kutta state, stages and lambda are a few registers per lane.
+//   - a matrix-vector product D·v: a lane computes its own output rows, the inputs v_k come from their owner lanes by
+//     __shfl_sync in a fixed order of k.  D^T·g: a lane computes its own columns, g_i by shuffle in a fixed order of i.
+//   - D1, D2 (the handle's padded copy, one 16-byte-multiple block, with the loss weights in front) are staged once per CTA by
+//     one elected thread with cp.async.bulk completing on an mbarrier.  theta, which ADAM updates in place every iteration, is
+//     staged by the CTA into the same padded layout.  Every leading dimension in shared memory is odd, so that the lanes'
+//     column reads (D·v) and row reads (D^T·g) are both free of bank conflicts.  Nothing goes through the constant bank:
+//     handles of this model run concurrently on one device.
+//   - the parameter gradient: one P-vector per warp in shared memory; dW_ik belongs to the lane that owns unit i, each bias to
+//     its owner lane, so there are no atomics and the summation order is fixed.  The CTA then sums its warps in a fixed order
+//     into its partial row (launch_reduce / launch_reduce_f64 do the rest).
+//   - adaptive stepping: the error norm is a shuffle-xor butterfly, so every lane holds the same bits and the accept / reject
+//     decision is warp-uniform.  No CTA barrier sits inside any stepping loop: each warp runs its own step count, and each
+//     trajectory's results are bitwise those of the trajectory solved alone.
+//
+// Handle records are component-fastest within a trajectory, [row][N][d]; the ABI arrays stay [..][d][N].
+//   Tsit5: dense (6 steps + 1) d N (row s*6 + j = k_j of step s; k_0 of step s = k_6 of step s-1), ustep (steps + 1) d N.
+//   RKC2:  ustep (steps + 1) d N and, in `dense`, f(u_n) (steps + 1) d N.
+// theta = per layer vec(W) column-major then b (Flux.destructure).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "ude_generic.cuh"
+
+namespace b200ude {
+namespace op {
+
+constexpr int MAXL = 5;
+constexpr int LW = 64;          // loss-weight slots at the front of the staged operator block
+constexpr int RKC_MAX = 64;     // RKC2 stages
+constexpr unsigned FULL = 0xffffffffu;
+// RKC2 table layout (the handle's device copy, in the handle's dtype): mt1, then c, w, mu, nu, mt, ga with RKC_MAX + 1 entries each
+constexpr int RKC_C = 1, RKC_W = RKC_C + RKC_MAX + 1, RKC_MU = RKC_W + RKC_MAX + 1, RKC_NU = RKC_MU + RKC_MAX + 1,
+              RKC_MT = RKC_NU + RKC_MAX + 1, RKC_GA = RKC_MT + RKC_MAX + 1, RKC_LEN = RKC_GA + RKC_MAX + 1;
+
+template <typename R>
+struct Run {
+    int D, M, L, P, has_d2;
+    int widths[MAXL + 1], acts[MAXL];
+    int woff[MAXL];   // layer l's vec(W) in theta (and in the gradient vector); b follows at woff + a b
+    int soff[MAXL];   // layer l's W in the staged theta, leading dimension ldw[l] (odd); b follows at soff + a ldw
+    int ldw[MAXL];
+    int ld1, ld2;     // odd leading dimensions of the staged D1 / D2
+    int ops_elems, theta_elems, gstride;   // staged block sizes (elements); gstride: one warp's gradient vector (>= P + 1)
+    const R *ops;     // [LW loss weights | D1 (ld1 x M) | D2 (ld2 x D)], ops_elems elements
+    const R *theta;   // the handle's theta [P]
+    const R *rkc;     // RKC2 tables (RKC_LEN)
+    int S;            // RKC2 stages
+    const R *u0;      // [d][N]
+    R *out;           // [n_save][d][N]
+    R *ustep, *dense, *usave;   // records [row][N][d]
+    int32_t *status;
+    const R *cot;     // fused_l2 ? data : dL/dout, [n_save][d][N]
+    R *grad_u0, *partial;
+    int fused_l2;
+    R *tgrid;         // adaptive: accepted step times [max_steps + 1][N]
+    int *nacc;
+    int N, n_steps, save_every, n_save, max_steps;
+    R t0, dt, save_dt, abstol, reltol;
+};
+
+template <typename R>
+struct V {
+    R a, b;   // components lane, lane + 32
+};
+
+template <typename R>
+__device__ __forceinline__ R act(int k, R z);
+template <>
+__device__ __forceinline__ float act<float>(int k, float z) { return k == ACT_TANH ? tanhf(z) : (k == ACT_RBF ? expf(-z * z) : z); }
+template <>
+__device__ __forceinline__ double act<double>(int k, double z) { return k == ACT_TANH ? tanh(z) : (k == ACT_RBF ? exp(-z * z) : z); }
+
+// v[c * stride] for the lane's components c < D (zero elsewhere)
+template <typename R>
+__device__ __forceinline__ V<R> ldv(const R *p, size_t stride, int D, int lane)
+{
+    return {lane < D ? p[(size_t)lane * stride] : (R)0, lane + 32 < D ? p[(size_t)(lane + 32) * stride] : (R)0};
+}
+template <typename R>
+__device__ __forceinline__ void stv(R *p, size_t stride, V<R> v, int D, int lane)
+{
+    if (lane < D) p[(size_t)lane * stride] = v.a;
+    if (lane + 32 < D) p[(size_t)(lane + 32) * stride] = v.b;
+}
+
+template <typename R>
+__device__ __forceinline__ R wsum(R v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+    return v;
+}
+
+// y_i = sum_{k < cols} A[i + k ld] x_k for the lane's rows i < rows, zero elsewhere
+template <typename R>
+__device__ __forceinline__ V<R> matvec(const R *A, int ld, int rows, int cols, V<R> x, int lane)
+{
+    const int r0 = lane < rows ? lane : 0, r1 = lane + 32 < rows ? lane + 32 : 0;
+    R y0 = (R)0, y1 = (R)0;
+    if (rows > 32) {
+        for (int k = 0; k < cols; ++k) {
+            const R xk = __shfl_sync(FULL, k < 32 ? x.a : x.b, k & 31);
+            y0 = fma(A[k * ld + r0], xk, y0);
+            y1 = fma(A[k * ld + r1], xk, y1);
+        }
+    } else {
+        for (int k = 0; k < cols; ++k) y0 = fma(A[k * ld + r0], __shfl_sync(FULL, k < 32 ? x.a : x.b, k & 31), y0);
+    }
+    return {lane < rows ? y0 : (R)0, lane + 32 < rows ? y1 : (R)0};
+}
+
+// y_k = sum_{i < rows} A[i + k ld] g_i for the lane's columns k < cols, zero elsewhere
+template <typename R>
+__device__ __forceinline__ V<R> matvec_t(const R *A, int ld, int rows, int cols, V<R> g, int lane)
+{
+    const int k0 = lane < cols ? lane : 0, k1 = lane + 32 < cols ? lane + 32 : 0;
+    R y0 = (R)0, y1 = (R)0;
+    if (cols > 32) {
+        for (int i = 0; i < rows; ++i) {
+            const R gi = __shfl_sync(FULL, i < 32 ? g.a : g.b, i & 31);
+            y0 = fma(A[k0 * ld + i], gi, y0);
+            y1 = fma(A[k1 * ld + i], gi, y1);
+        }
+    } else {
+        for (int i = 0; i < rows; ++i) y0 = fma(A[k0 * ld + i], __shfl_sync(FULL, i < 32 ? g.a : g.b, i & 31), y0);
+    }
+    return {lane < cols ? y0 : (R)0, lane + 32 < cols ? y1 : (R)0};
+}
+
+// the chain NN(x); with KEEP, xs[l] = input of layer l (xs[L] = output) and zs[l] = its pre-activation
+template <typename R, bool KEEP>
+__device__ __forceinline__ V<R> chain(const Run<R> &p, const R *sth, V<R> x, V<R> *xs, V<R> *zs, int lane)
+{
+#pragma unroll
+    for (int l = 0; l < MAXL; ++l) {
+        if (l < p.L) {
+            const int a = p.widths[l], b = p.widths[l + 1], ld = p.ldw[l];
+            const R *W = sth + p.soff[l];
+            if (KEEP) xs[l] = x;
+            V<R> z = matvec(W, ld, b, a, x, lane);
+            z.a += lane < b ? W[a * ld + lane] : (R)0;
+            z.b += lane + 32 < b ? W[a * ld + lane + 32] : (R)0;
+            if (KEEP) zs[l] = z;
+            x.a = lane < b ? act<R>(p.acts[l], z.a) : (R)0;
+            x.b = lane + 32 < b ? act<R>(p.acts[l], z.b) : (R)0;
+        }
+    }
+    if (KEEP) {
+#pragma unroll
+        for (int l = 1; l <= MAXL; ++l)
+            if (l == p.L) xs[l] = x;
+    }
+    return x;
+}
+
+// f(u) = D1 NN(u) + D2 u
+template <typename R>
+__device__ __forceinline__ V<R> rhs(const Run<R> &p, const R *sops, const R *sth, V<R> u, int lane)
+{
+    const V<R> y = chain<R, false>(p, sth, u, nullptr, nullptr, lane);
+    V<R> f = matvec(sops + LW, p.ld1, p.D, p.M, y, lane);
+    if (p.has_d2) {
+        const V<R> e = matvec(sops + LW + p.ld1 * p.M, p.ld2, p.D, p.D, u, lane);
+        f.a += e.a;
+        f.b += e.b;
+    }
+    return f;
+}
+
+// (df/du)^T g; the warp's gradient vector gw += w (df/dtheta)^T g
+template <typename R>
+__device__ __forceinline__ V<R> rhs_vjp(const Run<R> &p, const R *sops, const R *sth, V<R> x, V<R> g, R w, R *gw, int lane)
+{
+    V<R> xs[MAXL + 1], zs[MAXL];
+    chain<R, true>(p, sth, x, xs, zs, lane);
+    V<R> v = matvec_t(sops + LW, p.ld1, p.D, p.M, g, lane);   // D1^T g
+#pragma unroll
+    for (int l = MAXL - 1; l >= 0; --l) {
+        if (l < p.L) {
+            const int a = p.widths[l], b = p.widths[l + 1];
+            V<R> dl;
+            dl.a = lane < b ? v.a * generic::actder_rt<R>(p.acts[l], zs[l].a, xs[l + 1].a) : (R)0;
+            dl.b = lane + 32 < b ? v.b * generic::actder_rt<R>(p.acts[l], zs[l].b, xs[l + 1].b) : (R)0;
+            R *gW = gw + p.woff[l];
+            const R wa = w * dl.a, wb = w * dl.b;
+            for (int k = 0; k < a; ++k) {
+                const R xk = __shfl_sync(FULL, k < 32 ? xs[l].a : xs[l].b, k & 31);
+                if (lane < b) gW[k * b + lane] = fma(wa, xk, gW[k * b + lane]);
+                if (lane + 32 < b) gW[k * b + lane + 32] = fma(wb, xk, gW[k * b + lane + 32]);
+            }
+            if (lane < b) gW[a * b + lane] += wa;
+            if (lane + 32 < b) gW[a * b + lane + 32] += wb;
+            v = matvec_t(sth + p.soff[l], p.ldw[l], b, a, dl, lane);
+        }
+    }
+    if (p.has_d2) {
+        const V<R> e = matvec_t(sops + LW + p.ld1 * p.M, p.ld2, p.D, p.D, g, lane);
+        v.a += e.a;
+        v.b += e.b;
+    }
+    return v;
+}
+
+// Stage the operator block (bulk copy on an mbarrier) and theta (padded, by the CTA) into shared memory.  Ends with every
+// thread past the mbarrier; the only CTA barrier of the kernel before its closing reduction.
+template <typename R>
+__device__ __forceinline__ void stage(const Run<R> &p, R *sops, R *sth)
+{
+    __shared__ __align__(8) uint64_t bar;
+    const uint32_t bar_a = (uint32_t)__cvta_generic_to_shared(&bar), dst_a = (uint32_t)__cvta_generic_to_shared(sops);
+    const uint32_t bytes = (uint32_t)(p.ops_elems * sizeof(R));
+    if (threadIdx.x == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(bytes) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a), "l"(p.ops),
+                     "r"(bytes), "r"(bar_a)
+                     : "memory");
+    }
+    for (int l = 0; l < p.L; ++l) {
+        const int a = p.widths[l], b = p.widths[l + 1], ld = p.ldw[l];
+        const R *src = p.theta + p.woff[l];
+        R *dst = sth + p.soff[l];
+        for (int e = threadIdx.x; e < a * b; e += blockDim.x) dst[(e / b) * ld + e % b] = __ldg(src + e);
+        for (int e = threadIdx.x; e < b; e += blockDim.x) dst[a * ld + e] = __ldg(src + a * b + e);
+    }
+    __syncthreads();   // theta staged; the mbarrier is initialised and armed before anybody polls it
+    uint32_t done = 0;
+    while (!done)
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(bar_a) : "memory");
+}
+
+template <typename R>
+struct Smem {
+    R *ops, *th, *g;
+};
+template <typename R>
+__device__ __forceinline__ Smem<R> carve(const Run<R> &p)
+{
+    extern __shared__ __align__(128) unsigned char s_raw[];
+    R *base = reinterpret_cast<R *>(s_raw);
+    return {base, base + p.ops_elems, base + p.ops_elems + p.theta_elems};
+}
+
+// the CTA's warps' gradient vectors (and losses at index P) summed in warp order into the CTA's partial row
+template <typename R>
+__device__ __forceinline__ void cta_reduce(const Run<R> &p, const R *sg)
+{
+    __syncthreads();
+    const int W = blockDim.x >> 5;
+    R *dst = p.partial + (size_t)blockIdx.x * (p.P + 1);
+    for (int e = threadIdx.x; e < p.P + 1; e += blockDim.x) {
+        R tot = sg[e];
+        for (int w = 1; w < W; ++w) tot += sg[(size_t)w * p.gstride + e];
+        dst[e] = tot;
+    }
+}
+
+template <typename R>
+__device__ __forceinline__ bool warp_finite(V<R> u)
+{
+    return __all_sync(FULL, fabs(u.a) <= Prec<R>::huge && fabs(u.b) <= Prec<R>::huge);
+}
+
+// the cotangent of save `is` at state us: lam += cot, or (fused L2) loss += w r^2, lam += 2 w r with r = us - data
+template <typename R>
+__device__ __forceinline__ void save_jump(const Run<R> &p, const R *sops, int is, V<R> us, V<R> &lam, R &loss, size_t n, int lane)
+{
+    const size_t N = (size_t)p.N;
+    const V<R> c = ldv(p.cot + (size_t)is * p.D * N + n, N, p.D, lane);
+    if (p.fused_l2) {
+        const R ra = us.a - c.a, rb = us.b - c.b;
+        const R wa = lane < p.D ? sops[lane] : (R)0, wb = lane + 32 < p.D ? sops[lane + 32] : (R)0;
+        loss = fma(wa * ra, ra, loss);
+        loss = fma(wb * rb, rb, loss);
+        lam.a = fma((R)2 * wa, ra, lam.a);
+        lam.b = fma((R)2 * wb, rb, lam.b);
+    } else {
+        lam.a += c.a;
+        lam.b += c.b;
+    }
+}
+
+// ---- 1. fixed-step Tsit5 forward, with the dense record ----
+template <typename R>
+__global__ void __launch_bounds__(128) tsit5_forward_kernel(Run<R> p)
+{
+    const Smem<R> sm = carve(p);
+    stage(p, sm.ops, sm.th);
+    const int lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const int traj = blockIdx.x * W + (threadIdx.x >> 5);
+    if (traj >= p.N) return;
+    const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+    const R dt = p.dt;
+    auto rec = [&](R *b, int row) { return b + ((size_t)row * N + n) * D; };
+    V<R> u = ldv(p.u0 + n, N, p.D, lane), k[7];
+    stv(p.out + n, N, u, p.D, lane);
+    stv(rec(p.ustep, 0), 1, u, p.D, lane);
+    k[0] = rhs(p, sm.ops, sm.th, u, lane);
+    stv(rec(p.dense, 0), 1, k[0], p.D, lane);
+    int isave = 1;
+    for (int s = 0; s < p.n_steps; ++s) {
+#pragma unroll
+        for (int i = 1; i < 7; ++i) {
+            R aa = (R)0, ab = (R)0;
+#pragma unroll
+            for (int j = 0; j < i; ++j)
+                if (Tsit5::a(i, j) != 0.0) { aa = fma((R)Tsit5::a(i, j), k[j].a, aa); ab = fma((R)Tsit5::a(i, j), k[j].b, ab); }
+            const V<R> g{fma(dt, aa, u.a), fma(dt, ab, u.b)};
+            if (i == 6) u = g;
+            k[i] = rhs(p, sm.ops, sm.th, g, lane);
+            stv(rec(p.dense, s * 6 + i), 1, k[i], p.D, lane);
+        }
+        stv(rec(p.ustep, s + 1), 1, u, p.D, lane);
+        if ((s + 1) % p.save_every == 0) { stv(p.out + (size_t)isave * D * N + n, N, u, p.D, lane); ++isave; }
+        k[0] = k[6];
+    }
+    const bool ok = warp_finite(u);
+    if (p.status && lane == 0) p.status[n] = ok ? 0 : 1;
+}
+
+// ---- 2. interpolating adjoint on the fixed Tsit5 grid ----
+template <typename R>
+__global__ void __launch_bounds__(128) tsit5_adjoint_kernel(Run<R> p)
+{
+    const Smem<R> sm = carve(p);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    R *gw = sm.g + (size_t)warp * p.gstride;
+    for (int q = lane; q < p.P + 1; q += 32) gw[q] = (R)0;
+    stage(p, sm.ops, sm.th);
+    const int traj = blockIdx.x * W + warp;
+    if (traj < p.N) {
+        const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+        const R dt = p.dt;
+        auto rec = [&](const R *b, int row) { return b + ((size_t)row * N + n) * D; };
+        V<R> lam{(R)0, (R)0}, kl[6];
+        R loss = (R)0;
+        auto jump = [&](int is) { save_jump(p, sm.ops, is, ldv(rec(p.ustep, is * p.save_every), 1, p.D, lane), lam, loss, n, lane); };
+        jump(p.n_steps / p.save_every);
+        for (int s = p.n_steps - 1; s >= 0; --s) {
+            const V<R> us = ldv(rec(p.ustep, s), 1, p.D, lane);
+#pragma unroll
+            for (int i = 0; i < 6; ++i) {
+                R xa = (R)0, xb = (R)0, ga = (R)0, gb = (R)0;
+#pragma unroll
+                for (int j = 0; j < 7; ++j)
+                    if (Tsit5::bw(i, j) != 0.0) {
+                        const V<R> kj = ldv(rec(p.dense, s * 6 + j), 1, p.D, lane);
+                        xa = fma((R)Tsit5::bw(i, j), kj.a, xa);
+                        xb = fma((R)Tsit5::bw(i, j), kj.b, xb);
+                    }
+#pragma unroll
+                for (int j = 0; j < i; ++j)
+                    if (Tsit5::a(i, j) != 0.0) { ga = fma((R)Tsit5::a(i, j), kl[j].a, ga); gb = fma((R)Tsit5::a(i, j), kl[j].b, gb); }
+                const V<R> x{fma(dt, xa, us.a), fma(dt, xb, us.b)}, g{fma(dt, ga, lam.a), fma(dt, gb, lam.b)};
+                kl[i] = rhs_vjp(p, sm.ops, sm.th, x, g, dt * (R)Tsit5::b(i), gw, lane);
+            }
+            R aa = (R)0, ab = (R)0;
+#pragma unroll
+            for (int j = 0; j < 6; ++j) { aa = fma((R)Tsit5::b(j), kl[j].a, aa); ab = fma((R)Tsit5::b(j), kl[j].b, ab); }
+            lam.a = fma(dt, aa, lam.a);
+            lam.b = fma(dt, ab, lam.b);
+            if (s % p.save_every == 0) jump(s / p.save_every);
+        }
+        if (p.grad_u0) stv(p.grad_u0 + n, N, lam, p.D, lane);
+        loss = wsum(loss);
+        if (lane == 0) gw[p.P] = loss;
+    }
+    cta_reduce(p, sm.g);
+}
+
+// ---- 3. adaptive Tsit5 forward: OrdinaryDiffEq's PI controller and initial step, saves from the free interpolant
+// (generic::adaptive_forward_kernel on one warp).  The norms are butterflies, so every decision is warp-uniform ----
+template <typename R>
+__global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
+{
+    using PR = Prec<R>;
+    const Smem<R> sm = carve(p);
+    stage(p, sm.ops, sm.th);
+    const int lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const int traj = blockIdx.x * W + (threadIdx.x >> 5);
+    if (traj >= p.N) return;
+    const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+    const bool on_a = lane < p.D, on_b = lane + 32 < p.D;
+    auto rec = [&](R *b, int row) { return b + ((size_t)row * N + n) * D; };
+    const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
+    const R abstol = p.abstol, reltol = p.reltol, Dr = (R)p.D;
+    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)50, beta2 = (R)2 / (R)25;
+    V<R> u = ldv(p.u0 + n, N, p.D, lane), un, k[7];
+    stv(p.out + n, N, u, p.D, lane);
+    stv(rec(p.usave, 0), 1, u, p.D, lane);
+    stv(rec(p.ustep, 0), 1, u, p.D, lane);
+    if (lane == 0) p.tgrid[n] = t0;
+    k[0] = rhs(p, sm.ops, sm.th, u, lane);
+    stv(rec(p.dense, 0), 1, k[0], p.D, lane);
+    // (x / (abstol + reltol |s|))^2 summed over the lane's components
+    auto sq2 = [&](R xa, R xb, R sa, R sb) {
+        const R ea = xa / (abstol + reltol * sa), eb = xb / (abstol + reltol * sb);
+        return (on_a ? ea * ea : (R)0) + (on_b ? eb * eb : (R)0);
+    };
+    R dt;
+    {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
+        const R d0 = PR::sq(wsum(sq2(u.a, u.b, fabs(u.a), fabs(u.b))) / Dr);
+        const R d1 = PR::sq(wsum(sq2(k[0].a, k[0].b, fabs(u.a), fabs(u.b))) / Dr);
+        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
+        dt0 = fmin(dt0, t1 - t0);
+        const V<R> g{fma(dt0, k[0].a, u.a), fma(dt0, k[0].b, u.b)};
+        un = rhs(p, sm.ops, sm.th, g, lane);
+        const R d2 = PR::sq(wsum(sq2(un.a - k[0].a, un.b - k[0].b, fabs(u.a), fabs(u.b))) / Dr) / dt0;
+        const R dm = fmax(d1, d2);
+        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)5);
+        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+    }
+    R t = t0, qold = (R)1e-4;
+    int nacc = 0, isave = 1, bad = 0;
+    while (isave < p.n_save) {
+        R h = dt;
+        bool clipped = false;
+        if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
+#pragma unroll
+        for (int i = 1; i < 7; ++i) {
+            R aa = (R)0, ab = (R)0;
+#pragma unroll
+            for (int j = 0; j < i; ++j)
+                if (Tsit5::a(i, j) != 0.0) { aa = fma((R)Tsit5::a(i, j), k[j].a, aa); ab = fma((R)Tsit5::a(i, j), k[j].b, ab); }
+            const V<R> g{fma(h, aa, u.a), fma(h, ab, u.b)};
+            if (i == 6) un = g;
+            k[i] = rhs(p, sm.ops, sm.th, g, lane);
+        }
+        R ea = (R)0, eb = (R)0;
+#pragma unroll
+        for (int j = 0; j < 7; ++j) { ea = fma(generic::tsit5_btilde<R>(j), k[j].a, ea); eb = fma(generic::tsit5_btilde<R>(j), k[j].b, eb); }
+        const R EEst = PR::sq(wsum(sq2(h * ea, h * eb, fmax(fabs(u.a), fabs(un.a)), fmax(fabs(u.b), fabs(un.b)))) / Dr);
+        if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
+        const R q11 = PR::pw(EEst, beta1);
+        const R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
+        if (EEst <= (R)1) {
+            if (nacc >= p.max_steps) { bad = 2; break; }
+            const R tn = clipped ? t1 : t + h;
+            for (int i = 1; i < 7; ++i) stv(rec(p.dense, nacc * 6 + i), 1, k[i], p.D, lane);
+            while (isave < p.n_save) {
+                const R ts = t0 + p.save_dt * (R)isave;
+                if (ts > tn + PR::clip * fabs(tn)) break;
+                R bw[7];
+                generic::tsit5_bw_rt(fmin((ts - t) / h, (R)1), bw);
+                R aa = (R)0, ab = (R)0;
+#pragma unroll
+                for (int j = 0; j < 7; ++j) { aa = fma(bw[j], k[j].a, aa); ab = fma(bw[j], k[j].b, ab); }
+                const V<R> us{fma(h, aa, u.a), fma(h, ab, u.b)};
+                stv(p.out + (size_t)isave * D * N + n, N, us, p.D, lane);
+                stv(rec(p.usave, isave), 1, us, p.D, lane);
+                ++isave;
+            }
+            qold = fmax(EEst, (R)1e-4);
+            if (!clipped || h >= dt) dt = h / q;
+            else dt = fmax(dt, h / q);
+            t = tn;
+            ++nacc;
+            if (lane == 0) p.tgrid[(size_t)nacc * N + n] = t;
+            u = un;
+            k[0] = k[6];
+            stv(rec(p.ustep, nacc), 1, u, p.D, lane);
+        } else {
+            dt = h / fmin((R)1 / qmin, q11 / gamma);
+        }
+    }
+    if (bad) {   // failed solve: the unreached save points are NaN
+        const V<R> nan{PR::nan(), PR::nan()};
+        for (int is = isave; is < p.n_save; ++is) {
+            stv(p.out + (size_t)is * D * N + n, N, nan, p.D, lane);
+            stv(rec(p.usave, is), 1, nan, p.D, lane);
+        }
+    }
+    const bool ok = warp_finite(u);
+    if (lane == 0) {
+        p.nacc[n] = nacc;
+        if (p.status) p.status[n] = bad == 2 ? 2 : ((bad || !ok) ? 1 : 0);
+    }
+}
+
+// ---- 4. replay adjoint of an adaptive solve: each accepted step split at the save times inside it, u(t) from the step's free
+// interpolant; the save cotangents at the saved states the forward recorded (the handle's copy, not the caller's `out`) ----
+template <typename R>
+__global__ void __launch_bounds__(128) tsit5_adaptive_adjoint_kernel(Run<R> p)
+{
+    using PR = Prec<R>;
+    const Smem<R> sm = carve(p);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    R *gw = sm.g + (size_t)warp * p.gstride;
+    for (int q = lane; q < p.P + 1; q += 32) gw[q] = (R)0;
+    stage(p, sm.ops, sm.th);
+    const int traj = blockIdx.x * W + warp;
+    if (traj < p.N) {
+        const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+        auto rec = [&](const R *b, int row) { return b + ((size_t)row * N + n) * D; };
+        const int nacc = p.nacc[n];
+        V<R> lam{(R)0, (R)0}, kl[6];
+        R loss = (R)0;
+        auto jump = [&](int is) { save_jump(p, sm.ops, is, ldv(rec(p.usave, is), 1, p.D, lane), lam, loss, n, lane); };
+        int isave = p.n_save - 1;
+        jump(isave);
+        --isave;
+        for (int s = nacc - 1; s >= 0; --s) {
+            const R tn = p.tgrid[(size_t)s * N + n], tn1 = p.tgrid[(size_t)(s + 1) * N + n], hn = tn1 - tn;
+            const R eps = PR::eta * hn;
+            const V<R> u_s = ldv(rec(p.ustep, s), 1, p.D, lane);
+            R cur = tn1;
+            while (cur > tn + eps) {
+                const R ts = p.t0 + p.save_dt * (R)isave;
+                const R ta = (isave >= 0 && ts > tn + eps) ? ts : tn;
+                const R h = cur - ta;
+#pragma unroll
+                for (int i = 0; i < 6; ++i) {
+                    R bw[7];
+                    generic::tsit5_bw_rt(fmin(fmax((cur - (R)Tsit5::c(i) * h - tn) / hn, (R)0), (R)1), bw);
+                    R xa = (R)0, xb = (R)0, ga = (R)0, gb = (R)0;
+#pragma unroll
+                    for (int j = 0; j < 7; ++j) {
+                        const V<R> kj = ldv(rec(p.dense, s * 6 + j), 1, p.D, lane);
+                        xa = fma(bw[j], kj.a, xa);
+                        xb = fma(bw[j], kj.b, xb);
+                    }
+#pragma unroll
+                    for (int j = 0; j < i; ++j)
+                        if (Tsit5::a(i, j) != 0.0) { ga = fma((R)Tsit5::a(i, j), kl[j].a, ga); gb = fma((R)Tsit5::a(i, j), kl[j].b, gb); }
+                    const V<R> x{fma(hn, xa, u_s.a), fma(hn, xb, u_s.b)}, g{fma(h, ga, lam.a), fma(h, gb, lam.b)};
+                    kl[i] = rhs_vjp(p, sm.ops, sm.th, x, g, h * (R)Tsit5::b(i), gw, lane);
+                }
+                R aa = (R)0, ab = (R)0;
+#pragma unroll
+                for (int j = 0; j < 6; ++j) { aa = fma((R)Tsit5::b(j), kl[j].a, aa); ab = fma((R)Tsit5::b(j), kl[j].b, ab); }
+                lam.a = fma(h, aa, lam.a);
+                lam.b = fma(h, ab, lam.b);
+                cur = ta;
+                if (isave >= 0 && fabs(ts - ta) <= eps) { jump(isave); --isave; }
+            }
+        }
+        if (p.grad_u0) stv(p.grad_u0 + n, N, lam, p.D, lane);
+        loss = wsum(loss);
+        if (lane == 0) gw[p.P] = loss;
+    }
+    cta_reduce(p, sm.g);
+}
+
+// ---- 5. RKC2 forward (the recurrence of fkpp_tuned.cuh::forward_rkc_kernel2); records u_n and f(u_n) ----
+template <typename R>
+__global__ void __launch_bounds__(128) rkc2_forward_kernel(Run<R> p)
+{
+    const Smem<R> sm = carve(p);
+    stage(p, sm.ops, sm.th);
+    const int lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const int traj = blockIdx.x * W + (threadIdx.x >> 5);
+    if (traj >= p.N) return;
+    const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+    const R dt = p.dt, mt1 = __ldg(p.rkc);
+    auto rec = [&](R *b, int row) { return b + ((size_t)row * N + n) * D; };
+    V<R> u = ldv(p.u0 + n, N, p.D, lane);
+    stv(p.out + n, N, u, p.D, lane);
+    int isave = 1;
+    for (int s = 0; s < p.n_steps; ++s) {
+        const V<R> F0 = rhs(p, sm.ops, sm.th, u, lane);
+        stv(rec(p.ustep, s), 1, u, p.D, lane);
+        stv(rec(p.dense, s), 1, F0, p.D, lane);
+        V<R> Y0 = u, Y1{fma(mt1 * dt, F0.a, u.a), fma(mt1 * dt, F0.b, u.b)};
+        for (int j = 2; j <= p.S; ++j) {
+            const V<R> F = rhs(p, sm.ops, sm.th, Y1, lane);
+            const R mu = __ldg(p.rkc + RKC_MU + j), nu = __ldg(p.rkc + RKC_NU + j), mt = __ldg(p.rkc + RKC_MT + j), ga = __ldg(p.rkc + RKC_GA + j);
+            const R c0 = (R)1 - mu - nu;
+            const V<R> Y2{fma(ga * dt, F0.a, fma(mt * dt, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * u.a)))),
+                          fma(ga * dt, F0.b, fma(mt * dt, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * u.b))))};
+            Y0 = Y1;
+            Y1 = Y2;
+        }
+        u = Y1;
+        if ((s + 1) % p.save_every == 0) { stv(p.out + (size_t)isave * D * N + n, N, u, p.D, lane); ++isave; }
+    }
+    stv(rec(p.ustep, p.n_steps), 1, u, p.D, lane);
+    stv(rec(p.dense, p.n_steps), 1, rhs(p, sm.ops, sm.th, u, lane), p.D, lane);
+    const bool ok = warp_finite(u);
+    if (p.status && lane == 0) p.status[n] = ok ? 0 : 1;
+}
+
+// ---- 6. RKC2 adjoint (fkpp_tuned.cuh::adjoint_kernel2<.., true>, the oracle's ude_adjoint_rkc2_fixed): lambda stepped backwards
+// with RKC2 itself, u(t) from the cubic Hermite interpolant on (u_n, f_n, u_{n+1}, f_{n+1}); stage j sits at t_{n+1} - c_j dt;
+// the theta-gradient of a step is dt sum_j w_j (df/dtheta)^T(x_j) Y_j with the recurrence's quadrature weights ----
+template <typename R>
+__global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
+{
+    const Smem<R> sm = carve(p);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    R *gw = sm.g + (size_t)warp * p.gstride;
+    for (int q = lane; q < p.P + 1; q += 32) gw[q] = (R)0;
+    stage(p, sm.ops, sm.th);
+    const int traj = blockIdx.x * W + warp;
+    if (traj < p.N) {
+        const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+        const R dt = p.dt, mt1 = __ldg(p.rkc);
+        auto rec = [&](const R *b, int row) { return b + ((size_t)row * N + n) * D; };
+        V<R> lam{(R)0, (R)0};
+        R loss = (R)0;
+        auto jump = [&](int is) { save_jump(p, sm.ops, is, ldv(rec(p.ustep, is * p.save_every), 1, p.D, lane), lam, loss, n, lane); };
+        jump(p.n_steps / p.save_every);
+        for (int s = p.n_steps - 1; s >= 0; --s) {
+            const V<R> y0 = ldv(rec(p.ustep, s), 1, p.D, lane), y1 = ldv(rec(p.ustep, s + 1), 1, p.D, lane);
+            const V<R> f0 = ldv(rec(p.dense, s), 1, p.D, lane), f1 = ldv(rec(p.dense, s + 1), 1, p.D, lane);
+            V<R> Y0 = lam, Y1 = lam, F0{(R)0, (R)0};
+            for (int j = 0; j < p.S; ++j) {
+                const R Th = (R)1 - __ldg(p.rkc + RKC_C + j);
+                // x = (1 - Th) y0 + Th y1 + Th (Th - 1) ((1 - 2 Th) (y1 - y0) + (Th - 1) dt f0 + Th dt f1)
+                auto herm = [&](R a0, R a1, R g0, R g1) {
+                    return ((R)1 - Th) * a0 + Th * a1 + Th * (Th - (R)1) * (((R)1 - (R)2 * Th) * (a1 - a0) + (Th - (R)1) * dt * g0 + Th * dt * g1);
+                };
+                const V<R> x{herm(y0.a, y1.a, f0.a, f1.a), herm(y0.b, y1.b, f0.b, f1.b)};
+                const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, j == 0 ? lam : Y1, dt * __ldg(p.rkc + RKC_W + j), gw, lane);
+                if (j == 0) {
+                    F0 = F;
+                    Y0 = lam;
+                    Y1 = V<R>{fma(mt1 * dt, F0.a, lam.a), fma(mt1 * dt, F0.b, lam.b)};
+                } else {
+                    const R mu = __ldg(p.rkc + RKC_MU + j + 1), nu = __ldg(p.rkc + RKC_NU + j + 1), mt = __ldg(p.rkc + RKC_MT + j + 1),
+                            ga = __ldg(p.rkc + RKC_GA + j + 1);
+                    const R c0 = (R)1 - mu - nu;
+                    const V<R> Y2{fma(ga * dt, F0.a, fma(mt * dt, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * lam.a)))),
+                                  fma(ga * dt, F0.b, fma(mt * dt, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * lam.b))))};
+                    Y0 = Y1;
+                    Y1 = Y2;
+                }
+            }
+            lam = Y1;
+            if (s % p.save_every == 0) jump(s / p.save_every);
+        }
+        if (p.grad_u0) stv(p.grad_u0 + n, N, lam, p.D, lane);
+        loss = wsum(loss);
+        if (lane == 0) gw[p.P] = loss;
+    }
+    cta_reduce(p, sm.g);
+}
+
+}  // namespace op
+}  // namespace b200ude

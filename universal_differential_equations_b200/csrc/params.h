@@ -250,4 +250,32 @@ int adj_rows_forced(int N, int dtype);
 cudaError_t launch_fwd_forced(const ForcedHost &, const ForcedRun &, cudaStream_t);
 cudaError_t launch_adj_forced(const ForcedHost &, const ForcedRun &, cudaStream_t, int *rows_out);
 
+// ---- wide-state operator UDE du = D1 NN(u) + D2 u (B200UDE_MODEL_OPERATOR; operator.cuh, k_operator.cu), fp32 and fp64 ----
+struct OperatorHost {
+    int dtype;                // 0 = float, 1 = double: every pointer below and in OperatorRun
+    int D, M, L, P, has_d2;   // states, chain outputs, layers, parameters, D2 given
+    int widths[6], acts[5];
+    int rkc2, S;              // RKC2 with S stages (else Tsit5)
+    int warps;                // warps (trajectories) per CTA
+    int dyn_cap;              // dynamic shared memory every launch is allowed: the device's opt-in limit less the kernels' static size
+    // staged layout (operator_layout): odd leading dimensions, offsets, block sizes in elements
+    int ld1, ld2, woff[5], soff[5], ldw[5], ops_elems, theta_elems, gstride;
+    const void *ops;          // [64 loss weights | D1 (ld1 x M) | D2 (ld2 x D)], ops_elems elements
+    const void *theta, *rkc;  // the handle's theta, RKC2 tables
+};
+struct OperatorRun {
+    const void *u0, *cot;
+    void *out, *ustep, *dense, *usave, *grad_u0, *partial, *tgrid;
+    int32_t *status;
+    int *nacc;
+    int N, n_steps, save_every, n_save, max_steps, fused_l2, adaptive;
+    double t0, dt, save_dt, abstol, reltol;
+};
+void operator_layout(OperatorHost &);                      // fills P and the staged layout from D, M, L, widths
+size_t operator_smem(const OperatorHost &, int warps);     // dynamic shared memory of a CTA (warps = 0: the forward kernels)
+int adj_rows_operator(int N, int warps);
+cudaError_t operator_static_smem(int dtype, size_t *bytes);   // the largest static shared memory of the dtype's six kernels (current device)
+cudaError_t launch_fwd_operator(const OperatorHost &, const OperatorRun &, cudaStream_t);
+cudaError_t launch_adj_operator(const OperatorHost &, const OperatorRun &, cudaStream_t, int *rows_out);
+
 }  // namespace b200ude

@@ -180,6 +180,41 @@ class NeuralODE:
         return self.chain.num_params()
 
 
+@dataclass(eq=False)
+class OperatorUDE:
+    """A method-of-lines UDE with a learned closure (Climate/NeuralPDE/npde.jl:75-78):
+
+        du = D1 @ chain(u) + D2 @ u,   chain: d -> ... -> m,  D1 [d, m] and D2 [d, d] fixed (not trained).
+
+    D2 = None is a zero D2, so OperatorUDE(chain, np.eye(d)) is a plain neural ODE of any width up to 64.  A UDESolver
+    uploads the operators when it is built; `UDESolver.set_operators` replaces them."""
+    chain: FastChain
+    D1: np.ndarray
+    D2: Optional[np.ndarray] = None
+
+    model = _lib.MODEL_OPERATOR
+
+    def __post_init__(self):
+        d, m = self.chain.widths[0], self.chain.widths[-1]
+        self.D1 = np.asarray(self.D1, dtype=np.float64)
+        if self.D1.shape != (d, m):
+            raise ValueError(f"D1 must be [{d}, {m}] (state_dim x chain output), got {self.D1.shape}")
+        if self.D2 is not None:
+            self.D2 = np.asarray(self.D2, dtype=np.float64)
+            if self.D2.shape != (d, d):
+                raise ValueError(f"D2 must be [{d}, {d}], got {self.D2.shape}")
+
+    @property
+    def state_dim(self):
+        return self.chain.widths[0]
+
+    def consts(self):
+        return ()
+
+    def num_params(self):
+        return self.chain.num_params()
+
+
 @dataclass
 class SEIRNeuralODE:
     """dudt_node of the SEIR script (seir_exposure.jl:52-64): dS,dE,dI,dR,dD = first five outputs of
@@ -443,6 +478,8 @@ class UDESolver:
         self.capacity = int(max_trajectories)
         self.adaptive, self.max_steps = bool(adaptive), int(max_steps)
         self.generation = 0   # bumped by every set_params / forward: identifies the forward record the handle holds
+        if f.model == _lib.MODEL_OPERATOR:
+            self.set_operators(f.D1, f.D2)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -479,6 +516,19 @@ class UDESolver:
         if not coef.is_cuda:
             torch.cuda.current_stream(self.device).synchronize()   # the host copy is read by the stream-ordered upload
         self._forcing = coef
+        self.generation += 1
+
+    def set_operators(self, D1, D2=None):
+        """Operator model: D1 [d, m] and D2 [d, d] (None: zero), uploaded column-major in the solver's dtype."""
+        def colmajor(A):
+            A = A.detach().cpu().numpy() if isinstance(A, torch.Tensor) else np.asarray(A)
+            return np.asfortranarray(A, dtype=np.float64 if self.dtype == torch.float64 else np.float32)
+        a1 = colmajor(D1)
+        a2 = None if D2 is None else colmajor(D2)
+        _lib.check(self._h, self._L.b200ude_set_operators(self._h, a1.ctypes.data, None if a2 is None else a2.ctypes.data,
+                                                           _lib.HOST, _stream_ptr(self.device)))
+        torch.cuda.current_stream(self.device).synchronize()   # the host arrays are read by the stream-ordered upload
+        self._ops_keepalive = (a1, a2)
         self.generation += 1
 
     def forward(self, u0: torch.Tensor, out: Optional[torch.Tensor] = None, status: Optional[torch.Tensor] = None):
