@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <atomic>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "params.h"
@@ -25,24 +26,26 @@ namespace {
 
 thread_local std::string g_create_error;
 
-// kernel families compiled into this build (one translation unit each, see k_*.cu)
+// kernel families compiled into this build (one translation unit each, see k_*.cu); a handle's dtype picks the precision
 //   K_LV32   LV 2 -> 32 -> 32 -> 2 tanh                      BASELINE config 2
 //   K_LV5Px  LV 2 -> 5 -> 5 -> 5 -> 2, per-layer activations, x trainable linear rates
 //            scenario_1.jl:62-73 (x=0), scenario_2.jl:79-98 (x=1), hudson_bay.jl:77-91 (x=2)
-//   K_GENERIC  any LV / SEIR / SEIR_NODE / NODE form with chain widths <= 64 and <= 5 layers (k_generic.cu): functional
-//            coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7, the adaptive path of untuned chains and
-//            the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh; through Vern7's interpolated
+//   K_GENERIC  any LV / SEIR / SEIR_NODE / NODE form with chain widths <= 64 and <= 5 layers (k_generic.cu fp32, k_f64.cu fp64):
+//            functional coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7, the adaptive path of untuned chains
+//            and the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh; through Vern7's interpolated
 //            saves: vern7_dense_discrete.cuh)
-//   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126); also
-//            adaptive Tsit5 (fkpp_adaptive.cuh) and adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
+//   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126); fixed step
+//            (fp32), adaptive Tsit5 (fkpp_adaptive.cuh) and adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
 //   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
 //   K_FKPP16   Fisher-KPP UPDE with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu)                BASELINE config 4
-//   K_FORCED   forced neural ODE with a readout network (FENEP.jl:41-62), fp32 (k_forced.cu; its fp64 handles are K_F64)
-//   K_OPERATOR wide-state operator UDE du = D1 NN(u) + D2 u (npde.jl:75-78), warp per trajectory, fp32 (k_operator.cu; its fp64
-//            handles are K_F64)
-enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_F64, K_FORCED, K_OPERATOR };
+//   K_FORCED   forced neural ODE with a readout network (FENEP.jl:41-62) (k_forced.cu)
+//   K_OPERATOR wide-state operator UDE du = D1 NN(u) + D2 u (npde.jl:75-78), warp per trajectory (k_operator.cu)
+// The fp64 handles are K_GENERIC, K_FKPP, K_FORCED and K_OPERATOR; the others are fp32 only.
+enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_FORCED, K_OPERATOR };
 
-int kernel_num_params(KernelId k)
+// parameters of a handle: the tuned chains' fixed counts, else n_prefix + the dense layers + n_suffix.  The forced model's f0 and f1
+// lie back to back in `widths`: its layers l >= L0 read one entry further on
+int num_params(const b200ude_desc *d, KernelId k)
 {
     switch (k) {
     case K_LV32: return 2 * 32 + 32 + 32 * 32 + 32 + 32 * 2 + 2;
@@ -51,8 +54,15 @@ int kernel_num_params(KernelId k)
     case K_LV5P0: return 87;
     case K_LV5P1: return 88;
     case K_LV5P2: return 89;
-    default: return 0;
+    default: break;
     }
+    const int L0 = k == K_FORCED ? (int)d->consts[0] : d->n_layers;
+    int P = d->n_prefix + d->n_suffix;
+    for (int l = 0; l < d->n_layers; ++l) {
+        const int a = l < L0 ? l : l + 1;
+        P += d->widths[a] * d->widths[a + 1] + d->widths[a + 1];
+    }
+    return P;
 }
 
 std::atomic<uint64_t> g_serial{0};   // handles may be created from several host threads (one per GPU)
@@ -62,8 +72,10 @@ std::atomic<uint64_t> g_serial{0};   // handles may be created from several host
 struct b200ude_handle {
     b200ude_desc desc;
     KernelId kid = K_NONE;
+    bool f64 = false;   // dtype = B200UDE_F64: every real-valued device array of the handle and of the callers is double
     Variant var;
-    ConstTables tab;
+    ConstTables tab;    // fp32 runtime-shape and tuned kernels
+    Tables64 tab64;     // fp64 runtime-shape kernels
     GenericShape gen;
     int P = 0, n_save = 0, D = 0;
     int DR = 0;      // rows per save of out / data / dL_dout: D, or D + r for the forced model
@@ -73,19 +85,19 @@ struct b200ude_handle {
     bool have_theta = false;
     int sm_count = 0;
     size_t wm_fwd_max = 0, wm_adj_max = 0;   // largest ensembles the warp-collective LV kernels are chosen for (auto mode)
-    // device buffers
-    float *d_theta = nullptr;
-    float *d_ustep = nullptr;
-    float *d_dense = nullptr;
-    float *d_partial = nullptr;
+    // device buffers of the handle's real type (es() bytes per element)
+    void *d_theta = nullptr;
+    void *d_ustep = nullptr;
+    void *d_dense = nullptr;
+    void *d_partial = nullptr;
     size_t partial_blocks = 0;
     // adaptive stepping
     bool adaptive = false;
-    float *d_tgrid = nullptr, *d_cot = nullptr, *d_block_loss = nullptr;
-    float *d_hstep = nullptr;   // discrete-adjoint Vern7: step sizes of the accepted steps
+    void *d_tgrid = nullptr, *d_cot = nullptr;
+    void *d_hstep = nullptr;   // discrete-adjoint Vern7: step sizes of the accepted steps
+    float *d_block_loss = nullptr;
     int *d_nacc = nullptr;
-    const float *last_out = nullptr;
-    AdaptiveGrid ag{};
+    const void *last_out = nullptr;
     // host-buffer path
     float *d_u0 = nullptr, *d_out = nullptr, *d_data = nullptr, *d_gu0 = nullptr, *d_grad = nullptr, *d_loss = nullptr;
     int32_t *d_status = nullptr;
@@ -99,32 +111,26 @@ struct b200ude_handle {
     PeerLinks peer;                 // every rank's buffer as mapped here
     bool peer_attached = false;
     // on-device optimiser (b200ude_adam_*, b200ude_train_adam)
-    float *d_u0_keep = nullptr, *d_aux_out = nullptr;   // Vern7: u0 of the last forward, saved states of the Tsit5 re-solve
+    void *d_u0_keep = nullptr, *d_aux_out = nullptr;   // Vern7: u0 of the last forward, saved states of the Tsit5 re-solve
     bool vern7_pending = false;
     bool vern7_dense = false;   // B200UDE_FLAG_VERN7_DENSE: saveat and the interpolating adjoint through Vern7's own dense output
     bool discrete_dense = false;   // B200UDE_FLAG_DISCRETE_DENSE on an adaptive grid: saveat through the interpolant, discrete adjoint through it
     float *d_adam_m = nullptr, *d_adam_v = nullptr, *d_train_out = nullptr;
     int *d_adam_t = nullptr;
     int adam_t = 0;   // host mirror of the step counter
-    // double-precision path (dtype = B200UDE_F64, kid = K_F64): every device array of the handle and of the callers is double
-    Shape64Host sh64{};
-    double *q_theta = nullptr, *q_ustep = nullptr, *q_dense = nullptr, *q_partial = nullptr, *q_tgrid = nullptr, *q_cot = nullptr;
-    double *q_u0_keep = nullptr, *q_aux_out = nullptr, *q_hstep = nullptr;
-    const double *q_last_out = nullptr;
-    // forced neural ODE (B200UDE_MODEL_FORCED, either dtype): shape, the forcing coefficients [3J][cap], the last forward's out
-    bool forced = false;
+    // forced neural ODE (K_FORCED): shape, the forcing coefficients [3J][cap], the last forward's out
     ForcedHost fh{};
     void *d_forcing = nullptr;
     size_t forcing_n = 0;   // trajectories of the last b200ude_set_forcing
     void *d_usave = nullptr;   // adaptive: the saved states of the last forward [n_save][D][cap], read by the replay adjoint
-    // operator UDE (B200UDE_MODEL_OPERATOR, either dtype): shape, the padded operator block, the RKC2 tables (handle dtype);
-    // it shares d_usave (as [n_save][cap][D]) and the record buffers with the forced model
-    bool op = false;
+    // operator UDE (K_OPERATOR): shape, the padded operator block, the RKC2 tables (handle dtype); it shares d_usave (as
+    // [n_save][cap][D]) and the record buffers with the forced model
     bool ops_set = false;
     OperatorHost oh{};
     void *d_ops = nullptr, *d_rkc = nullptr;
     size_t dev_bytes = 0;
     std::string err;
+    size_t es() const { return f64 ? sizeof(double) : sizeof(float); }
 };
 
 namespace {
@@ -149,13 +155,21 @@ int32_t fail(b200ude_handle *h, int32_t code, const char *fmt, ...)
         }                                                                                                \
     } while (0)
 
+cudaError_t dalloc_bytes(b200ude_handle *h, void **p, size_t bytes)
+{
+    cudaError_t e = cudaMalloc(p, bytes);
+    if (e == cudaSuccess) h->dev_bytes += bytes;
+    return e;
+}
+
 template <class T>
 cudaError_t dalloc(b200ude_handle *h, T **p, size_t count)
 {
-    cudaError_t e = cudaMalloc((void **)p, count * sizeof(T));
-    if (e == cudaSuccess) h->dev_bytes += count * sizeof(T);
-    return e;
+    return dalloc_bytes(h, (void **)p, count * sizeof(T));
 }
+
+// count elements of the handle's real type
+cudaError_t dalloc_real(b200ude_handle *h, void **p, size_t count) { return dalloc_bytes(h, p, count * h->es()); }
 
 // RKC2 (Sommeijer, Shampine, Verwer 1998) recurrence coefficients, stage abscissae and the quadrature weights of the stage
 // integrands (from running the recurrence on unit impulses)
@@ -265,69 +279,170 @@ KernelId pick_kernel(const b200ude_desc &d)
 }
 
 
-// the forced neural ODE's forward and adjoint (both dtypes; defined with the fp64 path below)
-int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
-int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer);
-// the operator UDE's forward and adjoint (both dtypes; defined with the fp64 path below)
-int32_t do_forward_operator(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
-int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer);
+template <typename R>
+constexpr bool is_f32 = std::is_same<R, float>::value;
 
-// Tsit5 forward solve with the dense record (stage derivatives) the interpolating adjoint reads
-int32_t tsit5_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int32_t *status, cudaStream_t st)
+// the forced neural ODE's and the operator UDE's forward, and the launch of their adjoints (both dtypes; defined below)
+int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
+int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *grad_u0, cudaStream_t st, int *rows);
+int32_t do_forward_operator(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
+int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *grad_u0, cudaStream_t st, int *rows);
+
+// the fp32-only kernels: the tuned families (LV 2-32-32-2, LV 2-5-5-5-2, SEIR 3-64-64-1 -- its fixed-step Vern7 included --,
+// Fisher-KPP 1-16-16-1, the only one with RKC2) and fixed-step Fisher-KPP.  Every other handle, fp32 or fp64, runs on the
+// runtime-shape kernels (RuntimeShape<R>).
+bool fp32_only(const b200ude_handle *h)
+{
+    return h->kid == K_LV32 || h->kid == K_LV5P0 || h->kid == K_LV5P1 || h->kid == K_LV5P2 || h->kid == K_SEIR64 || h->kid == K_FKPP16 ||
+           (h->kid == K_FKPP && !h->adaptive);
+}
+
+// the kernels' parameter structs of each precision
+FwdParams fwd_params(const b200ude_handle *h, const float *u0, float *out, void *ustep, void *dense, int32_t *status, size_t N)
 {
     FwdParams p;
-    p.u0 = u0; p.out = out; p.ustep = h->d_ustep; p.dense = h->d_dense; p.status = status; p.theta = h->d_theta;
+    p.u0 = u0; p.out = out; p.ustep = (float *)ustep; p.dense = (float *)dense; p.status = status; p.theta = (const float *)h->d_theta;
     p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
-    cudaError_t e = cudaSuccess;
-    if (h->adaptive) {
-        e = h->kid == K_LV32 ? launch_fwd_lv32_adaptive(h->var, h->tab, p, h->ag, st)
-            : h->kid == K_SEIR64 ? launch_fwd_seir_adaptive(h->var, h->tab, p, h->ag, st)
-            : h->kid == K_FKPP ? launch_fwd_fkpp_adaptive(h->gen, h->tab, p, h->ag, st) : launch_fwd_adaptive(h->gen, h->tab, p, h->ag, st);
-        CUDA_TRY(h, e);
-        h->last_out = out;
-        return B200UDE_OK;
-    }
-    if (h->desc.solver == B200UDE_RKC2) {
-        CUDA_TRY(h, launch_fwd_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st));
-        return B200UDE_OK;
-    }
+    return p;
+}
+Fwd64Host fwd_params(const b200ude_handle *h, const double *u0, double *out, void *ustep, void *dense, int32_t *status, size_t N)
+{
+    return Fwd64Host{u0, out, (double *)ustep, (double *)dense, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
+}
+AdjParams adj_params(const b200ude_handle *h, const float *cot, float *grad_u0, bool l2)
+{
+    AdjParams p;
+    p.ustep = (const float *)h->d_ustep; p.dense = (const float *)h->d_dense; p.cot = cot; p.grad_u0 = grad_u0; p.partial = (float *)h->d_partial;
+    p.theta = (const float *)h->d_theta; p.N = (int)h->N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P;
+    p.fused_l2 = l2 ? 1 : 0;
+    p.dt = (float)h->desc.dt;
+    return p;
+}
+Adj64Host adj_params(const b200ude_handle *h, const double *cot, double *grad_u0, bool l2)
+{
+    return Adj64Host{(const double *)h->d_ustep, (const double *)h->d_dense, cot, grad_u0, (double *)h->d_partial, (int)h->N, h->desc.n_steps,
+                     h->desc.save_every, l2 ? 1 : 0, h->desc.dt};
+}
+template <typename R>
+typename RealParams<R>::Adapt adapt(const b200ude_handle *h)
+{
+    return {(R)h->desc.t0, (R)(h->desc.dt * h->desc.save_every), (R)h->desc.abstol, (R)h->desc.reltol, h->n_save, h->desc.max_steps,
+            (R *)h->d_tgrid, h->d_nacc, (R *)h->d_hstep};
+}
+template <typename R>
+const typename RealParams<R>::Tab &tables(const b200ude_handle *h)
+{
+    if constexpr (is_f32<R>) return h->tab;
+    else return h->tab64;
+}
+
+// forward of the fp32-only kernels; solver 1: the SEIR chain's fixed-step Vern7
+cudaError_t forward32(b200ude_handle *h, const FwdParams &p, size_t N, int solver, cudaStream_t st)
+{
+    if (solver == 1) return launch_fwd_seir_vern7(h->var, h->tab, p, st);   // tensor-core kernels (seir_tc.cuh)
+    if (h->adaptive)   // the headline chains: tensor-core kernels with CTA-uniform attempt loops
+        return h->kid == K_LV32 ? launch_fwd_lv32_adaptive(h->var, h->tab, p, adapt<float>(h), st)
+                                : launch_fwd_seir_adaptive(h->var, h->tab, p, adapt<float>(h), st);
+    if (h->desc.solver == B200UDE_RKC2) return launch_fwd_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st);
     switch (h->kid) {
     case K_LV32:
         // small / medium ensembles: the warp-collective family (latency per stage ~4x lower); large ones: one trajectory per thread
-        e = use_wm(h->var.fwd_wm, N, h->wm_fwd_max) ? launch_fwd_lv32_wm(h->var, h->tab, p, st) : launch_fwd_lv32(h->var, h->tab, p, st);
-        break;
-    case K_LV5P0: e = launch_fwd_lv5(0, h->var, h->tab, p, st); break;
-    case K_LV5P1: e = launch_fwd_lv5(1, h->var, h->tab, p, st); break;
-    case K_LV5P2: e = launch_fwd_lv5(2, h->var, h->tab, p, st); break;
-    case K_GENERIC: e = launch_fwd_generic(h->gen, h->tab, p, st); break;
-    case K_FKPP: e = launch_fwd_fkpp(h->gen, h->tab, p, st); break;
-    case K_SEIR64: e = launch_fwd_seir(h->var, h->tab, p, st); break;
-    case K_FKPP16: e = launch_fwd_fkpp16(h->var, h->tab, p, h->D, st); break;
-    default: return fail(h, B200UDE_EUNSUPPORTED, "forward: no kernel");
+        return use_wm(h->var.fwd_wm, N, h->wm_fwd_max) ? launch_fwd_lv32_wm(h->var, h->tab, p, st) : launch_fwd_lv32(h->var, h->tab, p, st);
+    case K_LV5P0: return launch_fwd_lv5(0, h->var, h->tab, p, st);
+    case K_LV5P1: return launch_fwd_lv5(1, h->var, h->tab, p, st);
+    case K_LV5P2: return launch_fwd_lv5(2, h->var, h->tab, p, st);
+    case K_FKPP: return launch_fwd_fkpp(h->gen, h->tab, p, st);
+    case K_SEIR64: return launch_fwd_seir(h->var, h->tab, p, st);
+    default: return launch_fwd_fkpp16(h->var, h->tab, p, h->D, st);   // K_FKPP16
     }
-    CUDA_TRY(h, e);
+}
+
+// adjoint of the fp32-only kernels.  split: the two data-ready events of the host-buffer path, under which the warp-collective LV
+// adjoint runs as two sub-range launches (the first one under the second half's upload), or nullptr
+cudaError_t adjoint32(b200ude_handle *h, const AdjParams &p, const cudaEvent_t *split, size_t split_at, cudaStream_t st, int *rows)
+{
+    if (h->adaptive)
+        return h->kid == K_LV32 ? launch_adj_lv32_adaptive(h->var, h->tab, p, adapt<float>(h), st, rows)
+                                : launch_adj_seir_adaptive(h->var, h->tab, p, adapt<float>(h), st, rows);
+    if (h->desc.solver == B200UDE_RKC2) return launch_adj_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st, rows);
+    switch (h->kid) {
+    case K_LV32:
+        if (split) {
+            int g0 = 0, g1 = 0;
+            AdjParams q = p;
+            q.n0 = 0; q.n_cnt = (int)split_at; q.row0 = 0;
+            cudaError_t e = cudaStreamWaitEvent(st, split[0], 0);
+            if (e == cudaSuccess) e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g0);
+            if (e == cudaSuccess) {
+                q.n0 = (int)split_at; q.n_cnt = (int)(h->N - split_at); q.row0 = g0;
+                e = cudaStreamWaitEvent(st, split[1], 0);
+                if (e == cudaSuccess) e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g1);
+            }
+            *rows = g0 + g1;
+            return e;
+        }
+        return (!h->var.discrete && use_wm(h->var.adj_wm, h->N, h->wm_adj_max)) ? launch_adj_lv32_wm(h->var, h->tab, p, st, rows)
+                                                                                : launch_adj_lv32(h->var, h->tab, p, st, rows);
+    case K_LV5P0: return launch_adj_lv5(0, h->var, h->tab, p, st, rows);
+    case K_LV5P1: return launch_adj_lv5(1, h->var, h->tab, p, st, rows);
+    case K_LV5P2: return launch_adj_lv5(2, h->var, h->tab, p, st, rows);
+    case K_FKPP: return launch_adj_fkpp(h->gen, h->tab, p, st, rows);
+    case K_SEIR64: return launch_adj_seir(h->var, h->tab, p, st, rows);
+    default: return launch_adj_fkpp16(h->var, h->tab, p, h->D, st, rows);   // K_FKPP16
+    }
+}
+
+// Tsit5 (solver 0) or Vern7 (solver 1) forward of a runtime-shape or fp32-only handle; the Tsit5 solve writes the dense record
+// (stage derivatives) the interpolating adjoint reads
+template <typename R>
+cudaError_t launch_forward(b200ude_handle *h, const typename RealParams<R>::Fwd &p, size_t N, int solver, cudaStream_t st)
+{
+    if constexpr (is_f32<R>)
+        if (fp32_only(h)) return forward32(h, p, N, solver, st);
+    const auto ag = adapt<R>(h);
+    if (h->kid == K_FKPP) return RuntimeShape<R>::fwd_fkpp_adaptive(h->gen, tables<R>(h), p, ag, st);   // adaptive Tsit5 (b200ude_create)
+    return RuntimeShape<R>::fwd(h->gen, tables<R>(h), p, solver, h->adaptive ? &ag : nullptr, st);
+}
+
+// the interpolating adjoint of that Tsit5 solve (the replay of an adaptive one)
+template <typename R>
+cudaError_t launch_adjoint(b200ude_handle *h, const typename RealParams<R>::Adj &p, const cudaEvent_t *split, size_t split_at, cudaStream_t st,
+                           int *rows)
+{
+    if constexpr (is_f32<R>)
+        if (fp32_only(h)) return adjoint32(h, p, split, split_at, st, rows);
+    const auto ag = adapt<R>(h);
+    if (h->kid == K_FKPP) return RuntimeShape<R>::adj_fkpp_adaptive(h->gen, tables<R>(h), p, ag, st, rows);
+    return RuntimeShape<R>::adj(h->gen, tables<R>(h), p, h->adaptive ? &ag : nullptr, st, rows);
+}
+
+template <typename R>
+int32_t tsit5_forward(b200ude_handle *h, const R *u0, size_t N, R *out, int32_t *status, cudaStream_t st)
+{
+    CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, u0, out, h->d_ustep, h->d_dense, status, N), N, 0, st));
+    h->last_out = out;
     return B200UDE_OK;
 }
 
-int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int32_t *status, cudaStream_t st)
+template <typename R>
+int32_t do_forward(b200ude_handle *h, const R *u0, size_t N, R *out, int32_t *status, cudaStream_t st)
 {
     CUDA_TRY(h, cudaSetDevice(h->desc.device));   // launches, symbol copies and function attributes go to the handle's device
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
-    if (h->forced) return do_forward_forced(h, u0, N, out, status, st);
-    if (h->op) return do_forward_operator(h, u0, N, out, status, st);
+    if (h->kid == K_FORCED) return do_forward_forced(h, u0, N, out, status, st);
+    if (h->kid == K_OPERATOR) return do_forward_operator(h, u0, N, out, status, st);
     if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
         // discrete adjoint, or the interpolating adjoint over Vern7's dense output: the forward records u_n of every (accepted)
         // step, which the adjoint recomputes the stages from.  With either dense flag an adaptive solve saves through the
         // interpolant; a fixed grid saves at step ends either way
-        FwdParams p;
-        p.u0 = u0; p.out = out; p.ustep = h->d_ustep; p.dense = nullptr; p.status = status; p.theta = h->d_theta;
-        p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
-        if (h->kid == K_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7(h->gen, h->tab, p, h->ag, st));   // adaptive only (b200ude_create)
-        else if (h->adaptive && (h->vern7_dense || h->discrete_dense)) CUDA_TRY(h, launch_fwd_vern7_dense(h->gen, h->tab, p, h->ag, st));
-        else if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
-        else CUDA_TRY(h, launch_fwd_vern7(h->gen, h->tab, p, st));
+        using RS = RuntimeShape<R>;
+        const auto p = fwd_params(h, u0, out, h->d_ustep, nullptr, status, N);
+        const auto ag = adapt<R>(h);
+        if (h->kid == K_FKPP) CUDA_TRY(h, RS::fwd_fkpp_vern7(h->gen, tables<R>(h), p, ag, st));   // adaptive only (b200ude_create)
+        else if (h->adaptive && (h->vern7_dense || h->discrete_dense)) CUDA_TRY(h, RS::fwd_vern7_dense(h->gen, tables<R>(h), p, ag, st));
+        else CUDA_TRY(h, RS::fwd(h->gen, tables<R>(h), p, 1, h->adaptive ? &ag : nullptr, st));
         h->last_out = out;
         h->N = N;
         h->have_forward = true;
@@ -337,15 +452,10 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
         // Vern7 writes the saved states only.  Its lazy dense output is not available (SURVEY.md App. A.3), so the
         // interpolating adjoint of a Vern7 solve runs over a Tsit5 re-solve from the same u0 with the same step /
         // tolerances, launched by the first adjoint call (do_adjoint); u0 is kept for that.
-        FwdParams p;
-        p.u0 = u0; p.out = out; p.ustep = nullptr; p.dense = nullptr; p.status = status; p.theta = h->d_theta;
-        p.N = (int)N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P; p.dt = (float)h->desc.dt;
-        if (h->adaptive) CUDA_TRY(h, launch_fwd_vern7_adaptive(h->gen, h->tab, p, h->ag, st));
-        else if (h->kid == K_SEIR64) CUDA_TRY(h, launch_fwd_seir_vern7(h->var, h->tab, p, st));   // tensor-core kernels (seir_tc.cuh)
-        else CUDA_TRY(h, launch_fwd_vern7(h->gen, h->tab, p, st));
-        if (!h->d_u0_keep && dalloc(h, &h->d_u0_keep, (size_t)h->D * h->cap) != cudaSuccess)
+        CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, u0, out, nullptr, nullptr, status, N), N, 1, st));
+        if (!h->d_u0_keep && dalloc_real(h, &h->d_u0_keep, (size_t)h->D * h->cap) != cudaSuccess)
             return fail(h, B200UDE_ENOMEM, "forward: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-        CUDA_TRY(h, cudaMemcpyAsync(h->d_u0_keep, u0, sizeof(float) * (size_t)h->D * N, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_u0_keep, u0, sizeof(R) * (size_t)h->D * N, cudaMemcpyDeviceToDevice, st));
         h->N = N;
         h->have_forward = false;
         h->vern7_pending = true;
@@ -358,18 +468,32 @@ int32_t do_forward(b200ude_handle *h, const float *u0, size_t N, float *out, int
     return B200UDE_OK;
 }
 
+// partial rows -> grad_theta and the loss (nullptr: not written): fp64 reduce, fp32 reduce fused with the all-reduce over the
+// attached peers, or fp32 reduce
+int32_t reduce_partials(b200ude_handle *h, int rows, void *grad_theta, void *loss, bool peer, cudaStream_t st)
+{
+    if (h->f64) CUDA_TRY(h, launch_reduce_f64((const double *)h->d_partial, rows, h->P + 1, (double *)grad_theta, (double *)loss, st));
+    else if (peer) CUDA_TRY(h, launch_reduce_exchange((const float *)h->d_partial, rows, h->P + 1, h->peer, (float *)grad_theta, (float *)loss, st));
+    else CUDA_TRY(h, launch_reduce((const float *)h->d_partial, rows, h->P + 1, (float *)grad_theta, (float *)loss, st));
+    return B200UDE_OK;
+}
+
 // split: two events (data of the first / second half of the trajectories resident) for the host-buffer path: the warp-collective LV
 // adjoint then runs as two sub-range launches, the first one under the second half's upload
-int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, float *grad_theta,
-                   float *grad_u0, cudaStream_t st, bool peer = false, const cudaEvent_t *split = nullptr, size_t split_at = 0)
+template <typename R>
+int32_t do_adjoint(b200ude_handle *h, bool l2, const R *cot, R *loss, R *grad_theta, R *grad_u0, cudaStream_t st, bool peer = false,
+                   const cudaEvent_t *split = nullptr, size_t split_at = 0)
 {
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
     if (peer && !h->peer_attached) return fail(h, B200UDE_ESTATE, "adjoint_l2_allreduce: b200ude_peer_attach has not been called");
     if (peer && h->adaptive) return fail(h, B200UDE_EUNSUPPORTED, "adjoint_l2_allreduce: not available with adaptive stepping (all-reduce the result of b200ude_adjoint_l2 instead)");
+    // an fp64 operator handle names its missing operators before the missing forward solution
+    if (h->f64 && h->kid == K_OPERATOR && !h->ops_set)
+        return fail(h, B200UDE_ESTATE, "adjoint: B200UDE_MODEL_OPERATOR needs its operators (call b200ude_set_operators first)");
     if (h->desc.solver == B200UDE_VERN7 && h->vern7_pending) {
-        if (!h->d_aux_out && dalloc(h, &h->d_aux_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
+        if (!h->d_aux_out && dalloc_real(h, &h->d_aux_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
             return fail(h, B200UDE_ENOMEM, "adjoint: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-        int32_t rc = tsit5_forward(h, h->d_u0_keep, h->N, h->d_aux_out, nullptr, st);
+        int32_t rc = tsit5_forward(h, (const R *)h->d_u0_keep, h->N, (R *)h->d_aux_out, nullptr, st);
         if (rc) return rc;
         h->vern7_pending = false;
         h->have_forward = true;
@@ -382,99 +506,54 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const float *cot, float *loss, fl
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[0], 0));
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[1], 0));
     }
-    if (h->forced) return do_adjoint_forced(h, l2, cot, loss, grad_theta, grad_u0, st, peer);
-    if (h->op) return do_adjoint_operator(h, l2, cot, loss, grad_theta, grad_u0, st, peer);
-    AdjParams p;
-    p.ustep = h->d_ustep; p.dense = h->d_dense; p.cot = cot; p.grad_u0 = grad_u0; p.partial = h->d_partial;
-    p.theta = h->d_theta; p.N = (int)h->N; p.n_steps = h->desc.n_steps; p.save_every = h->desc.save_every; p.P = h->P;
-    p.fused_l2 = l2 ? 1 : 0;
-    p.dt = (float)h->desc.dt;
-    cudaError_t e = cudaSuccess;
-    int grid = 0;
+    int rows = 0;
+    if (h->kid == K_FORCED || h->kid == K_OPERATOR) {
+        const int32_t rc = h->kid == K_FORCED ? do_adjoint_forced(h, l2, cot, grad_u0, st, &rows) : do_adjoint_operator(h, l2, cot, grad_u0, st, &rows);
+        return rc ? rc : reduce_partials(h, rows, grad_theta, loss, peer, st);
+    }
+    using RS = RuntimeShape<R>;
+    const auto &t = tables<R>(h);
+    const auto ag = adapt<R>(h);
+    auto p = adj_params(h, cot, grad_u0, l2);
+    const R *saved = (const R *)h->last_out;
+    R *reduce_loss = loss;
+    bool finish_l2 = false;   // fp32 two-stage L2 cotangent: its loss follows the reduce
     if (h->vern7_dense) {
         // interpolating adjoint over the Vern7 solve's own dense output; the fused L2 reads the states the forward returned
-        CUDA_TRY(h, launch_adj_vern7_dense(h->gen, h->tab, p, h->adaptive ? &h->ag : nullptr, h->last_out, st, &grid));
-        if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
-        else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->discrete_dense) {
+        CUDA_TRY(h, RS::adj_vern7_dense(h->gen, t, p, h->adaptive ? &ag : nullptr, saved, st, &rows));
+    } else if (h->discrete_dense) {
         // discrete adjoint of the free-stepping Vern7 solve through its interpolated saves; the fused L2 reads the states the forward
-        // returned.  Adaptive, so never peer (refused above)
-        CUDA_TRY(h, launch_adj_vern7_dense_discrete(h->gen, h->tab, p, h->ag, h->last_out, st, &grid));
-        CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->var.discrete && h->kid == K_GENERIC) {
+        // returned
+        CUDA_TRY(h, RS::adj_vern7_dense_discrete(h->gen, t, p, ag, saved, st, &rows));
+    } else if (h->var.discrete && h->kid == K_FKPP) {
+        // discrete adjoint of an adaptive Vern7 Fisher-KPP solve (grid-per-CTA kernels)
+        CUDA_TRY(h, RS::adj_fkpp_vern7(h->gen, t, p, ag, st, &rows));
+    } else if (h->var.discrete && h->kid == K_GENERIC) {
         // discrete adjoint of a runtime-shape Tsit5 / Vern7 solve over its recorded steps; the fused L2 reads the recorded step-end states
-        CUDA_TRY(h, launch_adj_discrete(h->gen, h->tab, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &h->ag : nullptr, st, &grid));
-        if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
-        else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->var.discrete && h->kid == K_FKPP) {
-        // discrete adjoint of an adaptive Vern7 Fisher-KPP solve (grid-per-CTA kernels); adaptive, so never peer (refused above)
-        CUDA_TRY(h, launch_adj_fkpp_vern7(h->gen, h->tab, p, h->ag, st, &grid));
-        CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->adaptive) {
-        if (l2) {   // form the cotangent 2 w (out - data) from the interpolated saved states of the last forward
-            CUDA_TRY(h, launch_l2_cot(h->tab, h->last_out, cot, h->d_cot, h->d_block_loss, h->D, h->N, h->n_save, st));
-            p.cot = h->d_cot;
+        CUDA_TRY(h, RS::adj_discrete(h->gen, t, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &ag : nullptr, st, &rows));
+    } else {
+        if (h->adaptive && l2) {
+            // form the cotangent 2 w (out - data) from the interpolated saved states of the last forward: in fp32 in two stages (the
+            // loss follows the reduce), in fp64 in one CTA that writes the loss itself
+            if constexpr (is_f32<R>) {
+                CUDA_TRY(h, launch_l2_cot(h->tab, saved, cot, (float *)h->d_cot, h->d_block_loss, h->D, h->N, h->n_save, st));
+                finish_l2 = loss != nullptr;
+            } else {
+                CUDA_TRY(h, launch_l2_cot_f64(h->tab64, saved, cot, (double *)h->d_cot, loss, h->D, h->N, h->n_save, st));
+                reduce_loss = nullptr;
+            }
+            p.cot = (const R *)h->d_cot;
             p.fused_l2 = 0;
         }
-        if (h->kid == K_LV32) CUDA_TRY(h, launch_adj_lv32_adaptive(h->var, h->tab, p, h->ag, st, &grid));
-        else if (h->kid == K_SEIR64) CUDA_TRY(h, launch_adj_seir_adaptive(h->var, h->tab, p, h->ag, st, &grid));
-        else if (h->kid == K_FKPP) CUDA_TRY(h, launch_adj_fkpp_adaptive(h->gen, h->tab, p, h->ag, st, &grid));
-        else CUDA_TRY(h, launch_adj_adaptive(h->gen, h->tab, p, h->ag, st, &grid));
-        CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
-        if (l2 && loss) CUDA_TRY(h, launch_l2_finish(h->d_block_loss, loss, st));
-        return B200UDE_OK;
+        CUDA_TRY(h, launch_adjoint<R>(h, p, split_ok ? split : nullptr, split_at, st, &rows));
     }
-    if (h->desc.solver == B200UDE_RKC2) {
-        CUDA_TRY(h, launch_adj_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st, &grid));
-        if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
-        else CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    switch (h->kid) {
-    case K_LV32:
-        if (split_ok) {
-            int g0 = 0, g1 = 0;
-            AdjParams q = p;
-            q.n0 = 0; q.n_cnt = (int)split_at; q.row0 = 0;
-            CUDA_TRY(h, cudaStreamWaitEvent(st, split[0], 0));
-            e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g0);
-            if (e == cudaSuccess) {
-                q.n0 = (int)split_at; q.n_cnt = (int)(h->N - split_at); q.row0 = g0;
-                CUDA_TRY(h, cudaStreamWaitEvent(st, split[1], 0));
-                e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g1);
-            }
-            grid = g0 + g1;
-        } else {
-            e = (!h->var.discrete && use_wm(h->var.adj_wm, h->N, h->wm_adj_max)) ? launch_adj_lv32_wm(h->var, h->tab, p, st, &grid)
-                                                                                  : launch_adj_lv32(h->var, h->tab, p, st, &grid);
-        }
-        break;
-    case K_LV5P0: e = launch_adj_lv5(0, h->var, h->tab, p, st, &grid); break;
-    case K_LV5P1: e = launch_adj_lv5(1, h->var, h->tab, p, st, &grid); break;
-    case K_LV5P2: e = launch_adj_lv5(2, h->var, h->tab, p, st, &grid); break;
-    case K_GENERIC: e = launch_adj_generic(h->gen, h->tab, p, st, &grid); break;
-    case K_FKPP: e = launch_adj_fkpp(h->gen, h->tab, p, st, &grid); break;
-    case K_SEIR64: e = launch_adj_seir(h->var, h->tab, p, st, &grid); break;
-    case K_FKPP16: e = launch_adj_fkpp16(h->var, h->tab, p, h->D, st, &grid); break;
-    default: return fail(h, B200UDE_EUNSUPPORTED, "adjoint: no kernel");
-    }
-    CUDA_TRY(h, e);
-    if (peer) {
-        CUDA_TRY(h, launch_reduce_exchange(h->d_partial, grid, h->P + 1, h->peer, grad_theta, loss, st));
-    } else {
-        CUDA_TRY(h, launch_reduce(h->d_partial, grid, h->P + 1, grad_theta, loss, st));
+    const int32_t rc = reduce_partials(h, rows, grad_theta, reduce_loss, peer, st);
+    if (rc) return rc;
+    if constexpr (is_f32<R>) {
+        if (finish_l2) CUDA_TRY(h, launch_l2_finish(h->d_block_loss, loss, st));
     }
     return B200UDE_OK;
 }
-
 
 // ---- ADAM on the device (Flux.ADAM(eta, (beta1, beta2)), eps = 1e-8: scenario_1.jl:114, seir_exposure.jl:160) ----
 // One CTA: L = loss_scale * L_data + l2_reg * sum theta^2, g = loss_scale * grad + 2 l2_reg theta, then the
@@ -523,7 +602,7 @@ __global__ void __launch_bounds__(1024, 1) adam_kernel(AdamArgs a)
 
 int32_t ensure_adam(b200ude_handle *h)
 {
-    if (h->kid == K_F64) return fail(h, B200UDE_EUNSUPPORTED, "adam: not available for B200UDE_F64 handles (update theta on the host side)");
+    if (h->f64) return fail(h, B200UDE_EUNSUPPORTED, "adam: not available for B200UDE_F64 handles (update theta on the host side)");
     if (h->d_adam_m) return B200UDE_OK;
     bool ok = dalloc(h, &h->d_adam_m, (size_t)h->P) == cudaSuccess && dalloc(h, &h->d_adam_v, (size_t)h->P) == cudaSuccess &&
               dalloc(h, &h->d_adam_t, 1) == cudaSuccess;
@@ -549,123 +628,12 @@ int32_t check_adam(b200ude_handle *h, const b200ude_adam *o)
 cudaError_t launch_adam(b200ude_handle *h, const b200ude_adam *o, const float *grad, const float *loss, float *hist, int t_base, cudaStream_t st)
 {
     AdamArgs a;
-    a.theta = h->d_theta; a.m = h->d_adam_m; a.v = h->d_adam_v; a.grad = grad; a.loss = loss; a.loss_history = hist;
+    a.theta = (float *)h->d_theta; a.m = h->d_adam_m; a.v = h->d_adam_v; a.grad = grad; a.loss = loss; a.loss_history = hist;
     a.t = h->d_adam_t; a.P = h->P; a.t_base = t_base; a.reg_from = h->desc.n_prefix > 0 ? h->desc.n_prefix : 0;
     a.eta = (float)o->eta; a.beta1 = (float)o->beta1; a.beta2 = (float)o->beta2; a.eps = (float)o->eps;
     a.loss_scale = (float)(o->loss_scale == 0.0 ? 1.0 : o->loss_scale); a.l2_reg = (float)o->l2_reg;
     adam_kernel<<<1, 1024, 0, st>>>(a);
     return cudaGetLastError();
-}
-
-// ---- double-precision path (kid = K_F64) ----------------------------------------------------------------------------------
-Adapt64Host adapt64(const b200ude_handle *h)
-{
-    return Adapt64Host{h->desc.t0, h->desc.dt * h->desc.save_every, h->desc.abstol, h->desc.reltol, h->n_save, h->desc.max_steps, h->q_tgrid, h->d_nacc,
-                       h->q_hstep};
-}
-
-int32_t tsit5_forward64(b200ude_handle *h, const double *u0, size_t N, double *out, int32_t *status, cudaStream_t st)
-{
-    Fwd64Host p{u0, out, h->q_ustep, h->q_dense, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
-    const Adapt64Host a = adapt64(h);
-    if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_fwd_fkpp_f64(h->sh64, p, a, st));   // adaptive only (b200ude_create)
-    else CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 0, h->adaptive ? &a : nullptr, st));
-    h->q_last_out = out;
-    return B200UDE_OK;
-}
-
-int32_t do_forward64(b200ude_handle *h, const double *u0, size_t N, double *out, int32_t *status, cudaStream_t st)
-{
-    CUDA_TRY(h, cudaSetDevice(h->desc.device));
-    if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
-    if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
-    if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
-    if (h->forced) return do_forward_forced(h, u0, N, out, status, st);
-    if (h->op) return do_forward_operator(h, u0, N, out, status, st);
-    if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
-        // discrete adjoint / Vern7 dense output: u_n of every (accepted) step recorded (as in fp32)
-        Fwd64Host p{u0, out, h->q_ustep, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
-        const Adapt64Host a = adapt64(h);
-        if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_fwd_fkpp_vern7_f64(h->sh64, p, a, st));   // adaptive only (b200ude_create)
-        else if (h->adaptive && (h->vern7_dense || h->discrete_dense)) CUDA_TRY(h, launch_fwd_vern7_dense_f64(h->sh64, p, a, st));
-        else CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
-        h->q_last_out = out;
-        h->N = N;
-        h->have_forward = true;
-        return B200UDE_OK;
-    }
-    if (h->desc.solver == B200UDE_VERN7) {
-        // saved states only; the interpolating adjoint runs over a Tsit5 re-solve with the same step / tolerances (as in fp32)
-        Fwd64Host p{u0, out, nullptr, nullptr, status, (int)N, h->desc.n_steps, h->desc.save_every, h->desc.dt};
-        const Adapt64Host a = adapt64(h);
-        CUDA_TRY(h, launch_fwd_f64(h->sh64, p, 1, h->adaptive ? &a : nullptr, st));
-        if (!h->q_u0_keep && dalloc(h, &h->q_u0_keep, (size_t)h->D * h->cap) != cudaSuccess)
-            return fail(h, B200UDE_ENOMEM, "forward: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-        CUDA_TRY(h, cudaMemcpyAsync(h->q_u0_keep, u0, sizeof(double) * (size_t)h->D * N, cudaMemcpyDeviceToDevice, st));
-        h->N = N;
-        h->have_forward = false;
-        h->vern7_pending = true;
-        return B200UDE_OK;
-    }
-    int32_t rc = tsit5_forward64(h, u0, N, out, status, st);
-    if (rc) return rc;
-    h->N = N;
-    h->have_forward = true;
-    return B200UDE_OK;
-}
-
-int32_t do_adjoint64(b200ude_handle *h, bool l2, const double *cot, double *loss, double *grad_theta, double *grad_u0, cudaStream_t st)
-{
-    CUDA_TRY(h, cudaSetDevice(h->desc.device));
-    if (h->forced) return do_adjoint_forced(h, l2, cot, loss, grad_theta, grad_u0, st, false);
-    if (h->op) return do_adjoint_operator(h, l2, cot, loss, grad_theta, grad_u0, st, false);
-    if (h->desc.solver == B200UDE_VERN7 && h->vern7_pending) {
-        if (!h->q_aux_out && dalloc(h, &h->q_aux_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
-            return fail(h, B200UDE_ENOMEM, "adjoint: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-        int32_t rc = tsit5_forward64(h, h->q_u0_keep, h->N, h->q_aux_out, nullptr, st);
-        if (rc) return rc;
-        h->vern7_pending = false;
-        h->have_forward = true;
-    }
-    if (!h->have_forward) return fail(h, B200UDE_ESTATE, "adjoint: no stored forward solution (call b200ude_forward first)");
-    if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
-    Adj64Host p{h->q_ustep, h->q_dense, cot, grad_u0, h->q_partial, (int)h->N, h->desc.n_steps, h->desc.save_every, l2 ? 1 : 0, h->desc.dt};
-    int rows = 0;
-    if (h->vern7_dense) {   // interpolating adjoint over the Vern7 dense output; the fused L2 reads the states the forward returned
-        const Adapt64Host a = adapt64(h);
-        CUDA_TRY(h, launch_adj_vern7_dense_f64(h->sh64, p, h->adaptive ? &a : nullptr, h->q_last_out, st, &rows));
-        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->discrete_dense) {   // discrete adjoint through the interpolated saves; the fused L2 reads the states the forward returned
-        CUDA_TRY(h, launch_adj_vern7_dense_discrete_f64(h->sh64, p, adapt64(h), h->q_last_out, st, &rows));
-        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->var.discrete) {   // fixed-step Tsit5 / Vern7, adaptive Vern7 (b200ude_create); the fused L2 reads the recorded step-end states
-        const Adapt64Host a = adapt64(h);
-        if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_adj_fkpp_vern7_f64(h->sh64, p, a, st, &rows));
-        else CUDA_TRY(h, launch_adj_discrete_f64(h->sh64, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &a : nullptr, st, &rows));
-        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
-        return B200UDE_OK;
-    }
-    if (h->adaptive) {
-        const Adapt64Host a = adapt64(h);
-        double *loss_l2 = nullptr;
-        if (l2) {   // cotangent 2 w (out - data) from the interpolated saved states of the last Tsit5 forward; the loss goes straight to `loss`
-            CUDA_TRY(h, launch_l2_cot_f64(h->sh64, h->q_last_out, cot, h->q_cot, loss, h->N, h->n_save, st));
-            p.cot = h->q_cot;
-            p.fused_l2 = 0;
-            loss_l2 = loss;
-        }
-        if (h->desc.model == B200UDE_MODEL_FKPP) CUDA_TRY(h, launch_adj_fkpp_f64(h->sh64, p, a, st, &rows));
-        else CUDA_TRY(h, launch_adj_f64(h->sh64, p, &a, st, &rows));
-        CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss_l2 ? nullptr : loss, st));
-        return B200UDE_OK;
-    }
-    CUDA_TRY(h, launch_adj_f64(h->sh64, p, nullptr, st, &rows));
-    CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, grad_theta, loss, st));
-    return B200UDE_OK;
 }
 
 // ---- forced neural ODE with a readout network (B200UDE_MODEL_FORCED; k_forced.cu), both dtypes ------------------------------
@@ -706,13 +674,9 @@ int32_t forced_check(const b200ude_desc *d)
 
 ForcedRun forced_run(const b200ude_handle *h, size_t N)
 {
-    const bool f64 = h->fh.dtype == 1;
     ForcedRun r{};
     r.forcing = h->d_forcing;
-    r.ustep = f64 ? (void *)h->q_ustep : (void *)h->d_ustep;
-    r.dense = f64 ? (void *)h->q_dense : (void *)h->d_dense;
-    r.partial = f64 ? (void *)h->q_partial : (void *)h->d_partial;
-    r.tgrid = f64 ? (void *)h->q_tgrid : (void *)h->d_tgrid;
+    r.ustep = h->d_ustep; r.dense = h->d_dense; r.partial = h->d_partial; r.tgrid = h->d_tgrid;
     r.nacc = h->d_nacc;
     r.usave = h->d_usave;
     r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.adaptive = h->adaptive ? 1 : 0;
@@ -735,18 +699,12 @@ int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out
 }
 
 // fused L2: the loss 2 w (out - data) over all d + r rows, the readout rows recomputed from the saved states
-int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer)
+int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *grad_u0, cudaStream_t st, int *rows)
 {
-    if (!h->have_forward) return fail(h, B200UDE_ESTATE, "adjoint: no stored forward solution (call b200ude_forward first)");
-    if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
     if (h->N > h->forcing_n) return fail(h, B200UDE_ESTATE, "adjoint: the forcing was reset to fewer trajectories than the forward solved");
     ForcedRun r = forced_run(h, h->N);
     r.cot = cot; r.saved = h->d_usave; r.grad_u0 = grad_u0; r.fused_l2 = l2 ? 1 : 0;
-    int rows = 0;
-    CUDA_TRY(h, launch_adj_forced(h->fh, r, st, &rows));
-    if (h->fh.dtype == 1) CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, (double *)grad_theta, (double *)loss, st));
-    else if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, rows, h->P + 1, h->peer, (float *)grad_theta, (float *)loss, st));
-    else CUDA_TRY(h, launch_reduce(h->d_partial, rows, h->P + 1, (float *)grad_theta, (float *)loss, st));
+    CUDA_TRY(h, launch_adj_forced(h->fh, r, st, rows));
     return B200UDE_OK;
 }
 
@@ -783,12 +741,8 @@ int32_t operator_check(const b200ude_desc *d)
 
 OperatorRun operator_run(const b200ude_handle *h, size_t N)
 {
-    const bool f64 = h->oh.dtype == 1;
     OperatorRun r{};
-    r.ustep = f64 ? (void *)h->q_ustep : (void *)h->d_ustep;
-    r.dense = f64 ? (void *)h->q_dense : (void *)h->d_dense;
-    r.partial = f64 ? (void *)h->q_partial : (void *)h->d_partial;
-    r.tgrid = f64 ? (void *)h->q_tgrid : (void *)h->d_tgrid;
+    r.ustep = h->d_ustep; r.dense = h->d_dense; r.partial = h->d_partial; r.tgrid = h->d_tgrid;
     r.usave = h->d_usave;
     r.nacc = h->d_nacc;
     r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.n_save = h->n_save; r.max_steps = h->desc.max_steps;
@@ -808,152 +762,18 @@ int32_t do_forward_operator(b200ude_handle *h, const void *u0, size_t N, void *o
     return B200UDE_OK;
 }
 
-int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *loss, void *grad_theta, void *grad_u0, cudaStream_t st, bool peer)
+// the operators are set: a forward solution exists (do_adjoint)
+int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *grad_u0, cudaStream_t st, int *rows)
 {
-    if (!h->ops_set) return fail(h, B200UDE_ESTATE, "adjoint: B200UDE_MODEL_OPERATOR needs its operators (call b200ude_set_operators first)");
-    if (!h->have_forward) return fail(h, B200UDE_ESTATE, "adjoint: no stored forward solution (call b200ude_forward first)");
-    if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
     OperatorRun r = operator_run(h, h->N);
     r.cot = cot; r.grad_u0 = grad_u0; r.fused_l2 = l2 ? 1 : 0;
-    int rows = 0;
-    CUDA_TRY(h, launch_adj_operator(h->oh, r, st, &rows));
-    if (h->oh.dtype == 1) CUDA_TRY(h, launch_reduce_f64(h->q_partial, rows, h->P + 1, (double *)grad_theta, (double *)loss, st));
-    else if (peer) CUDA_TRY(h, launch_reduce_exchange(h->d_partial, rows, h->P + 1, h->peer, (float *)grad_theta, (float *)loss, st));
-    else CUDA_TRY(h, launch_reduce(h->d_partial, rows, h->P + 1, (float *)grad_theta, (float *)loss, st));
+    CUDA_TRY(h, launch_adj_operator(h->oh, r, st, rows));
     return B200UDE_OK;
 }
 
-// create for B200UDE_MODEL_OPERATOR (the descriptor is validated before the device check, so that it is testable without a GPU)
-int32_t create_operator(const b200ude_desc *d, b200ude_handle **out)
+// the descriptor checks of every model but the operator UDE (operator_check), and the kernel family that runs the descriptor
+int32_t select_kernel(const b200ude_desc *d, KernelId *kid_out)
 {
-    int32_t rc = operator_check(d);
-    if (rc) return rc;
-    const bool want64 = d->dtype == B200UDE_F64;
-    OperatorHost oh{};
-    oh.dtype = want64 ? 1 : 0; oh.D = d->state_dim; oh.M = d->widths[d->n_layers]; oh.L = d->n_layers;
-    for (int l = 0; l < 6; ++l) oh.widths[l] = l <= d->n_layers ? d->widths[l] : 0;
-    for (int l = 0; l < 5; ++l) oh.acts[l] = l < d->n_layers ? d->acts[l] : 0;
-    oh.rkc2 = d->solver == B200UDE_RKC2 ? 1 : 0;
-    oh.S = oh.rkc2 ? d->n_stages : 0;
-    operator_layout(oh);
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) return fail(nullptr, B200UDE_ENODEVICE, "create: no CUDA device (%s)", cudaGetErrorString(e));
-    if (d->device < 0 || d->device >= ndev) return fail(nullptr, B200UDE_EINVAL, "create: device %d of %d", d->device, ndev);
-    cudaDeviceProp prop;
-    e = cudaGetDeviceProperties(&prop, d->device);
-    if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 9 || prop.minor != 0)
-        return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_90a code only", d->device, prop.major, prop.minor);
-    e = cudaSetDevice(d->device);
-    if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaSetDevice: %s", cudaGetErrorString(e));
-    // four warps (trajectories) per CTA, fewer when their gradient vectors do not fit next to the kernels' static shared memory
-    size_t stat = 0;
-    e = operator_static_smem(oh.dtype, &stat);
-    if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaFuncGetAttributes: %s", cudaGetErrorString(e));
-    oh.dyn_cap = (int)(prop.sharedMemPerBlockOptin - stat);
-    oh.warps = 4;
-    while (oh.warps > 0 && operator_smem(oh, oh.warps) > (size_t)oh.dyn_cap) --oh.warps;
-    if (oh.warps == 0)
-        return fail(nullptr, B200UDE_EUNSUPPORTED,
-                    "create: B200UDE_MODEL_OPERATOR with d = %d, m = %d and %d parameters needs %zu B of shared memory for one warp "
-                    "(%zu B dynamic + %zu B static; device limit %zu B)",
-                    oh.D, oh.M, oh.P, operator_smem(oh, 1) + stat, operator_smem(oh, 1), stat, (size_t)prop.sharedMemPerBlockOptin);
-    b200ude_handle *h = new (std::nothrow) b200ude_handle();
-    if (!h) return fail(nullptr, B200UDE_ENOMEM, "create: out of host memory");
-    h->desc = *d;
-    h->kid = want64 ? K_F64 : K_OPERATOR;
-    h->op = true;
-    h->D = h->DR = d->state_dim;
-    h->n_save = d->n_steps / d->save_every + 1;
-    h->cap = (size_t)d->max_trajectories;
-    h->sm_count = prop.multiProcessorCount;
-    h->adaptive = d->adaptive != 0;
-    h->P = oh.P;
-    const size_t N = h->cap, D = (size_t)h->D, P = (size_t)oh.P, es = want64 ? sizeof(double) : sizeof(float);
-    const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
-    const size_t dense_rows = oh.rkc2 ? rec + 1 : rec * 6 + 1;   // RKC2: f(u_n); Tsit5: the stages
-    h->partial_blocks = (size_t)adj_rows_operator((int)N, oh.warps);
-    bool ok = true;
-    if (want64) {
-        ok = dalloc(h, &h->q_theta, P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D * N) == cudaSuccess &&
-             dalloc(h, &h->q_dense, dense_rows * D * N) == cudaSuccess && dalloc(h, &h->q_partial, h->partial_blocks * (P + 1)) == cudaSuccess;
-        if (h->adaptive) ok = ok && dalloc(h, &h->q_tgrid, (rec + 1) * N) == cudaSuccess;
-        oh.theta = h->q_theta;
-    } else {
-        ok = dalloc(h, &h->d_theta, P + 1) == cudaSuccess && dalloc(h, &h->d_ustep, (rec + 1) * D * N) == cudaSuccess &&
-             dalloc(h, &h->d_dense, dense_rows * D * N) == cudaSuccess && dalloc(h, &h->d_partial, h->partial_blocks * (P + 1)) == cudaSuccess &&
-             dalloc(h, &h->d_grad, P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
-        if (h->adaptive) ok = ok && dalloc(h, &h->d_tgrid, (rec + 1) * N) == cudaSuccess;
-        oh.theta = h->d_theta;
-    }
-    if (h->adaptive)
-        ok = ok && dalloc(h, &h->d_nacc, N) == cudaSuccess && dalloc(h, (unsigned char **)&h->d_usave, es * (size_t)h->n_save * D * N) == cudaSuccess;
-    ok = ok && dalloc(h, (unsigned char **)&h->d_ops, es * (size_t)oh.ops_elems) == cudaSuccess;
-    if (oh.rkc2) ok = ok && dalloc(h, (unsigned char **)&h->d_rkc, es * (size_t)op_rkc_len()) == cudaSuccess;
-    if (ok) {
-        // the loss weights in front of the operator block; the operators follow in b200ude_set_operators
-        std::vector<double> w64(oh.ops_elems, 0.0);
-        for (int c = 0; c < 64; ++c) w64[c] = c < oh.D ? (d->n_loss_weights > 0 ? d->loss_weights[c] : 1.0) : 0.0;
-        ok = upload_as(h->d_ops, w64.data(), w64.size(), want64) == cudaSuccess &&
-             cudaMemset(want64 ? (void *)h->q_theta : (void *)h->d_theta, 0, es * (P + 1)) == cudaSuccess;
-        if (ok && oh.rkc2) {
-            std::vector<double> t(op_rkc_len(), 0.0);
-            rkc2_tables64(oh.S, t[0], &t[op_rkc_off(2)], &t[op_rkc_off(3)], &t[op_rkc_off(4)], &t[op_rkc_off(5)], &t[op_rkc_off(0)], &t[op_rkc_off(1)]);
-            ok = upload_as(h->d_rkc, t.data(), t.size(), want64) == cudaSuccess;
-        }
-    }
-    if (!ok) {
-        g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
-        b200ude_destroy(h);
-        return B200UDE_ENOMEM;
-    }
-    oh.ops = h->d_ops;
-    oh.rkc = h->d_rkc;
-    h->oh = oh;
-    if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->data_ready, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->data_ready2, cudaEventDisableTiming) != cudaSuccess ||
-        (!want64 && cudaMallocHost((void **)&h->h_loss, sizeof(float)) != cudaSuccess)) {
-        g_create_error = "create: stream / pinned allocation failed";
-        b200ude_destroy(h);
-        return B200UDE_ENOMEM;
-    }
-    *out = h;
-    return B200UDE_OK;
-}
-
-int32_t f64_unsupported(b200ude_handle *h, const char *what)
-{
-    return fail(h, B200UDE_EUNSUPPORTED, "%s: not available for B200UDE_F64 handles (device-pointer forward / adjoint entry points only)", what);
-}
-
-}  // namespace
-
-// ---- exported entry points ------------------------------------------------------------------------
-extern "C" {
-
-int32_t b200ude_version(void) { return B200UDE_ABI_VERSION; }
-
-const char *b200ude_last_error(const b200ude_handle *h) { return h ? h->err.c_str() : g_create_error.c_str(); }
-
-int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
-{
-    if (!d || !out) return fail(nullptr, B200UDE_EINVAL, "create: null argument");
-    *out = nullptr;
-    if (d->struct_size != sizeof(b200ude_desc))
-        return fail(nullptr, B200UDE_EINVAL, "create: struct_size %u != %zu (ABI mismatch)", d->struct_size, sizeof(b200ude_desc));
-    if (d->dtype != B200UDE_F32 && d->dtype != B200UDE_F64) return fail(nullptr, B200UDE_EINVAL, "create: unknown dtype %d", d->dtype);
-    if (d->n_layers < 1 || d->n_layers > B200UDE_MAX_LAYERS) return fail(nullptr, B200UDE_EINVAL, "create: n_layers=%d out of range", d->n_layers);
-    if (d->solver != B200UDE_TSIT5 && d->solver != B200UDE_VERN7 && d->solver != B200UDE_RKC2)
-        return fail(nullptr, B200UDE_EINVAL, "create: unknown solver %d", d->solver);
-    if (d->sensealg != B200UDE_INTERPOLATING_ADJOINT && d->sensealg != B200UDE_DISCRETE_ADJOINT)
-        return fail(nullptr, B200UDE_EUNSUPPORTED, "create: unknown sensealg %d", d->sensealg);
-    if (!(d->dt > 0) || d->n_steps < 1 || d->save_every < 1 || d->n_steps % d->save_every != 0)
-        return fail(nullptr, B200UDE_EINVAL, "create: need dt>0, n_steps>=1, save_every>=1 dividing n_steps");
-    if (d->max_trajectories == 0 || d->max_trajectories > (1ull << 26)) return fail(nullptr, B200UDE_EINVAL, "create: max_trajectories out of range");
-    if (d->model == B200UDE_MODEL_OPERATOR) return create_operator(d, out);
     const bool forced = d->model == B200UDE_MODEL_FORCED;
     if (forced) {
         const int32_t rc = forced_check(d);
@@ -1001,7 +821,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                         "only; fixed-step Fisher-KPP is fp32");
         if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1))
             return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
-        kid = K_F64;
+        kid = d->model == B200UDE_MODEL_FKPP ? K_FKPP : K_GENERIC;
     }
     if (!want64 && d->solver == B200UDE_VERN7) {
         if (!generic_ok(*d) || (d->model == B200UDE_MODEL_FKPP && !(fkpp_v7 && disc)))
@@ -1038,115 +858,134 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     // fixed-step Tsit5 with the discrete adjoint: LV 2-32-32-2 / 2-5-5-5-2 keep their tuned kernels, every other form runs on the
     // runtime-shape ones (the SEIR tensor-core kernels have no discrete adjoint)
     if (disc && !want64 && kid != K_NONE && !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2 || kid == K_FKPP)) kid = K_GENERIC;
-    if (forced) kid = want64 ? K_F64 : K_FORCED;
+    if (forced) kid = K_FORCED;
     if (kid == K_NONE)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: no sm_90a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");
+    *kid_out = kid;
+    return B200UDE_OK;
+}
+
+int32_t probe_device(const b200ude_desc *d, cudaDeviceProp *prop)
+{
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0) return fail(nullptr, B200UDE_ENODEVICE, "create: no CUDA device (%s)", cudaGetErrorString(e));
     if (d->device < 0 || d->device >= ndev) return fail(nullptr, B200UDE_EINVAL, "create: device %d of %d", d->device, ndev);
-    cudaDeviceProp prop;
-    e = cudaGetDeviceProperties(&prop, d->device);
+    e = cudaGetDeviceProperties(prop, d->device);
     if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 9 || prop.minor != 0)
-        return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_90a code only", d->device, prop.major, prop.minor);
+    if (prop->major != 9 || prop->minor != 0)
+        return fail(nullptr, B200UDE_ENODEVICE, "create: device %d is sm_%d%d; this library carries sm_90a code only", d->device, prop->major, prop->minor);
+    return B200UDE_OK;
+}
+
+// partial gradient rows of the handle's adjoint kernels at max_trajectories
+size_t partial_rows(const b200ude_handle *h)
+{
+    const int N = (int)h->cap;
+    switch (h->kid) {
+    case K_OPERATOR: return (size_t)adj_rows_operator(N, h->oh.warps);
+    case K_FORCED: return (size_t)adj_rows_forced(N, h->f64 ? 1 : 0);
+    case K_GENERIC: return (size_t)(h->f64 ? RuntimeShape<double>::adj_rows(N) : RuntimeShape<float>::adj_rows(N));
+    case K_FKPP: return (size_t)adj_rows_fkpp(N, h->D);
+    case K_LV32: return (size_t)std::max(adj_grid_lv32(N), adj_rows_lv32_wm(N));
+    case K_SEIR64: return (size_t)adj_rows_seir(N);
+    case K_FKPP16: return (size_t)adj_rows_fkpp16(N, h->D);
+    default: return (size_t)adj_grid_lv5(N);
+    }
+}
+
+int32_t f64_unsupported(b200ude_handle *h, const char *what)
+{
+    return fail(h, B200UDE_EUNSUPPORTED, "%s: not available for B200UDE_F64 handles (device-pointer forward / adjoint entry points only)", what);
+}
+
+}  // namespace
+
+// ---- exported entry points ------------------------------------------------------------------------
+extern "C" {
+
+int32_t b200ude_version(void) { return B200UDE_ABI_VERSION; }
+
+const char *b200ude_last_error(const b200ude_handle *h) { return h ? h->err.c_str() : g_create_error.c_str(); }
+
+int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
+{
+    if (!d || !out) return fail(nullptr, B200UDE_EINVAL, "create: null argument");
+    *out = nullptr;
+    if (d->struct_size != sizeof(b200ude_desc))
+        return fail(nullptr, B200UDE_EINVAL, "create: struct_size %u != %zu (ABI mismatch)", d->struct_size, sizeof(b200ude_desc));
+    if (d->dtype != B200UDE_F32 && d->dtype != B200UDE_F64) return fail(nullptr, B200UDE_EINVAL, "create: unknown dtype %d", d->dtype);
+    if (d->n_layers < 1 || d->n_layers > B200UDE_MAX_LAYERS) return fail(nullptr, B200UDE_EINVAL, "create: n_layers=%d out of range", d->n_layers);
+    if (d->solver != B200UDE_TSIT5 && d->solver != B200UDE_VERN7 && d->solver != B200UDE_RKC2)
+        return fail(nullptr, B200UDE_EINVAL, "create: unknown solver %d", d->solver);
+    if (d->sensealg != B200UDE_INTERPOLATING_ADJOINT && d->sensealg != B200UDE_DISCRETE_ADJOINT)
+        return fail(nullptr, B200UDE_EUNSUPPORTED, "create: unknown sensealg %d", d->sensealg);
+    if (!(d->dt > 0) || d->n_steps < 1 || d->save_every < 1 || d->n_steps % d->save_every != 0)
+        return fail(nullptr, B200UDE_EINVAL, "create: need dt>0, n_steps>=1, save_every>=1 dividing n_steps");
+    if (d->max_trajectories == 0 || d->max_trajectories > (1ull << 26)) return fail(nullptr, B200UDE_EINVAL, "create: max_trajectories out of range");
+    const bool op = d->model == B200UDE_MODEL_OPERATOR, forced = d->model == B200UDE_MODEL_FORCED, want64 = d->dtype == B200UDE_F64;
+    // the descriptor is validated before the device check, so that it is testable without a GPU
+    KernelId kid = K_OPERATOR;
+    int32_t rc = op ? operator_check(d) : select_kernel(d, &kid);
+    if (rc) return rc;
+    OperatorHost oh{};
+    if (op) {
+        oh.dtype = want64 ? 1 : 0; oh.D = d->state_dim; oh.M = d->widths[d->n_layers]; oh.L = d->n_layers;
+        for (int l = 0; l < 6; ++l) oh.widths[l] = l <= d->n_layers ? d->widths[l] : 0;
+        for (int l = 0; l < 5; ++l) oh.acts[l] = l < d->n_layers ? d->acts[l] : 0;
+        oh.rkc2 = d->solver == B200UDE_RKC2 ? 1 : 0;
+        oh.S = oh.rkc2 ? d->n_stages : 0;
+        operator_layout(oh);
+    }
+    cudaDeviceProp prop;
+    rc = probe_device(d, &prop);
+    if (rc) return rc;
+    const int P = op ? oh.P : num_params(d, kid);
     if (d->model == B200UDE_MODEL_FKPP && d->adaptive) {
         // the adjoint keeps one gradient vector (P + 1 entries) per warp in shared memory: refuse here what could not launch
-        int P = d->n_prefix + d->n_suffix;
-        for (int l = 0; l < d->n_layers; ++l) P += d->widths[l] * d->widths[l + 1] + d->widths[l + 1];
         const size_t smem = fkpp_adaptive_smem(d->state_dim, P, want64 ? (int)sizeof(double) : (int)sizeof(float)) + 16;   // + static
         if (smem > prop.sharedMemPerBlockOptin)
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: adaptive Fisher-KPP with %d grid points and %d parameters needs %zu B of shared memory per CTA (device limit %zu B)",
                         d->state_dim, P, smem, (size_t)prop.sharedMemPerBlockOptin);
     }
-    e = cudaSetDevice(d->device);
+    cudaError_t e = cudaSetDevice(d->device);
     if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaSetDevice: %s", cudaGetErrorString(e));
+    if (op) {
+        // four warps (trajectories) per CTA, fewer when their gradient vectors do not fit next to the kernels' static shared memory
+        size_t stat = 0;
+        e = operator_static_smem(oh.dtype, &stat);
+        if (e != cudaSuccess) return fail(nullptr, (int32_t)e, "create: cudaFuncGetAttributes: %s", cudaGetErrorString(e));
+        oh.dyn_cap = (int)(prop.sharedMemPerBlockOptin - stat);
+        oh.warps = 4;
+        while (oh.warps > 0 && operator_smem(oh, oh.warps) > (size_t)oh.dyn_cap) --oh.warps;
+        if (oh.warps == 0)
+            return fail(nullptr, B200UDE_EUNSUPPORTED,
+                        "create: B200UDE_MODEL_OPERATOR with d = %d, m = %d and %d parameters needs %zu B of shared memory for one warp "
+                        "(%zu B dynamic + %zu B static; device limit %zu B)",
+                        oh.D, oh.M, oh.P, operator_smem(oh, 1) + stat, operator_smem(oh, 1), stat, (size_t)prop.sharedMemPerBlockOptin);
+    }
+    if (!want64 && (kid == K_GENERIC || kid == K_FKPP || kid == K_FORCED) && P > 12288)
+        return fail(nullptr, B200UDE_EUNSUPPORTED, "create: %d parameters exceed the constant-bank budget", P);
 
     b200ude_handle *h = new (std::nothrow) b200ude_handle();
     if (!h) return fail(nullptr, B200UDE_ENOMEM, "create: out of host memory");
-    const uint64_t serial = ++g_serial;   // taken once: gen.serial and tab.serial must agree
+    const uint64_t serial = ++g_serial;   // taken once: the shape and the tables must agree
     h->desc = *d;
     h->kid = kid;
-    h->D = d->state_dim;
-    h->DR = d->state_dim;
+    h->f64 = want64;
+    h->D = h->DR = d->state_dim;
     h->n_save = d->n_steps / d->save_every + 1;
     h->cap = (size_t)d->max_trajectories;
     h->sm_count = prop.multiProcessorCount;
     h->adaptive = d->adaptive != 0;
-    h->P = kernel_num_params(kid);
-    if (kid == K_GENERIC || kid == K_FKPP || kid == K_F64) {
-        int P = d->n_prefix + d->n_suffix;
-        for (int l = 0; l < d->n_layers; ++l) P += d->widths[l] * d->widths[l + 1] + d->widths[l + 1];
-        h->P = P;
-        h->gen.serial = serial;   // same serial as the tables set below
-        h->gen.model = d->model; h->gen.D = d->state_dim; h->gen.din = d->widths[0]; h->gen.dout = d->widths[d->n_layers];
-        h->gen.n_layers = d->n_layers; h->gen.n_prefix = d->n_prefix; h->gen.P = P;
-        for (int l = 0; l < 8; ++l) { h->gen.widths[l] = l <= d->n_layers ? d->widths[l] : 0; h->gen.acts[l] = l < d->n_layers ? d->acts[l] : 0; }
-        if (kid != K_F64 && P > 12288) { delete h; return fail(nullptr, B200UDE_EUNSUPPORTED, "create: %d parameters exceed the constant-bank budget", P); }
-    }
-    if (forced) {
-        // both chains back to back; P as the layer list says
-        const int L0 = (int)d->consts[0], L1 = d->n_layers - L0;
-        int P = 0;
-        for (int l = 0; l < L0 + L1; ++l) {
-            const int a = l < L0 ? l : l + 1;
-            P += d->widths[a] * d->widths[a + 1] + d->widths[a + 1];
-        }
-        if (!want64 && P > 12288) { delete h; return fail(nullptr, B200UDE_EUNSUPPORTED, "create: %d parameters exceed the constant-bank budget", P); }
-        h->P = P;
-        h->forced = true;
-        h->DR = d->state_dim + d->widths[L0];
-        ForcedHost &f = h->fh;
-        f.serial = serial; f.dtype = want64 ? 1 : 0; f.D = d->state_dim; f.R = d->widths[L0]; f.J = (int)d->consts[1]; f.L0 = L0; f.L1 = L1; f.P = P;
-        for (int l = 0; l < 8; ++l) {
-            f.widths[l] = l <= d->n_layers + 1 ? d->widths[l] : 0;
-            f.acts[l] = l < d->n_layers ? d->acts[l] : 0;
-        }
-        for (int i = 0; i < 16; ++i) f.lossw[i] = d->n_loss_weights > 0 ? (i < d->n_loss_weights ? d->loss_weights[i] : 0.0) : 1.0;
-        const size_t N = h->cap, D = (size_t)h->D, es = want64 ? sizeof(double) : sizeof(float);
-        const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
-        h->partial_blocks = (size_t)adj_rows_forced((int)N, f.dtype);
-        bool ok = true;
-        if (want64) {
-            ok = dalloc(h, &h->q_theta, (size_t)P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D * N) == cudaSuccess &&
-                 dalloc(h, &h->q_dense, (rec * 6 + 1) * D * N) == cudaSuccess && dalloc(h, &h->q_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess;
-            if (h->adaptive) ok = ok && dalloc(h, &h->q_tgrid, (rec + 1) * N) == cudaSuccess;
-            f.theta = h->q_theta;
-        } else {
-            ok = dalloc(h, &h->d_theta, (size_t)P + 1) == cudaSuccess && dalloc(h, &h->d_ustep, (rec + 1) * D * N) == cudaSuccess &&
-                 dalloc(h, &h->d_dense, (rec * 6 + 1) * D * N) == cudaSuccess && dalloc(h, &h->d_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess &&
-                 dalloc(h, &h->d_grad, (size_t)P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
-            if (h->adaptive) ok = ok && dalloc(h, &h->d_tgrid, (rec + 1) * N) == cudaSuccess;
-            f.theta = h->d_theta;
-        }
-        if (h->adaptive)
-            ok = ok && dalloc(h, &h->d_nacc, N) == cudaSuccess &&
-                 dalloc(h, (unsigned char **)&h->d_usave, es * (size_t)h->n_save * D * N) == cudaSuccess;
-        ok = ok && dalloc(h, (unsigned char **)&h->d_forcing, es * 3 * (size_t)f.J * N) == cudaSuccess;
-        if (ok) ok = cudaMemset(want64 ? (void *)h->q_theta : (void *)h->d_theta, 0, es * ((size_t)P + 1)) == cudaSuccess;
-        if (!ok) {
-            g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
-            b200ude_destroy(h);
-            return B200UDE_ENOMEM;
-        }
-        if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&h->data_ready, cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&h->data_ready2, cudaEventDisableTiming) != cudaSuccess ||
-            (!want64 && cudaMallocHost((void **)&h->h_loss, sizeof(float)) != cudaSuccess)) {
-            g_create_error = "create: stream / pinned allocation failed";
-            b200ude_destroy(h);
-            return B200UDE_ENOMEM;
-        }
-        *out = h;
-        return B200UDE_OK;
-    }
+    h->P = P;
+    h->oh = oh;
     h->var.approx_tanh = (d->flags & B200UDE_FLAG_APPROX_TANH) ? 1 : 0;
     h->var.discrete = d->sensealg == B200UDE_DISCRETE_ADJOINT ? 1 : 0;
-    h->vern7_dense = v7dense;
-    h->discrete_dense = disc_dense && d->adaptive;
+    h->vern7_dense = (d->flags & B200UDE_FLAG_VERN7_DENSE) != 0;
+    h->discrete_dense = (d->flags & B200UDE_FLAG_DISCRETE_DENSE) && d->adaptive;
     if (d->solver == B200UDE_RKC2) rkc2_tables(d->n_stages, &h->rkc);
     // tuning knobs for experiments (defaults are the measured-best variant, see DESIGN.md)
     h->var.fwd_smem = env_int("B200UDE_FWD_SMEM", 0);
@@ -1163,86 +1002,89 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     h->wm_fwd_max = (size_t)env_int("B200UDE_WM_FWD_MAX", 1 << 26);
     h->wm_adj_max = (size_t)env_int("B200UDE_WM_ADJ_MAX", 1 << 26);
 
-    if (kid == K_F64) {
-        const size_t N64 = h->cap, D64 = (size_t)h->D;
-        const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;
-        h->partial_blocks = (size_t)(d->model == B200UDE_MODEL_FKPP ? adj_rows_fkpp((int)N64, d->state_dim) : adj_rows_f64((int)N64));
-        // a discrete-adjoint or dense-output Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead
-        // when adaptive
-        const bool disc_vern7 = (disc && d->solver == B200UDE_VERN7) || v7dense;
-        bool ok64 = dalloc(h, &h->q_theta, (size_t)h->P + 1) == cudaSuccess && dalloc(h, &h->q_ustep, (rec + 1) * D64 * N64) == cudaSuccess &&
-                    (disc_vern7 || dalloc(h, &h->q_dense, (rec * 6 + 1) * D64 * N64) == cudaSuccess) &&
-                    dalloc(h, &h->q_partial, h->partial_blocks * (size_t)(h->P + 1)) == cudaSuccess;
-        if (h->adaptive)
-            ok64 = ok64 && dalloc(h, &h->q_tgrid, (rec + 1) * N64) == cudaSuccess && dalloc(h, &h->d_nacc, N64) == cudaSuccess &&
-                   dalloc(h, &h->q_cot, (size_t)h->n_save * D64 * N64) == cudaSuccess &&
-                   (!disc_vern7 || dalloc(h, &h->q_hstep, rec * N64) == cudaSuccess);
-        if (!ok64) {
-            g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
-            b200ude_destroy(h);
-            return B200UDE_ENOMEM;
-        }
-        cudaMemset(h->q_theta, 0, sizeof(double) * ((size_t)h->P + 1));
-        Shape64Host &sh = h->sh64;
-        sh.serial = serial; sh.model = d->model; sh.D = d->state_dim; sh.din = d->widths[0]; sh.dout = d->widths[d->n_layers];
-        sh.n_layers = d->n_layers; sh.n_prefix = d->n_prefix; sh.P = h->P; sh.theta = h->q_theta;
-        for (int l = 0; l < 8; ++l) { sh.widths[l] = l <= d->n_layers ? d->widths[l] : 0; sh.acts[l] = l < d->n_layers ? d->acts[l] : 0; }
-        for (int i = 0; i < 16; ++i) {
-            sh.consts[i] = i < d->n_consts ? d->consts[i] : 0.0;
-            sh.lossw[i] = d->n_loss_weights > 0 ? (i < d->n_loss_weights ? d->loss_weights[i] : 0.0) : 1.0;
-        }
-        if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess) {
-            g_create_error = "create: stream allocation failed";
-            b200ude_destroy(h);
-            return B200UDE_ENOMEM;
-        }
-        *out = h;
-        return B200UDE_OK;
-    }
-    const size_t N = h->cap, D = (size_t)h->D;
-    h->partial_blocks = (size_t)(kid == K_LV32 ? std::max(adj_grid_lv32((int)N), adj_rows_lv32_wm((int)N)) : kid == K_GENERIC ? adj_rows_generic((int)N) : kid == K_FKPP ? adj_rows_fkpp((int)N, d->state_dim) : kid == K_SEIR64 ? adj_rows_seir((int)N) : kid == K_FKPP16 ? adj_rows_fkpp16((int)N, d->state_dim) : adj_grid_lv5((int)N));
-    bool ok = true;
-    ok = ok && dalloc(h, &h->d_theta, (size_t)((h->P + 3) / 4) * 4) == cudaSuccess;
-    const size_t rec_steps = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;   // capacity of the step record
-    ok = ok && dalloc(h, &h->d_ustep, (rec_steps + 1) * D * N) == cudaSuccess;
-    const bool disc_vern7 = (disc && d->solver == B200UDE_VERN7) || v7dense;   // stages recomputed from u_n: no dense record
-    if (!disc_vern7) ok = ok && dalloc(h, &h->d_dense, (rec_steps * 6 + 1) * D * N) == cudaSuccess;
+    const size_t N = h->cap, D = (size_t)h->D, es = h->es();
+    const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;   // capacity of the step record
+    // a discrete-adjoint or dense-output Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead when adaptive
+    const bool disc_vern7 = (h->var.discrete && d->solver == B200UDE_VERN7) || h->vern7_dense;
+    const size_t dense_rows = oh.rkc2 ? rec + 1 : rec * 6 + 1;   // operator RKC2: f(u_n); Tsit5: the stages
+    // theta: the fp32 runtime-shape and tuned kernels read it as float4
+    const size_t theta_n = want64 || forced || op ? (size_t)P + 1 : (size_t)((P + 3) / 4) * 4;
+    h->partial_blocks = partial_rows(h);
+    bool ok = dalloc_real(h, &h->d_theta, theta_n) == cudaSuccess && dalloc_real(h, &h->d_ustep, (rec + 1) * D * N) == cudaSuccess &&
+              (disc_vern7 || dalloc_real(h, &h->d_dense, dense_rows * D * N) == cudaSuccess) &&
+              dalloc_real(h, &h->d_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess;
+    if (!want64) ok = ok && dalloc(h, &h->d_grad, (size_t)P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
     if (h->adaptive) {
-        if (disc_vern7) ok = ok && dalloc(h, &h->d_hstep, rec_steps * N) == cudaSuccess;
-        ok = ok && dalloc(h, &h->d_tgrid, (rec_steps + 1) * N) == cudaSuccess;
-        ok = ok && dalloc(h, &h->d_nacc, N) == cudaSuccess;
-        ok = ok && dalloc(h, &h->d_cot, (size_t)h->n_save * D * N) == cudaSuccess;
-        ok = ok && dalloc(h, &h->d_block_loss, (size_t)L2_BLOCKS) == cudaSuccess;
+        ok = ok && dalloc_real(h, &h->d_tgrid, (rec + 1) * N) == cudaSuccess && dalloc(h, &h->d_nacc, N) == cudaSuccess;
+        if (forced || op)   // the saved states of the last forward, read by the replay adjoint
+            ok = ok && dalloc_real(h, &h->d_usave, (size_t)h->n_save * D * N) == cudaSuccess;
+        else   // the cotangent of the fused L2 and, in fp32, its per-block losses
+            ok = ok && dalloc_real(h, &h->d_cot, (size_t)h->n_save * D * N) == cudaSuccess &&
+                 (!disc_vern7 || dalloc_real(h, &h->d_hstep, rec * N) == cudaSuccess) &&
+                 (want64 || dalloc(h, &h->d_block_loss, (size_t)L2_BLOCKS) == cudaSuccess);
     }
-    ok = ok && dalloc(h, &h->d_partial, h->partial_blocks * (size_t)(h->P + 1)) == cudaSuccess;
-    ok = ok && dalloc(h, &h->d_grad, (size_t)h->P) == cudaSuccess;
-    ok = ok && dalloc(h, &h->d_loss, 1) == cudaSuccess;
+    if (forced) ok = ok && dalloc_real(h, &h->d_forcing, 3 * (size_t)d->consts[1] * N) == cudaSuccess;
+    if (op) ok = ok && dalloc_real(h, &h->d_ops, (size_t)oh.ops_elems) == cudaSuccess && (!oh.rkc2 || dalloc_real(h, &h->d_rkc, op_rkc_len()) == cudaSuccess);
+    if (ok) ok = cudaMemset(h->d_theta, 0, es * theta_n) == cudaSuccess;
+    if (ok && op) {
+        // the loss weights in front of the operator block; the operators follow in b200ude_set_operators
+        std::vector<double> w64(oh.ops_elems, 0.0);
+        for (int c = 0; c < 64; ++c) w64[c] = c < oh.D ? (d->n_loss_weights > 0 ? d->loss_weights[c] : 1.0) : 0.0;
+        ok = upload_as(h->d_ops, w64.data(), w64.size(), want64) == cudaSuccess;
+        if (ok && oh.rkc2) {
+            std::vector<double> t(op_rkc_len(), 0.0);
+            rkc2_tables64(oh.S, t[0], &t[op_rkc_off(2)], &t[op_rkc_off(3)], &t[op_rkc_off(4)], &t[op_rkc_off(5)], &t[op_rkc_off(0)], &t[op_rkc_off(1)]);
+            ok = upload_as(h->d_rkc, t.data(), t.size(), want64) == cudaSuccess;
+        }
+    }
     if (!ok) {
-        cudaError_t le = cudaGetLastError();
-        g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(le);
+        g_create_error = std::string("create: device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
         b200ude_destroy(h);
         return B200UDE_ENOMEM;
     }
-    cudaMemset(h->d_theta, 0, sizeof(float) * ((h->P + 3) / 4) * 4);
     if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->data_ready, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&h->data_ready2, cudaEventDisableTiming) != cudaSuccess ||
-        cudaMallocHost((void **)&h->h_loss, sizeof(float)) != cudaSuccess) {
+        (!want64 && cudaMallocHost((void **)&h->h_loss, sizeof(float)) != cudaSuccess)) {
         g_create_error = "create: stream / pinned allocation failed";
         b200ude_destroy(h);
         return B200UDE_ENOMEM;
     }
+
+    // the shape and tables the kernels read
+    GenericShape &g = h->gen;
+    g.serial = serial;
+    g.model = d->model; g.D = d->state_dim; g.din = d->widths[0]; g.dout = d->widths[d->n_layers];
+    g.n_layers = d->n_layers; g.n_prefix = d->n_prefix; g.P = P;
+    for (int l = 0; l < 8; ++l) { g.widths[l] = l <= d->n_layers ? d->widths[l] : 0; g.acts[l] = l < d->n_layers ? d->acts[l] : 0; }
     h->tab.serial = serial;
-    h->ag.t0 = (float)d->t0; h->ag.save_dt = (float)(d->dt * d->save_every); h->ag.abstol = (float)d->abstol; h->ag.reltol = (float)d->reltol;
-    h->ag.n_save = h->n_save; h->ag.max_steps = d->max_steps; h->ag.tgrid = h->d_tgrid; h->ag.nacc = h->d_nacc; h->ag.hstep = h->d_hstep;
-    h->tab.d_theta = h->d_theta;
-    h->tab.P = h->P;
+    h->tab.d_theta = (const float *)h->d_theta;
+    h->tab.P = P;
+    h->tab64.theta = (const double *)h->d_theta;
     for (int i = 0; i < 16; ++i) {
-        h->tab.consts[i] = i < d->n_consts ? (float)d->consts[i] : 0.0f;
-        h->tab.lossw[i] = d->n_loss_weights > 0 ? (i < d->n_loss_weights ? (float)d->loss_weights[i] : 0.0f) : 1.0f;
+        h->tab64.consts[i] = i < d->n_consts ? d->consts[i] : 0.0;
+        h->tab64.lossw[i] = d->n_loss_weights > 0 ? (i < d->n_loss_weights ? d->loss_weights[i] : 0.0) : 1.0;
+        h->tab.consts[i] = (float)h->tab64.consts[i];
+        h->tab.lossw[i] = (float)h->tab64.lossw[i];
     }
     for (int i = 0; i < 8; ++i) h->tab.acts[i] = i < d->n_layers ? d->acts[i] : 0;
+    if (forced) {   // both chains back to back
+        ForcedHost &f = h->fh;
+        const int L0 = (int)d->consts[0];
+        h->DR = d->state_dim + d->widths[L0];
+        f.serial = serial; f.dtype = want64 ? 1 : 0; f.D = d->state_dim; f.R = d->widths[L0]; f.J = (int)d->consts[1]; f.L0 = L0;
+        f.L1 = d->n_layers - L0; f.P = P;
+        for (int l = 0; l < 8; ++l) {
+            f.widths[l] = l <= d->n_layers + 1 ? d->widths[l] : 0;
+            f.acts[l] = l < d->n_layers ? d->acts[l] : 0;
+        }
+        for (int i = 0; i < 16; ++i) f.lossw[i] = h->tab64.lossw[i];
+        f.theta = h->d_theta;
+    }
+    h->oh.theta = h->d_theta;
+    h->oh.ops = h->d_ops;
+    h->oh.rkc = h->d_rkc;
     *out = h;
     return B200UDE_OK;
 }
@@ -1258,8 +1100,6 @@ void b200ude_destroy(b200ude_handle *h)
     cudaFree(h->d_u0_keep); cudaFree(h->d_aux_out);
     cudaFree(h->d_adam_m); cudaFree(h->d_adam_v); cudaFree(h->d_adam_t); cudaFree(h->d_train_out);
     cudaFree(h->d_tgrid); cudaFree(h->d_nacc); cudaFree(h->d_cot); cudaFree(h->d_block_loss); cudaFree(h->d_hstep);
-    cudaFree(h->q_theta); cudaFree(h->q_ustep); cudaFree(h->q_dense); cudaFree(h->q_partial); cudaFree(h->q_tgrid); cudaFree(h->q_cot);
-    cudaFree(h->q_u0_keep); cudaFree(h->q_aux_out); cudaFree(h->q_hstep);
     cudaFree(h->d_forcing); cudaFree(h->d_usave);
     cudaFree(h->d_ops); cudaFree(h->d_rkc);
     if (h->h_loss) cudaFreeHost(h->h_loss);
@@ -1279,11 +1119,7 @@ int32_t b200ude_set_params(b200ude_handle *h, const void *theta, size_t P, int32
     if (!h) return B200UDE_EINVAL;
     if (!theta || P != (size_t)h->P) return fail(h, B200UDE_EINVAL, "set_params: P=%zu, expected %d", P, h->P);
     cudaStream_t st = (cudaStream_t)stream;
-    if (h->kid == K_F64)
-        CUDA_TRY(h, cudaMemcpyAsync(h->q_theta, theta, sizeof(double) * P, mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-    else
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_theta, theta, sizeof(float) * P,
-                                mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_theta, theta, h->es() * P, mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
     h->have_theta = true;
     return B200UDE_OK;
 }
@@ -1291,10 +1127,10 @@ int32_t b200ude_set_params(b200ude_handle *h, const void *theta, size_t P, int32
 int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32_t mem, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (!h->forced) return fail(h, B200UDE_EUNSUPPORTED, "set_forcing: only B200UDE_MODEL_FORCED handles take a forcing (this handle: model %d)", h->desc.model);
+    if (h->kid != K_FORCED) return fail(h, B200UDE_EUNSUPPORTED, "set_forcing: only B200UDE_MODEL_FORCED handles take a forcing (this handle: model %d)", h->desc.model);
     if (!coef || N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "set_forcing: null pointer or N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
-    const size_t es = h->fh.dtype == 1 ? sizeof(double) : sizeof(float);
+    const size_t es = h->es();
     CUDA_TRY(h, cudaMemcpy2DAsync(h->d_forcing, es * h->cap, coef, es * N, es * N, (size_t)3 * h->fh.J,
                                   mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, (cudaStream_t)stream));
     h->forcing_n = N;
@@ -1304,7 +1140,7 @@ int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32
 int32_t b200ude_set_operators(b200ude_handle *h, const void *D1, const void *D2, int32_t mem, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (!h->op) return fail(h, B200UDE_EUNSUPPORTED, "set_operators: only B200UDE_MODEL_OPERATOR handles take operators (this handle: model %d)", h->desc.model);
+    if (h->kid != K_OPERATOR) return fail(h, B200UDE_EUNSUPPORTED, "set_operators: only B200UDE_MODEL_OPERATOR handles take operators (this handle: model %d)", h->desc.model);
     if (!D1) return fail(h, B200UDE_EINVAL, "set_operators: D1 is a null pointer");
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
     const OperatorHost &o = h->oh;
@@ -1323,22 +1159,22 @@ int32_t b200ude_set_operators(b200ude_handle *h, const void *D1, const void *D2,
 int32_t b200ude_forward(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid == K_F64) return do_forward64(h, (const double *)u0, N, (double *)out, status, (cudaStream_t)stream);
+    if (h->f64) return do_forward(h, (const double *)u0, N, (double *)out, status, (cudaStream_t)stream);
     return do_forward(h, (const float *)u0, N, (float *)out, status, (cudaStream_t)stream);
 }
 
 int32_t b200ude_adjoint(b200ude_handle *h, const void *dL_dout, void *grad_theta, void *grad_u0, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid == K_F64) return do_adjoint64(h, false, (const double *)dL_dout, nullptr, (double *)grad_theta, (double *)grad_u0, (cudaStream_t)stream);
-    return do_adjoint(h, false, (const float *)dL_dout, nullptr, (float *)grad_theta, (float *)grad_u0,
+    if (h->f64) return do_adjoint<double>(h, false, (const double *)dL_dout, nullptr, (double *)grad_theta, (double *)grad_u0, (cudaStream_t)stream);
+    return do_adjoint<float>(h, false, (const float *)dL_dout, nullptr, (float *)grad_theta, (float *)grad_u0,
                       (cudaStream_t)stream);
 }
 
 int32_t b200ude_adjoint_l2(b200ude_handle *h, const void *data, void *loss, void *grad_theta, void *grad_u0, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid == K_F64) return do_adjoint64(h, true, (const double *)data, (double *)loss, (double *)grad_theta, (double *)grad_u0, (cudaStream_t)stream);
+    if (h->f64) return do_adjoint(h, true, (const double *)data, (double *)loss, (double *)grad_theta, (double *)grad_u0, (cudaStream_t)stream);
     return do_adjoint(h, true, (const float *)data, (float *)loss, (float *)grad_theta, (float *)grad_u0,
                       (cudaStream_t)stream);
 }
@@ -1361,7 +1197,7 @@ static int32_t ensure_host_path(b200ude_handle *h)
 int32_t b200ude_solve_host(b200ude_handle *h, const void *theta, const void *u0, size_t N, void *out, int32_t *status)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid == K_F64) return f64_unsupported(h, "solve_host");
+    if (h->f64) return f64_unsupported(h, "solve_host");
     if (!theta || !u0 || !out) return fail(h, B200UDE_EINVAL, "solve_host: null pointer");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "solve_host: N=%zu outside (0, %zu]", N, h->cap);
     int32_t rc = ensure_host_path(h);
@@ -1383,7 +1219,7 @@ int32_t b200ude_loss_gradient_host(b200ude_handle *h, const void *theta, const v
                                    double *loss, void *grad_theta, void *grad_u0)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid == K_F64) return f64_unsupported(h, "loss_gradient_host");
+    if (h->f64) return f64_unsupported(h, "loss_gradient_host");
     if (!theta || !u0 || !data || !grad_theta) return fail(h, B200UDE_EINVAL, "loss_gradient_host: null pointer");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "loss_gradient_host: N=%zu outside (0, %zu]", N, h->cap);
     int32_t rc = ensure_host_path(h);
@@ -1423,12 +1259,8 @@ int32_t b200ude_get_params(b200ude_handle *h, void *theta, size_t P, int32_t mem
 {
     if (!h) return B200UDE_EINVAL;
     if (!theta || P != (size_t)h->P) return fail(h, B200UDE_EINVAL, "get_params: P=%zu, expected %d", P, h->P);
-    if (h->kid == K_F64)
-        CUDA_TRY(h, cudaMemcpyAsync(theta, h->q_theta, sizeof(double) * P, mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                                    (cudaStream_t)stream));
-    else
-    CUDA_TRY(h, cudaMemcpyAsync(theta, h->d_theta, sizeof(float) * P,
-                                mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    CUDA_TRY(h, cudaMemcpyAsync(theta, h->d_theta, h->es() * P, mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                                (cudaStream_t)stream));
     if (mem != B200UDE_DEVICE) CUDA_TRY(h, cudaStreamSynchronize((cudaStream_t)stream));
     return B200UDE_OK;
 }
@@ -1480,7 +1312,7 @@ int32_t b200ude_train_adam(b200ude_handle *h, const b200ude_adam *opt, const voi
         if (r) return r;
         // with peers attached (b200ude_peer_attach) the gradient and the loss are the sums over all ranks: every rank runs the
         // same iterations in lock step and applies the identical update to its replica of theta
-        r = do_adjoint(h, true, (const float *)data, h->d_loss, h->d_grad, nullptr, st, h->peer_attached);
+        r = do_adjoint<float>(h, true, (const float *)data, h->d_loss, h->d_grad, nullptr, st, h->peer_attached);
         if (r) return r;
         CUDA_TRY(h, launch_adam(h, opt, h->d_grad, h->d_loss, (float *)loss_history, t_base, st));
         return B200UDE_OK;
@@ -1521,7 +1353,7 @@ static size_t peer_buf_bytes(const b200ude_handle *h)
 int32_t b200ude_peer_export(b200ude_handle *h, void *handle_out)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid == K_F64) return fail(h, B200UDE_EUNSUPPORTED, "peer_export: not available for B200UDE_F64 handles (all-reduce the result of b200ude_adjoint_l2)");
+    if (h->f64) return fail(h, B200UDE_EUNSUPPORTED, "peer_export: not available for B200UDE_F64 handles (all-reduce the result of b200ude_adjoint_l2)");
     if (!handle_out) return fail(h, B200UDE_EINVAL, "peer_export: null pointer");
     static_assert(sizeof(cudaIpcMemHandle_t) == B200UDE_PEER_HANDLE_BYTES, "CUDA IPC handle size");
     if (!h->d_peer_buf) {

@@ -1,12 +1,7 @@
-// k_generic.cu -- shape-generic UDE kernels (runtime chain widths / activations; LV, SEIR, NODE forms) in fp32, and the
-// fixed-step Fisher-KPP kernels.
+// k_generic.cu -- shape-generic UDE kernels (runtime chain widths / activations; LV, SEIR, NODE forms) in fp32: their constant-bank
+// symbols and launchers (ude_launch.cuh), the two-stage L2 cotangent, and the fixed-step Fisher-KPP kernels.
 #include "ude_adjoint.cuh"
-#include "ude_generic.cuh"
-#include "fkpp_adaptive.cuh"
-#include "discrete_adjoint.cuh"
-#include "fkpp_vern7_discrete.cuh"
-#include "vern7_dense.cuh"
-#include "vern7_dense_discrete.cuh"
+#include "ude_launch.cuh"
 
 #include <algorithm>
 
@@ -46,10 +41,6 @@ struct Ops32 {
     static __device__ __forceinline__ float act(int k, float a) { return k == ACT_TANH ? tanh_dev<0>(a) : (k == ACT_RBF ? rbf_dev(a) : a); }
 };
 
-constexpr int GEN_BLOCK = 128;
-
-int adj_rows_generic(int N) { return ((N + GEN_BLOCK - 1) / GEN_BLOCK) * (GEN_BLOCK / 32); }
-
 static cudaError_t upload_gen(const GenericShape &g, cudaStream_t st)
 {
     static SerialCache cache;
@@ -68,165 +59,17 @@ static cudaError_t upload_gen(const GenericShape &g, cudaStream_t st)
     return e;
 }
 
-cudaError_t launch_fwd_generic(const GenericShape &g, const ConstTables &t, const FwdParams &p, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    generic::forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_adj_generic(const GenericShape &g, const ConstTables &t, const AdjParams &p, cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    auto kern = generic::adjoint_kernel<Ops32, GEN_BLOCK>;
-    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
-    *rows_out = grid * (GEN_BLOCK / 32);
-    kern<<<grid, GEN_BLOCK, smem, st>>>(p);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_fwd_vern7(const GenericShape &g, const ConstTables &t, const FwdParams &p, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    generic::vern7_forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_fwd_vern7_adaptive(const GenericShape &g, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    // the step record only for the discrete adjoint (p.ustep set); the interpolating adjoint re-solves with Tsit5
-    generic::vern7_adaptive_forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ag);
-    return cudaGetLastError();
-}
-
-// ---- discrete adjoint (discrete_adjoint.cuh in fp32) ----
-
-cudaError_t launch_adj_discrete(const GenericShape &g, const ConstTables &t, const AdjParams &p, int solver, const AdaptiveGrid *ag,
-                                cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    discrete::Params<float> q;
-    q.ustep = p.ustep; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
-    q.tgrid = ag ? ag->tgrid : nullptr; q.hstep = ag ? ag->hstep : nullptr; q.nacc = ag ? ag->nacc : nullptr;
-    q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
-    q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
-    q.margin = 5e-7f;   // half the clipping margin of vern7_adaptive_forward_kernel
-    auto kern = solver == 1 ? discrete::adjoint_kernel<Ops32, discrete::Vern7Scheme, GEN_BLOCK>
-                            : discrete::adjoint_kernel<Ops32, discrete::Tsit5Scheme, GEN_BLOCK>;
-    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
-    *rows_out = grid * (GEN_BLOCK / 32);
-    kern<<<grid, GEN_BLOCK, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
-// ---- Vern7 with its lazy dense output (vern7_dense.cuh in fp32) ----
-
-cudaError_t launch_fwd_vern7_dense(const GenericShape &g, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    vern7_dense::Fwd<float> q;
-    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.tgrid = ag.tgrid; q.hstep = ag.hstep; q.nacc = ag.nacc; q.status = p.status;
-    q.N = p.N; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
-    q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    vern7_dense::forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(q);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_adj_vern7_dense(const GenericShape &g, const ConstTables &t, const AdjParams &p, const AdaptiveGrid *ag, const float *saved,
-                                   cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    vern7_dense::Adj<float> q;
-    q.ustep = p.ustep; q.tgrid = ag ? ag->tgrid : nullptr; q.hstep = ag ? ag->hstep : nullptr; q.nacc = ag ? ag->nacc : nullptr;
-    q.cot = p.cot; q.saved = saved; q.grad_u0 = p.grad_u0; q.partial = p.partial;
-    q.N = p.N; q.n_steps = p.n_steps; q.save_every = p.save_every; q.n_save = p.n_steps / p.save_every + 1; q.fused_l2 = p.fused_l2;
-    q.dt = p.dt; q.t0 = ag ? ag->t0 : 0.0f; q.save_dt = ag ? ag->save_dt : 0.0f;
-    auto kern = vern7_dense::adjoint_kernel<Ops32, GEN_BLOCK>;
-    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
-    *rows_out = grid * (GEN_BLOCK / 32);
-    kern<<<grid, GEN_BLOCK, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
-// ---- discrete adjoint through the interpolated saves of the dense-output forward (vern7_dense_discrete.cuh in fp32) ----
-cudaError_t launch_adj_vern7_dense_discrete(const GenericShape &g, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag,
-                                            const float *saved, cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    vern7_dense_discrete::Params<float> q;
-    q.ustep = p.ustep; q.tgrid = ag.tgrid; q.hstep = ag.hstep; q.nacc = ag.nacc; q.cot = p.cot; q.saved = saved;
-    q.grad_u0 = p.grad_u0; q.partial = p.partial; q.N = p.N; q.n_save = ag.n_save; q.fused_l2 = p.fused_l2;
-    q.t0 = ag.t0; q.save_dt = ag.save_dt;
-    auto kern = vern7_dense_discrete::adjoint_kernel<Ops32, GEN_BLOCK>;
-    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
-    *rows_out = grid * (GEN_BLOCK / 32);
-    kern<<<grid, GEN_BLOCK, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
-// ---- adaptive stepping ----
-cudaError_t launch_fwd_adaptive(const GenericShape &g, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    generic::adaptive_forward_kernel<Ops32, GEN_BLOCK><<<(p.N + GEN_BLOCK - 1) / GEN_BLOCK, GEN_BLOCK, 0, st>>>(p, ag);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_adj_adaptive(const GenericShape &g, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag, cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(g, st);
-    if (e != cudaSuccess) return e;
-    auto kern = generic::adaptive_adjoint_kernel<Ops32, GEN_BLOCK>;
-    const size_t smem = sizeof(float) * (size_t)(GEN_BLOCK / 32) * (g.P + 1);
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + GEN_BLOCK - 1) / GEN_BLOCK;
-    *rows_out = grid * (GEN_BLOCK / 32);
-    kern<<<grid, GEN_BLOCK, smem, st>>>(p, ag);
-    return cudaGetLastError();
-}
+template <>
+struct ShapeUnit<float> {
+    using Ops = Ops32;
+    static constexpr int BLOCK = 128;
+    static cudaError_t upload(const GenericShape &g, const ConstTables &t, cudaStream_t st)
+    {
+        cudaError_t e = upload_tables(t, st);
+        return e != cudaSuccess ? e : upload_gen(g, st);
+    }
+};
+template struct RuntimeShape<float>;
 
 // L2 cotangent 2 w (out - data) and loss for paths that take a generic cotangent (adaptive solves)
 struct LossW { float w[16]; };
@@ -425,9 +268,7 @@ int adj_rows_fkpp(int N, int Nx)
 
 cudaError_t launch_fwd_fkpp(const GenericShape &gs, const ConstTables &t, const FwdParams &p, cudaStream_t st)
 {
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(gs, st);
+    cudaError_t e = ShapeUnit<float>::upload(gs, t, st);
     if (e != cudaSuccess) return e;
     int tpc, th;
     fkpp_adapt::cta_geometry(gs.D, &tpc, &th);
@@ -438,9 +279,7 @@ cudaError_t launch_fwd_fkpp(const GenericShape &gs, const ConstTables &t, const 
 
 cudaError_t launch_adj_fkpp(const GenericShape &gs, const ConstTables &t, const AdjParams &p, cudaStream_t st, int *rows_out)
 {
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(gs, st);
+    cudaError_t e = ShapeUnit<float>::upload(gs, t, st);
     if (e != cudaSuccess) return e;
     int tpc, th;
     fkpp_adapt::cta_geometry(gs.D, &tpc, &th);
@@ -453,94 +292,10 @@ cudaError_t launch_adj_fkpp(const GenericShape &gs, const ConstTables &t, const 
     return cudaGetLastError();
 }
 
-// ---- Fisher-KPP, adaptive Tsit5 (fkpp_adaptive.cuh in fp32) ----
+// ---- Fisher-KPP, adaptive (fkpp_adaptive.cuh): the shared-memory check of b200ude_create, both precisions ----
 size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes)
 {
     return std::max(fkpp_adapt::fwd_smem(Nx, real_bytes), fkpp_adapt::adj_smem(Nx, P, real_bytes));
-}
-
-cudaError_t launch_fwd_fkpp_adaptive(const GenericShape &gs, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(gs, st);
-    if (e != cudaSuccess) return e;
-    fkpp_adapt::Fwd<float> q;
-    int th;
-    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
-    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
-    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
-    q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    auto kern = fkpp_adapt::forward_kernel<Ops32>;
-    const size_t smem = fkpp_adapt::fwd_smem(gs.D, sizeof(float));
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kern<<<(p.N + q.tpc - 1) / q.tpc, th, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_adj_fkpp_adaptive(const GenericShape &gs, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag, cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(gs, st);
-    if (e != cudaSuccess) return e;
-    fkpp_adapt::Adj<float> q;
-    int th;
-    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
-    q.ustep = p.ustep; q.dense = p.dense; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
-    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.t0 = ag.t0; q.save_dt = ag.save_dt;
-    auto kern = fkpp_adapt::adjoint_kernel<Ops32>;
-    const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + q.tpc - 1) / q.tpc;
-    *rows_out = grid * (th / 32);
-    kern<<<grid, th, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
-// ---- Fisher-KPP, adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh in fp32) ----
-cudaError_t launch_fwd_fkpp_vern7(const GenericShape &gs, const ConstTables &t, const FwdParams &p, const AdaptiveGrid &ag, cudaStream_t st)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(gs, st);
-    if (e != cudaSuccess) return e;
-    fkpp_vern7::Fwd<float> q;
-    int th;
-    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
-    q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.hstep = ag.hstep; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
-    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
-    q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    auto kern = fkpp_vern7::vern7_forward_kernel<Ops32>;
-    const size_t smem = fkpp_adapt::fwd_smem(gs.D, sizeof(float));
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kern<<<(p.N + q.tpc - 1) / q.tpc, th, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_adj_fkpp_vern7(const GenericShape &gs, const ConstTables &t, const AdjParams &p, const AdaptiveGrid &ag, cudaStream_t st, int *rows_out)
-{
-    cudaError_t e = upload_tables(t, st);
-    if (e != cudaSuccess) return e;
-    e = upload_gen(gs, st);
-    if (e != cudaSuccess) return e;
-    fkpp_vern7::Adj<float> q;
-    int th;
-    fkpp_adapt::cta_geometry(gs.D, &q.tpc, &th);
-    q.ustep = p.ustep; q.hstep = ag.hstep; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
-    q.N = p.N; q.Nx = gs.D; q.n_save = ag.n_save; q.fused_l2 = p.fused_l2; q.t0 = ag.t0; q.save_dt = ag.save_dt;
-    q.margin = 5e-7f;   // half the clipping margin of the forward
-    auto kern = fkpp_vern7::discrete_adjoint_kernel<Ops32>;
-    const size_t smem = fkpp_adapt::adj_smem(gs.D, gs.P, sizeof(float));
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    const int grid = (p.N + q.tpc - 1) / q.tpc;
-    *rows_out = grid * (th / 32);
-    kern<<<grid, th, smem, st>>>(q);
-    return cudaGetLastError();
 }
 
 }  // namespace b200ude

@@ -122,40 +122,12 @@ cudaError_t launch_tanh_selftest(const float *x, float *y, size_t n, cudaStream_
 cudaError_t launch_fwd_lv32_adaptive(const Variant &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
 cudaError_t launch_adj_lv32_adaptive(const Variant &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
 int adj_grid_lv5(int N);
-cudaError_t launch_fwd_generic(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
-cudaError_t launch_adj_generic(const GenericShape &, const ConstTables &, const AdjParams &, cudaStream_t, int *rows_out);
-int adj_rows_generic(int N);
-cudaError_t launch_fwd_vern7(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
-cudaError_t launch_fwd_vern7_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
-cudaError_t launch_fwd_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
-cudaError_t launch_adj_adaptive(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
-// discrete adjoint (discrete_adjoint.cuh) of a runtime-shape Tsit5 (solver 0) / Vern7 (solver 1) solve; ag: the adaptive Vern7
-// record, nullptr on a fixed grid.  Partial rows as adj_rows_generic.
-cudaError_t launch_adj_discrete(const GenericShape &, const ConstTables &, const AdjParams &, int solver, const AdaptiveGrid *ag,
-                                cudaStream_t, int *rows_out);
-// Vern7 with its lazy dense output (vern7_dense.cuh, B200UDE_FLAG_VERN7_DENSE): the adaptive forward saving through the interpolant
-// (record: p.ustep, ag.tgrid, ag.hstep, ag.nacc), and the interpolating adjoint over that dense output, ag = nullptr on a fixed grid
-// (record: p.ustep of launch_fwd_vern7).  saved: the forward's `out`, read by the fused L2 on an adaptive grid.  Rows as adj_rows_generic.
-cudaError_t launch_fwd_vern7_dense(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
-cudaError_t launch_adj_vern7_dense(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid *ag, const float *saved,
-                                   cudaStream_t, int *rows_out);
-// discrete adjoint of that adaptive forward through its interpolated saves (vern7_dense_discrete.cuh, B200UDE_FLAG_DISCRETE_DENSE):
-// record and `saved` as above, rows as adj_rows_generic
-cudaError_t launch_adj_vern7_dense_discrete(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &,
-                                            const float *saved, cudaStream_t, int *rows_out);
 cudaError_t launch_l2_cot(const ConstTables &, const float *out, const float *data, float *cot, float *block_loss, int D, size_t N, int n_save, cudaStream_t);
 cudaError_t launch_l2_finish(const float *block_loss, float *loss, cudaStream_t);
 cudaError_t launch_fwd_fkpp(const GenericShape &, const ConstTables &, const FwdParams &, cudaStream_t);
 cudaError_t launch_adj_fkpp(const GenericShape &, const ConstTables &, const AdjParams &, cudaStream_t, int *rows_out);
 int adj_rows_fkpp(int N, int Nx);
-// adaptive Tsit5 of the Fisher-KPP UPDE (fkpp_adaptive.cuh): partial rows as adj_rows_fkpp in both precisions
-cudaError_t launch_fwd_fkpp_adaptive(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
-cudaError_t launch_adj_fkpp_adaptive(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
-size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes);   // per-CTA dynamic shared memory of the larger of the two kernels
-// adaptive Vern7 of the Fisher-KPP UPDE with the discrete adjoint (fkpp_vern7_discrete.cuh): same geometry and shared memory as
-// adaptive Tsit5; the record is ustep / ag.tgrid / ag.hstep / ag.nacc; p.fused_l2 reads the recorded step-end states
-cudaError_t launch_fwd_fkpp_vern7(const GenericShape &, const ConstTables &, const FwdParams &, const AdaptiveGrid &, cudaStream_t);
-cudaError_t launch_adj_fkpp_vern7(const GenericShape &, const ConstTables &, const AdjParams &, const AdaptiveGrid &, cudaStream_t, int *rows_out);
+size_t fkpp_adaptive_smem(int Nx, int P, int real_bytes);   // per-CTA dynamic shared memory of the larger of the two adaptive kernels
 cudaError_t launch_fwd_seir(const Variant &, const ConstTables &, const FwdParams &, cudaStream_t);
 cudaError_t launch_adj_seir(const Variant &, const ConstTables &, const AdjParams &, cudaStream_t, int *rows_out);
 cudaError_t launch_fwd_seir_vern7(const Variant &, const ConstTables &, const FwdParams &, cudaStream_t);
@@ -182,12 +154,10 @@ struct PeerLinks {
 cudaError_t launch_reduce_exchange(const float *partial, int nblocks, int P1, const PeerLinks &, float *grad, float *loss, cudaStream_t);
 cudaError_t launch_reduce(const float *partial, int nblocks, int P1, float *grad, float *loss, cudaStream_t);
 
-// ---- double-precision path (dtype = B200UDE_F64; k_f64.cu).  Fwd64Host / Adj64Host / Adapt64Host are also the parameters of the
-// fp64 runtime-shape kernels (ude_generic.cuh), as FwdParams / AdjParams / AdaptiveGrid are of the fp32 ones ----
-struct Shape64Host {
-    uint64_t serial;
-    int model, D, din, dout, n_layers, n_prefix, P;
-    int widths[8], acts[8];
+// ---- the runtime-shape kernels (ude_generic.cuh and the headers written over its Ops) in both precisions: fp32 (k_generic.cu) and
+// fp64 (dtype = B200UDE_F64, k_f64.cu).  Fwd64Host / Adj64Host / Adapt64Host are the parameters of the fp64 kernels, as FwdParams /
+// AdjParams / AdaptiveGrid are of the fp32 ones ----
+struct Tables64 {   // fp64 counterpart of ConstTables: theta, constants and loss weights of a handle
     const double *theta;
     double consts[16], lossw[16];
 };
@@ -211,23 +181,56 @@ struct Adapt64Host {
     int *nacc;
     double *hstep;   // discrete-adjoint Vern7 handles only, else nullptr
 };
-int adj_rows_f64(int N);
-cudaError_t launch_fwd_f64(const Shape64Host &, const Fwd64Host &, int solver, const Adapt64Host *adaptive_or_null, cudaStream_t);
-cudaError_t launch_adj_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *adaptive_or_null, cudaStream_t, int *rows_out);
-// discrete adjoint in fp64 (discrete_adjoint.cuh): solver 0 = Tsit5, 1 = Vern7; ad = adaptive Vern7 record or nullptr
-cudaError_t launch_adj_discrete_f64(const Shape64Host &, const Adj64Host &, int solver, const Adapt64Host *ad, cudaStream_t, int *rows_out);
-// Vern7 with its lazy dense output in fp64 (as launch_fwd_vern7_dense / launch_adj_vern7_dense); rows as adj_rows_f64
-cudaError_t launch_fwd_vern7_dense_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);
-cudaError_t launch_adj_vern7_dense_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host *ad, const double *saved, cudaStream_t,
-                                       int *rows_out);
-cudaError_t launch_adj_vern7_dense_discrete_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, const double *saved,
-                                                cudaStream_t, int *rows_out);   // as launch_adj_vern7_dense_discrete
+template <typename R>
+struct RealParams;
+template <>
+struct RealParams<float> {
+    using Tab = ConstTables;
+    using Fwd = FwdParams;
+    using Adj = AdjParams;
+    using Adapt = AdaptiveGrid;
+};
+template <>
+struct RealParams<double> {
+    using Tab = Tables64;
+    using Fwd = Fwd64Host;
+    using Adj = Adj64Host;
+    using Adapt = Adapt64Host;
+};
+// launchers (ude_launch.cuh).  ag: the adaptive record, nullptr on a fixed grid.  The partial rows of every adjoint but the
+// Fisher-KPP ones are adj_rows(N); the Fisher-KPP ones are adj_rows_fkpp(N, Nx)
+template <typename R>
+struct RuntimeShape {
+    using Tab = typename RealParams<R>::Tab;
+    using Fwd = typename RealParams<R>::Fwd;
+    using Adj = typename RealParams<R>::Adj;
+    using Adapt = typename RealParams<R>::Adapt;
+    static int adj_rows(int N);
+    // Tsit5 (solver 0) / Vern7 (solver 1) forward; Vern7 records u_n of every step when p.ustep is set (discrete adjoint)
+    static cudaError_t fwd(const GenericShape &, const Tab &, const Fwd &, int solver, const Adapt *ag, cudaStream_t);
+    // interpolating adjoint over the Tsit5 dense record, the replay of an adaptive solve when ag is set
+    static cudaError_t adj(const GenericShape &, const Tab &, const Adj &, const Adapt *ag, cudaStream_t, int *rows_out);
+    // discrete adjoint (discrete_adjoint.cuh) of a Tsit5 (solver 0) / Vern7 (solver 1) solve over its recorded steps
+    static cudaError_t adj_discrete(const GenericShape &, const Tab &, const Adj &, int solver, const Adapt *ag, cudaStream_t, int *rows_out);
+    // Vern7 with its lazy dense output (vern7_dense.cuh, B200UDE_FLAG_VERN7_DENSE): the adaptive forward saving through the interpolant
+    // (record: p.ustep, ag.tgrid, ag.hstep, ag.nacc), and the interpolating adjoint over that dense output, ag = nullptr on a fixed grid
+    // (record: p.ustep of fwd with solver 1).  saved: the forward's `out`, read by the fused L2 on an adaptive grid
+    static cudaError_t fwd_vern7_dense(const GenericShape &, const Tab &, const Fwd &, const Adapt &, cudaStream_t);
+    static cudaError_t adj_vern7_dense(const GenericShape &, const Tab &, const Adj &, const Adapt *ag, const R *saved, cudaStream_t, int *rows_out);
+    // discrete adjoint of that adaptive forward through its interpolated saves (vern7_dense_discrete.cuh, B200UDE_FLAG_DISCRETE_DENSE)
+    static cudaError_t adj_vern7_dense_discrete(const GenericShape &, const Tab &, const Adj &, const Adapt &, const R *saved, cudaStream_t,
+                                                int *rows_out);
+    // adaptive Tsit5 of the Fisher-KPP UPDE (fkpp_adaptive.cuh)
+    static cudaError_t fwd_fkpp_adaptive(const GenericShape &, const Tab &, const Fwd &, const Adapt &, cudaStream_t);
+    static cudaError_t adj_fkpp_adaptive(const GenericShape &, const Tab &, const Adj &, const Adapt &, cudaStream_t, int *rows_out);
+    // adaptive Vern7 of the Fisher-KPP UPDE with the discrete adjoint (fkpp_vern7_discrete.cuh): same geometry and shared memory as
+    // adaptive Tsit5; the record is p.ustep / ag.tgrid / ag.hstep / ag.nacc; p.fused_l2 reads the recorded step-end states
+    static cudaError_t fwd_fkpp_vern7(const GenericShape &, const Tab &, const Fwd &, const Adapt &, cudaStream_t);
+    static cudaError_t adj_fkpp_vern7(const GenericShape &, const Tab &, const Adj &, const Adapt &, cudaStream_t, int *rows_out);
+};
 cudaError_t launch_reduce_f64(const double *partial, int nrows, int P1, double *grad, double *loss, cudaStream_t);
-cudaError_t launch_fwd_fkpp_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // adaptive Tsit5 only
-cudaError_t launch_adj_fkpp_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);
-cudaError_t launch_fwd_fkpp_vern7_f64(const Shape64Host &, const Fwd64Host &, const Adapt64Host &, cudaStream_t);   // discrete adjoint handles
-cudaError_t launch_adj_fkpp_vern7_f64(const Shape64Host &, const Adj64Host &, const Adapt64Host &, cudaStream_t, int *rows_out);
-cudaError_t launch_l2_cot_f64(const Shape64Host &, const double *out, const double *data, double *cot, double *loss, size_t N, int n_save, cudaStream_t);
+cudaError_t launch_l2_cot_f64(const Tables64 &, const double *out, const double *data, double *cot, double *loss, int D, size_t N, int n_save,
+                              cudaStream_t);
 
 // ---- forced neural ODE with a readout network (B200UDE_MODEL_FORCED; forced.cuh, k_forced.cu), fp32 and fp64 ----
 struct ForcedHost {
