@@ -92,10 +92,12 @@ extern "C" {
 #define B200UDE_MODEL_OPERATOR 6 /* wide-state operator UDE (Climate/NeuralPDE/npde.jl:75-78):  du = D1 * NN(u) + D2 * u,
                                     NN: widths[0] = d -> ... -> widths[n_layers] = m; D1 (d x m) and D2 (d x d) fixed, column-major,
                                     set by b200ude_set_operators.  Envelope: d 1..64, every width 1..64, 1..5 layers, activations
-                                    identity / tanh / rbf; n_prefix = n_suffix = n_consts = 0; n_loss_weights 0, or d when d <= 16.
+                                    identity / tanh / rbf; n_prefix = n_suffix = n_consts = 0 (adaptive RKC2: n_consts = 1,
+                                    consts[0] = eigen_est); n_loss_weights 0, or d when d <= 16.
                                     theta = per layer vec(W) then b (Flux.destructure).  A warp integrates one trajectory.
-                                    Tsit5 fixed step or adaptive, RKC2 fixed step (2..64 stages), interpolating adjoint, fp32 and
-                                    fp64.  Vern7, the discrete adjoint and the dense flags return B200UDE_EUNSUPPORTED;
+                                    Tsit5 fixed step or adaptive, RKC2 fixed step (2..64 stages) or adaptive (each step takes the
+                                    fewest stages, up to n_stages, that are stable for h * eigen_est; eigen_est finite and > 0),
+                                    interpolating adjoint, fp32 and fp64.  Vern7, the discrete adjoint and the dense flags return B200UDE_EUNSUPPORTED;
                                     B200UDE_FLAG_APPROX_TANH is accepted and ignored.  create returns B200UDE_EUNSUPPORTED when the
                                     staged operators, theta and one warp's gradient vector exceed the device's shared memory. */
 
@@ -110,7 +112,11 @@ extern "C" {
 #define B200UDE_RKC2 2 /* second-order Runge-Kutta-Chebyshev with desc.n_stages stages per step: the closed-form stabilised explicit
                           method of the class of ROCK2 (Climate/NeuralPDE/npde.jl:61,82; ROCK2's own coefficient tables are not in the
                           reference); real stability interval ~ 0.65 n_stages^2; dense output = cubic Hermite; the interpolating
-                          adjoint steps lambda backwards with RKC2 itself.  Fisher-KPP UPDE (1-16-16-1 chain, even grids), fixed step */
+                          adjoint steps lambda backwards with RKC2 itself.  Fisher-KPP UPDE (1-16-16-1 chain, even grids), fixed step;
+                          B200UDE_MODEL_OPERATOR, fixed step, or adaptive (ROCK2(eigen_est = rho) without dt): consts[0] = rho, an
+                          upper bound of the spectral radius of df/du, n_consts = 1, n_stages = the cap on stages per step; each
+                          step takes the fewest stages s with stability interval >= 1.05 h rho, the RKC error estimate and the
+                          PI controller pick h, and the replay adjoint steps each recorded step with its own s */
 
 /* sensealg */
 #define B200UDE_INTERPOLATING_ADJOINT 0 /* InterpolatingAdjoint(autojacvec = ReverseDiffVJP())  seir_exposure.jl:71,140 */
@@ -209,7 +215,7 @@ typedef struct b200ude_desc {
                            saveat = t0 + i*save_every*dt, i = 0..n_steps/save_every (dt only defines the save grid).
                            LV / SEIR / NODE forms (Tsit5 or Vern7) and the Fisher-KPP UPDE (Tsit5, or Vern7 with the discrete
                            adjoint; its error norm is taken over the whole grid, as OrdinaryDiffEq's default norm over the state
-                           vector), fp32 and fp64 */
+                           vector), fp32 and fp64.  On B200UDE_MODEL_OPERATOR: Tsit5, or RKC2 with eigen_est in consts[0] */
     int32_t max_steps;  /* adaptive: capacity of ACCEPTED steps per trajectory (status 2 when exceeded) */
     int32_t n_stages;   /* B200UDE_RKC2: stages per step (2..64); choose dt * spectral_radius <= 0.65 n_stages^2.  0 otherwise */
 } b200ude_desc;

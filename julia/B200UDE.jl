@@ -121,6 +121,28 @@ unflat(p::AbstractVector, g) = eltype(p).(g)
 const HANDLES = Dict{Any,Handle}()
 solver_code(::Tsit5) = TSIT5
 solver_code(::Vern7) = VERN7
+# ROCK2 / ROCK4 (npde.jl:61,82,111,122) run as RKC2, the stabilised explicit method of the same class this library has (ROCK's own
+# tables are not in the reference).  Their eigen_est is a callback that stores the bound in integ.eigen_est: it is called once
+# on a probe to read the bound.  With dt: fixed-step RKC2 with the fewest stages whose stability interval covers 1.05 dt rho.
+# Without dt on the operator model: adaptive RKC2, rho in consts[0], each step choosing its own stage count (at most 64).
+solver_code(::Union{ROCK2,ROCK4}) = RKC2
+mutable struct EigenProbe
+    eigen_est::Float64
+end
+function eigen_est_of(alg)
+    probe = EigenProbe(0.0)
+    alg.eigen_est(probe)
+    probe.eigen_est
+end
+function rkc2_beta(s)   # real stability interval of s-stage RKC2 (sciml._rkc2_beta)
+    w0 = 1 + (2 / 13) / s^2
+    T0, T1, d0, d1, e0, e1 = 1.0, w0, 0.0, 1.0, 0.0, 0.0
+    for _ in 2:s
+        T0, T1, d0, d1, e0, e1 = T1, 2w0 * T1 - T0, d1, 2T1 + 2w0 * d1 - d0, e1, 4d1 + 2w0 * e1 - e0
+    end
+    (w0 + 1) * e1 / d1
+end
+rock_stages(dt, rho) = something(findfirst(s -> s >= 2 && rkc2_beta(s) >= 1.05 * dt * rho, 1:64), 0)   # 0: create refuses it
 sens_code(::InterpolatingAdjoint) = INTERPOLATING_ADJOINT
 sens_code(::ForwardDiffSensitivity) = DISCRETE_ADJOINT      # same quantity (exact derivative of the discrete scheme), reverse mode
 sens_code(::Nothing) = INTERPOLATING_ADJOINT
@@ -139,14 +161,18 @@ function handle_for(f::B200UDEFunction, alg, sensealg, tspan, saveat, dt, abstol
     all(isapprox.(diff(ts), save_dt; rtol = 1e-9)) || error("B200UDE: uniformly spaced saveat only")
     adaptive = dt === nothing
     step = adaptive ? save_dt : dt
-    key = (objectid(f), typeof(alg), sens_code(sensealg), dense_flag(f, alg, sensealg), tspan, save_dt, step, adaptive, abstol, reltol)
+    rock = alg isa Union{ROCK2,ROCK4}
+    rho = rock ? eigen_est_of(alg) : 0.0
+    key = (objectid(f), typeof(alg), rho, sens_code(sensealg), dense_flag(f, alg, sensealg), tspan, save_dt, step, adaptive, abstol, reltol)
     h = get(HANDLES, key, nothing)
     (h !== nothing && h.cap >= N) && return h
     nl = length(f.acts)
+    cs = rock && adaptive && f.model == MODEL_OPERATOR ? [f.consts; rho] : f.consts
     d = Desc(model = f.model, state_dim = f.state_dim, n_layers = nl,
              widths = ntuple(i -> i <= nl + 1 ? f.widths[i] : Int32(0), 7), acts = ntuple(i -> i <= nl ? f.acts[i] : Int32(0), 6),
-             n_prefix = f.n_prefix, n_suffix = f.n_suffix, n_consts = length(f.consts),
-             consts = ntuple(i -> i <= length(f.consts) ? f.consts[i] : 0.0, 16),
+             n_prefix = f.n_prefix, n_suffix = f.n_suffix, n_consts = length(cs),
+             consts = ntuple(i -> i <= length(cs) ? cs[i] : 0.0, 16),
+             n_stages = !rock ? 0 : adaptive ? 64 : rock_stages(step, rho),
              solver = solver_code(alg), sensealg = sens_code(sensealg), t0 = tspan[1], dt = step,
              n_steps = round(Int32, (tspan[2] - tspan[1]) / step), save_every = round(Int32, save_dt / step),
              adaptive = adaptive ? 1 : 0, abstol = abstol, reltol = reltol, max_steps = adaptive ? 512 : 0, max_trajectories = N,

@@ -81,4 +81,20 @@ L, g, gu = s.adjoint_l2(out8 + 0.1, want_grad_u0=True)
 torch.cuda.synchronize()
 print("node8_max f64", float(L), float(g.abs().sum()))
 s.close()
+# adaptive RKC2 on the operator UDE (operator.cuh kernels 7 and 8): npde.jl's 30-8-30 closure, stage count per step from eigen_est
+import operator_ref as OR
+D1, D2 = OR.npde_ops()
+opf = ude.OperatorUDE(ude.FastChain(ude.FastDense(30, 8, ude.tanh), ude.FastDense(8, 30, ude.tanh)), D1, D2)
+zo = OR.npde_grid()[1:31]
+uo = np.exp(-200.0 * (zo[:, None] - rng.uniform(0.2, 0.8, 70)[None, :]) ** 2).astype(np.float32)
+yo = np.repeat(uo[None], 11, axis=0)
+tho = OR.glorot([30, 8, 30], np.random.default_rng(0))
+run("operator-rkc2-adaptive f32", opf, tho, uo, yo, 0.15, 10, 1, alg=ude.RKC2(eigen_est=191.7), adaptive=True, max_steps=400)
+s = ude.UDESolver(opf, 0.0, 0.15, 10, 1, max_trajectories=70, alg=ude.RKC2(eigen_est=191.7), adaptive=True, max_steps=400, dtype=torch.float64)
+s.set_params(torch.from_numpy(tho).cuda())
+s.forward(torch.from_numpy(uo.astype(np.float64)).cuda())
+L, g, gu = s.adjoint_l2(torch.from_numpy(yo.astype(np.float64)).cuda(), want_grad_u0=True)
+torch.cuda.synchronize()
+print("operator-rkc2-adaptive f64", float(L), float(g.abs().sum()))
+s.close()
 print("ALL DONE")

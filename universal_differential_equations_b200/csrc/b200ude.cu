@@ -7,6 +7,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -128,6 +129,7 @@ struct b200ude_handle {
     bool ops_set = false;
     OperatorHost oh{};
     void *d_ops = nullptr, *d_rkc = nullptr;
+    int *d_sstep = nullptr;   // adaptive RKC2: the stage count of each accepted step [max_steps][cap]
     size_t dev_bytes = 0;
     std::string err;
     size_t es() const { return f64 ? sizeof(double) : sizeof(float); }
@@ -222,6 +224,18 @@ void rkc2_tables(int s, RkcHost *out)
 // operator UDE RKC2 table layout (operator.cuh: mt1, then c, w, mu, nu, mt, ga with 65 entries each); k = 0..5 in that order
 constexpr int op_rkc_len() { return 1 + 6 * 65; }
 constexpr int op_rkc_off(int k) { return 1 + 65 * k; }
+
+// length of the real stability interval of s-stage RKC2 (damping 2/13): (w0 + 1) T''_s(w0) / T'_s(w0) ~ 0.65 s^2
+double rkc2_beta64(int s)
+{
+    const double w0 = 1.0 + (2.0 / 13.0) / ((double)s * s);
+    double T0 = 1, T1 = w0, d0 = 0, d1 = 1, e0 = 0, e1 = 0;
+    for (int j = 2; j <= s; ++j) {
+        const double T2 = 2 * w0 * T1 - T0, d2 = 2 * T1 + 2 * w0 * d1 - d0, e2 = 4 * d1 + 2 * w0 * e1 - e0;
+        T0 = T1; T1 = T2; d0 = d1; d1 = d2; e0 = e1; e1 = e2;
+    }
+    return (w0 + 1.0) * e1 / d1;
+}
 
 // n doubles -> dst (device) in the handle's dtype, synchronously
 cudaError_t upload_as(void *dst, const double *src, size_t n, bool f64)
@@ -714,14 +728,17 @@ int32_t operator_check(const b200ude_desc *d)
     if (d->solver == B200UDE_VERN7 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT ||
         (d->flags & (B200UDE_FLAG_VERN7_DENSE | B200UDE_FLAG_DISCRETE_DENSE)))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
-                    "create: B200UDE_MODEL_OPERATOR (operator UDE du = D1 NN(u) + D2 u) has kernels for Tsit5, fixed step or adaptive, and "
-                    "fixed-step RKC2, with the interpolating adjoint; not for Vern7, the discrete adjoint, B200UDE_FLAG_VERN7_DENSE or "
+                    "create: B200UDE_MODEL_OPERATOR (operator UDE du = D1 NN(u) + D2 u) has kernels for Tsit5 and RKC2, fixed step or "
+                    "adaptive, with the interpolating adjoint; not for Vern7, the discrete adjoint, B200UDE_FLAG_VERN7_DENSE or "
                     "B200UDE_FLAG_DISCRETE_DENSE");
     const char *why = nullptr;
     const int D = d->state_dim, NL = d->n_layers;
+    // adaptive RKC2 picks each step's stage count from eigen_est, the one constant this model takes (consts[0])
+    const bool ark = d->solver == B200UDE_RKC2 && d->adaptive;
     if (D < 1 || D > 64) why = "state_dim must be 1..64";
     else if (NL > 5) why = "n_layers must be 1..5";
-    else if (d->n_prefix != 0 || d->n_suffix != 0 || d->n_consts != 0) why = "n_prefix, n_suffix and n_consts must be 0";
+    else if (d->n_prefix != 0 || d->n_suffix != 0 || (d->n_consts != 0 && !(ark && d->n_consts == 1)))
+        why = "n_prefix, n_suffix and n_consts must be 0 (n_consts = 1 only for adaptive RKC2: eigen_est in consts[0])";
     if (!why) {
         for (int l = 0; l <= NL; ++l)
             if (d->widths[l] < 1 || d->widths[l] > 64) why = "every width must be 1..64";
@@ -732,7 +749,10 @@ int32_t operator_check(const b200ude_desc *d)
         if (d->widths[0] != D) why = "the chain's input widths[0] must be state_dim";
         else if (d->n_loss_weights != 0 && (d->n_loss_weights != D || D > 16)) why = "n_loss_weights must be 0, or state_dim when state_dim <= 16";
         else if (d->solver == B200UDE_RKC2 && (d->n_stages < 2 || d->n_stages > 64)) why = "RKC2 needs 2 <= n_stages <= 64";
-        else if (d->solver == B200UDE_RKC2 && d->adaptive) why = "RKC2 runs with a fixed step (adaptive = 0)";
+        else if (ark && d->n_consts != 1)
+            why = "adaptive RKC2 needs eigen_est (a bound of the spectral radius of df/du) in consts[0] with n_consts = 1; without it "
+                  "RKC2 runs with a fixed step (adaptive = 0)";
+        else if (ark && !(std::isfinite(d->consts[0]) && d->consts[0] > 0)) why = "adaptive RKC2 needs a finite eigen_est > 0 in consts[0]";
         else if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)) why = "adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1";
     }
     if (why) return fail(nullptr, B200UDE_EINVAL, "create: B200UDE_MODEL_OPERATOR: %s", why);
@@ -745,6 +765,7 @@ OperatorRun operator_run(const b200ude_handle *h, size_t N)
     r.ustep = h->d_ustep; r.dense = h->d_dense; r.partial = h->d_partial; r.tgrid = h->d_tgrid;
     r.usave = h->d_usave;
     r.nacc = h->d_nacc;
+    r.sstep = h->d_sstep;
     r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.n_save = h->n_save; r.max_steps = h->desc.max_steps;
     r.adaptive = h->adaptive ? 1 : 0;
     r.t0 = h->desc.t0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;
@@ -936,6 +957,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         for (int l = 0; l < 5; ++l) oh.acts[l] = l < d->n_layers ? d->acts[l] : 0;
         oh.rkc2 = d->solver == B200UDE_RKC2 ? 1 : 0;
         oh.S = oh.rkc2 ? d->n_stages : 0;
+        oh.rho = oh.rkc2 && d->adaptive ? d->consts[0] : 0.0;
         operator_layout(oh);
     }
     cudaDeviceProp prop;
@@ -1024,7 +1046,11 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                  (want64 || dalloc(h, &h->d_block_loss, (size_t)L2_BLOCKS) == cudaSuccess);
     }
     if (forced) ok = ok && dalloc_real(h, &h->d_forcing, 3 * (size_t)d->consts[1] * N) == cudaSuccess;
-    if (op) ok = ok && dalloc_real(h, &h->d_ops, (size_t)oh.ops_elems) == cudaSuccess && (!oh.rkc2 || dalloc_real(h, &h->d_rkc, op_rkc_len()) == cudaSuccess);
+    // operator RKC2 tables: one block for n_stages; adaptive, one block per stage count 2..n_stages and then beta[0..64]
+    const bool op_ark = op && oh.rkc2 && h->adaptive;
+    const size_t rkc_n = op_ark ? (size_t)(oh.S - 1) * op_rkc_len() + 65 : (size_t)op_rkc_len();
+    if (op) ok = ok && dalloc_real(h, &h->d_ops, (size_t)oh.ops_elems) == cudaSuccess && (!oh.rkc2 || dalloc_real(h, &h->d_rkc, rkc_n) == cudaSuccess);
+    if (op_ark) ok = ok && dalloc(h, &h->d_sstep, (size_t)d->max_steps * N) == cudaSuccess;
     if (ok) ok = cudaMemset(h->d_theta, 0, es * theta_n) == cudaSuccess;
     if (ok && op) {
         // the loss weights in front of the operator block; the operators follow in b200ude_set_operators
@@ -1032,8 +1058,13 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
         for (int c = 0; c < 64; ++c) w64[c] = c < oh.D ? (d->n_loss_weights > 0 ? d->loss_weights[c] : 1.0) : 0.0;
         ok = upload_as(h->d_ops, w64.data(), w64.size(), want64) == cudaSuccess;
         if (ok && oh.rkc2) {
-            std::vector<double> t(op_rkc_len(), 0.0);
-            rkc2_tables64(oh.S, t[0], &t[op_rkc_off(2)], &t[op_rkc_off(3)], &t[op_rkc_off(4)], &t[op_rkc_off(5)], &t[op_rkc_off(0)], &t[op_rkc_off(1)]);
+            std::vector<double> t(rkc_n, 0.0);
+            for (int s = op_ark ? 2 : oh.S; s <= oh.S; ++s) {
+                double *b = &t[op_ark ? (size_t)(s - 2) * op_rkc_len() : 0];
+                rkc2_tables64(s, b[0], &b[op_rkc_off(2)], &b[op_rkc_off(3)], &b[op_rkc_off(4)], &b[op_rkc_off(5)], &b[op_rkc_off(0)], &b[op_rkc_off(1)]);
+            }
+            if (op_ark)
+                for (int s = 2; s <= 64; ++s) t[(size_t)(oh.S - 1) * op_rkc_len() + s] = rkc2_beta64(s);
             ok = upload_as(h->d_rkc, t.data(), t.size(), want64) == cudaSuccess;
         }
     }
@@ -1085,6 +1116,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     h->oh.theta = h->d_theta;
     h->oh.ops = h->d_ops;
     h->oh.rkc = h->d_rkc;
+    h->oh.beta = op_ark ? (const void *)((const unsigned char *)h->d_rkc + es * (size_t)(oh.S - 1) * op_rkc_len()) : nullptr;
     *out = h;
     return B200UDE_OK;
 }
@@ -1101,7 +1133,7 @@ void b200ude_destroy(b200ude_handle *h)
     cudaFree(h->d_adam_m); cudaFree(h->d_adam_v); cudaFree(h->d_adam_t); cudaFree(h->d_train_out);
     cudaFree(h->d_tgrid); cudaFree(h->d_nacc); cudaFree(h->d_cot); cudaFree(h->d_block_loss); cudaFree(h->d_hstep);
     cudaFree(h->d_forcing); cudaFree(h->d_usave);
-    cudaFree(h->d_ops); cudaFree(h->d_rkc);
+    cudaFree(h->d_ops); cudaFree(h->d_rkc); cudaFree(h->d_sstep);
     if (h->h_loss) cudaFreeHost(h->h_loss);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
     if (h->copy_stream) cudaStreamDestroy(h->copy_stream);

@@ -51,6 +51,7 @@ static op::Run<R> make_run(const OperatorHost &h, const OperatorRun &r)
     p.u0 = (const R *)r.u0; p.out = (R *)r.out; p.ustep = (R *)r.ustep; p.dense = (R *)r.dense; p.usave = (R *)r.usave;
     p.status = r.status; p.cot = (const R *)r.cot; p.grad_u0 = (R *)r.grad_u0; p.partial = (R *)r.partial; p.fused_l2 = r.fused_l2;
     p.tgrid = (R *)r.tgrid; p.nacc = r.nacc;
+    p.beta = (const R *)h.beta; p.sstep = r.sstep; p.rho = (R)h.rho;
     p.N = r.N; p.n_steps = r.n_steps; p.save_every = r.save_every; p.n_save = r.n_save; p.max_steps = r.max_steps;
     p.t0 = (R)r.t0; p.dt = (R)r.dt; p.save_dt = (R)r.save_dt; p.abstol = (R)r.abstol; p.reltol = (R)r.reltol;
     return p;
@@ -73,6 +74,7 @@ static cudaError_t fwd(const OperatorHost &h, const OperatorRun &r, cudaStream_t
 {
     const op::Run<R> p = make_run<R>(h, r);
     const size_t smem = operator_smem(h, 0);
+    if (h.rkc2 && r.adaptive) return launch<R>(op::rkc2_adaptive_forward_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
     if (h.rkc2) return launch<R>(op::rkc2_forward_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
     if (r.adaptive) return launch<R>(op::tsit5_adaptive_forward_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
     return launch<R>(op::tsit5_forward_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
@@ -83,6 +85,7 @@ static cudaError_t adj(const OperatorHost &h, const OperatorRun &r, cudaStream_t
 {
     const op::Run<R> p = make_run<R>(h, r);
     const size_t smem = operator_smem(h, h.warps);
+    if (h.rkc2 && r.adaptive) return launch<R>(op::rkc2_adaptive_adjoint_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
     if (h.rkc2) return launch<R>(op::rkc2_adjoint_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
     if (r.adaptive) return launch<R>(op::tsit5_adaptive_adjoint_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
     return launch<R>(op::tsit5_adjoint_kernel<R>, p, h.warps, smem, h.dyn_cap, st);
@@ -93,8 +96,10 @@ int adj_rows_operator(int N, int warps) { return (N + warps - 1) / warps; }
 template <typename R>
 static cudaError_t static_smem(size_t *bytes)
 {
-    void (*kerns[6])(op::Run<R>) = {op::tsit5_forward_kernel<R>, op::tsit5_adjoint_kernel<R>, op::tsit5_adaptive_forward_kernel<R>,
-                                    op::tsit5_adaptive_adjoint_kernel<R>, op::rkc2_forward_kernel<R>, op::rkc2_adjoint_kernel<R>};
+    void (*kerns[8])(op::Run<R>) = {op::tsit5_forward_kernel<R>,         op::tsit5_adjoint_kernel<R>,
+                                    op::tsit5_adaptive_forward_kernel<R>, op::tsit5_adaptive_adjoint_kernel<R>,
+                                    op::rkc2_forward_kernel<R>,          op::rkc2_adjoint_kernel<R>,
+                                    op::rkc2_adaptive_forward_kernel<R>, op::rkc2_adaptive_adjoint_kernel<R>};
     *bytes = 0;
     for (auto k : kerns) {
         cudaFuncAttributes a;

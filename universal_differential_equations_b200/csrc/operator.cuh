@@ -24,7 +24,8 @@
 //
 // Handle records are component-fastest within a trajectory, [row][N][d]; the ABI arrays stay [..][d][N].
 //   Tsit5: dense (6 steps + 1) d N (row s*6 + j = k_j of step s; k_0 of step s = k_6 of step s-1), ustep (steps + 1) d N.
-//   RKC2:  ustep (steps + 1) d N and, in `dense`, f(u_n) (steps + 1) d N.
+//   RKC2:  ustep (steps + 1) d N and, in `dense`, f(u_n) (steps + 1) d N; adaptive RKC2 also the stage count of each
+//          accepted step, sstep [max_steps][N].
 // theta = per layer vec(W) column-major then b (Flux.destructure).
 #pragma once
 #include <cuda_runtime.h>
@@ -54,7 +55,7 @@ struct Run {
     int ops_elems, theta_elems, gstride;   // staged block sizes (elements); gstride: one warp's gradient vector (>= P + 1)
     const R *ops;     // [LW loss weights | D1 (ld1 x M) | D2 (ld2 x D)], ops_elems elements
     const R *theta;   // the handle's theta [P]
-    const R *rkc;     // RKC2 tables (RKC_LEN)
+    const R *rkc;     // RKC2 tables (RKC_LEN; adaptive RKC2: (S - 1) RKC_LEN, the block of s stages at (s - 2) RKC_LEN)
     int S;            // RKC2 stages
     const R *u0;      // [d][N]
     R *out;           // [n_save][d][N]
@@ -67,6 +68,12 @@ struct Run {
     int *nacc;
     int N, n_steps, save_every, n_save, max_steps;
     R t0, dt, save_dt, abstol, reltol;
+    // adaptive RKC2 (appended, so that the fields above keep their parameter offsets): `rkc` then holds one RKC_LEN block per
+    // stage count 2..S, beta[s] is the real stability interval of s stages, sstep [max_steps][N] the stage count of each
+    // accepted step, rho the caller's bound of the spectral radius of df/du (eigen_est)
+    const R *beta;
+    int *sstep;
+    R rho;
 };
 
 template <typename R>
@@ -639,6 +646,202 @@ __global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
             }
             lam = Y1;
             if (s % p.save_every == 0) jump(s / p.save_every);
+        }
+        if (p.grad_u0) stv(p.grad_u0 + n, N, lam, p.D, lane);
+        loss = wsum(loss);
+        if (lane == 0) gw[p.P] = loss;
+    }
+    cta_reduce(p, sm.g);
+}
+
+// The adaptive RKC2 kernels below repeat the stage recurrence of kernels 5 / 6 and the controller of kernel 3 instead of
+// calling shared helpers: moving that code out of the existing kernels would recompile them, and their SASS stays as it was.
+
+// the cubic Hermite interpolant on (a0, g0, a1, g1) over a step of length h at fraction Th (OrdinaryDiffEq's dense output of
+// the ROCK methods; kernel 6 writes the same expression inline)
+template <typename R>
+__device__ __forceinline__ R herm3(R Th, R h, R a0, R a1, R g0, R g1)
+{
+    return ((R)1 - Th) * a0 + Th * a1 + Th * (Th - (R)1) * (((R)1 - (R)2 * Th) * (a1 - a0) + (Th - (R)1) * h * g0 + Th * h * g1);
+}
+
+// ---- 7. adaptive RKC2 forward (ROCK2(eigen_est = rho) without dt, npde.jl:80-84,120-123).  Per attempt the fewest stages
+// s in 2..S with beta(s) >= 1.05 h rho (none: s = S and h = beta(S) / (1.05 rho)), the s-stage recurrence of kernel 5, the
+// error estimate of Sommeijer, Shampine and Verwer est = 0.8 (u_n - u_{n+1}) + 0.4 h (f(u_n) + f(u_{n+1})), kernel 3's PI
+// controller with the order-2 exponents (7/20, 1/5).  Saves from the cubic Hermite interpolant; f(u_{n+1}) is the next
+// step's f(u_n), so an accepted step of s stages costs s right-hand sides.  Records u_n, f(u_n), t_n and s_n ----
+template <typename R>
+__global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
+{
+    using PR = Prec<R>;
+    const Smem<R> sm = carve(p);
+    stage(p, sm.ops, sm.th);
+    const int lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const int traj = blockIdx.x * W + (threadIdx.x >> 5);
+    if (traj >= p.N) return;
+    const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+    const bool on_a = lane < p.D, on_b = lane + 32 < p.D;
+    auto rec = [&](R *b, int row) { return b + ((size_t)row * N + n) * D; };
+    const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
+    const R abstol = p.abstol, reltol = p.reltol, Dr = (R)p.D, rho = p.rho;
+    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)20, beta2 = (R)1 / (R)5;
+    V<R> u = ldv(p.u0 + n, N, p.D, lane), F0, un, F1;
+    stv(p.out + n, N, u, p.D, lane);
+    stv(rec(p.usave, 0), 1, u, p.D, lane);
+    stv(rec(p.ustep, 0), 1, u, p.D, lane);
+    if (lane == 0) p.tgrid[n] = t0;
+    F0 = rhs(p, sm.ops, sm.th, u, lane);
+    stv(rec(p.dense, 0), 1, F0, p.D, lane);
+    auto sq2 = [&](R xa, R xb, R sa, R sb) {
+        const R ea = xa / (abstol + reltol * sa), eb = xb / (abstol + reltol * sb);
+        return (on_a ? ea * ea : (R)0) + (on_b ? eb * eb : (R)0);
+    };
+    R dt;
+    {   // initial step: kernel 3's heuristic at order 2
+        const R d0 = PR::sq(wsum(sq2(u.a, u.b, fabs(u.a), fabs(u.b))) / Dr);
+        const R d1 = PR::sq(wsum(sq2(F0.a, F0.b, fabs(u.a), fabs(u.b))) / Dr);
+        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
+        dt0 = fmin(dt0, t1 - t0);
+        const V<R> g{fma(dt0, F0.a, u.a), fma(dt0, F0.b, u.b)};
+        un = rhs(p, sm.ops, sm.th, g, lane);
+        const R d2 = PR::sq(wsum(sq2(un.a - F0.a, un.b - F0.b, fabs(u.a), fabs(u.b))) / Dr) / dt0;
+        const R dm = fmax(d1, d2);
+        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)3);
+        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+    }
+    R t = t0, qold = (R)1e-4;
+    int nacc = 0, isave = 1, bad = 0;
+    while (isave < p.n_save) {
+        R h = dt;
+        bool clipped = false;
+        if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
+        const R hr = (R)1.05 * h * rho;
+        int s = 2;
+        while (s < p.S && __ldg(p.beta + s) < hr) ++s;
+        if (__ldg(p.beta + s) < hr) {   // even S stages are not stable at h: the step the cap allows
+            h = __ldg(p.beta + s) / ((R)1.05 * rho);
+            clipped = false;
+        }
+        const R *T = p.rkc + (size_t)(s - 2) * RKC_LEN;
+        const R mt1 = __ldg(T);
+        V<R> Y0 = u, Y1{fma(mt1 * h, F0.a, u.a), fma(mt1 * h, F0.b, u.b)};
+        for (int j = 2; j <= s; ++j) {
+            const V<R> F = rhs(p, sm.ops, sm.th, Y1, lane);
+            const R mu = __ldg(T + RKC_MU + j), nu = __ldg(T + RKC_NU + j), mt = __ldg(T + RKC_MT + j), ga = __ldg(T + RKC_GA + j);
+            const R c0 = (R)1 - mu - nu;
+            const V<R> Y2{fma(ga * h, F0.a, fma(mt * h, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * u.a)))),
+                          fma(ga * h, F0.b, fma(mt * h, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * u.b))))};
+            Y0 = Y1;
+            Y1 = Y2;
+        }
+        un = Y1;
+        F1 = rhs(p, sm.ops, sm.th, un, lane);
+        const R ea = fma((R)0.4 * h, F0.a + F1.a, (R)0.8 * (u.a - un.a)), eb = fma((R)0.4 * h, F0.b + F1.b, (R)0.8 * (u.b - un.b));
+        const R EEst = PR::sq(wsum(sq2(ea, eb, fmax(fabs(u.a), fabs(un.a)), fmax(fabs(u.b), fabs(un.b)))) / Dr);
+        if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
+        const R q11 = PR::pw(EEst, beta1);
+        const R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
+        if (EEst <= (R)1) {
+            if (nacc >= p.max_steps) { bad = 2; break; }
+            const R tn = clipped ? t1 : t + h;
+            while (isave < p.n_save) {
+                const R ts = t0 + p.save_dt * (R)isave;
+                if (ts > tn + PR::clip * fabs(tn)) break;
+                const R Th = fmin((ts - t) / h, (R)1);
+                const V<R> us{herm3(Th, h, u.a, un.a, F0.a, F1.a), herm3(Th, h, u.b, un.b, F0.b, F1.b)};
+                stv(p.out + (size_t)isave * D * N + n, N, us, p.D, lane);
+                stv(rec(p.usave, isave), 1, us, p.D, lane);
+                ++isave;
+            }
+            qold = fmax(EEst, (R)1e-4);
+            if (!clipped || h >= dt) dt = h / q;
+            else dt = fmax(dt, h / q);
+            t = tn;
+            if (lane == 0) p.sstep[(size_t)nacc * N + n] = s;
+            ++nacc;
+            if (lane == 0) p.tgrid[(size_t)nacc * N + n] = t;
+            u = un;
+            F0 = F1;
+            stv(rec(p.ustep, nacc), 1, u, p.D, lane);
+            stv(rec(p.dense, nacc), 1, F0, p.D, lane);
+        } else {
+            dt = h / fmin((R)1 / qmin, q11 / gamma);
+        }
+    }
+    if (bad) {   // failed solve: the unreached save points are NaN
+        const V<R> nan{PR::nan(), PR::nan()};
+        for (int is = isave; is < p.n_save; ++is) {
+            stv(p.out + (size_t)is * D * N + n, N, nan, p.D, lane);
+            stv(rec(p.usave, is), 1, nan, p.D, lane);
+        }
+    }
+    const bool ok = warp_finite(u);
+    if (lane == 0) {
+        p.nacc[n] = nacc;
+        if (p.status) p.status[n] = bad == 2 ? 2 : ((bad || !ok) ? 1 : 0);
+    }
+}
+
+// ---- 8. replay adjoint of an adaptive RKC2 solve: each accepted step split at the save times inside it (kernel 4); a piece
+// of length h' <= h_n steps lambda back with RKC2 of the step's recorded s_n stages (stable: h' rho <= h_n rho), stage j at
+// cur - c_j h' with u from the step's Hermite interpolant, the theta-gradient with the quadrature weights h' w_j (kernel 6 with
+// dt -> h'); the save cotangents at the saved states the forward recorded ----
+template <typename R>
+__global__ void __launch_bounds__(128) rkc2_adaptive_adjoint_kernel(Run<R> p)
+{
+    using PR = Prec<R>;
+    const Smem<R> sm = carve(p);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
+    R *gw = sm.g + (size_t)warp * p.gstride;
+    for (int q = lane; q < p.P + 1; q += 32) gw[q] = (R)0;
+    stage(p, sm.ops, sm.th);
+    const int traj = blockIdx.x * W + warp;
+    if (traj < p.N) {
+        const size_t N = (size_t)p.N, n = (size_t)traj, D = (size_t)p.D;
+        auto rec = [&](const R *b, int row) { return b + ((size_t)row * N + n) * D; };
+        const int nacc = p.nacc[n];
+        V<R> lam{(R)0, (R)0};
+        R loss = (R)0;
+        auto jump = [&](int is) { save_jump(p, sm.ops, is, ldv(rec(p.usave, is), 1, p.D, lane), lam, loss, n, lane); };
+        int isave = p.n_save - 1;
+        jump(isave);
+        --isave;
+        for (int st = nacc - 1; st >= 0; --st) {
+            const R tn = p.tgrid[(size_t)st * N + n], tn1 = p.tgrid[(size_t)(st + 1) * N + n], hn = tn1 - tn;
+            const R eps = PR::eta * hn;
+            const V<R> y0 = ldv(rec(p.ustep, st), 1, p.D, lane), y1 = ldv(rec(p.ustep, st + 1), 1, p.D, lane);
+            const V<R> f0 = ldv(rec(p.dense, st), 1, p.D, lane), f1 = ldv(rec(p.dense, st + 1), 1, p.D, lane);
+            const int s = p.sstep[(size_t)st * N + n];
+            const R *T = p.rkc + (size_t)(s - 2) * RKC_LEN;
+            const R mt1 = __ldg(T);
+            R cur = tn1;
+            while (cur > tn + eps) {
+                const R ts = p.t0 + p.save_dt * (R)isave;
+                const R ta = (isave >= 0 && ts > tn + eps) ? ts : tn;
+                const R h = cur - ta;
+                V<R> Y0 = lam, Y1 = lam, F0{(R)0, (R)0};
+                for (int j = 0; j < s; ++j) {
+                    const R Th = fmin(fmax((cur - __ldg(T + RKC_C + j) * h - tn) / hn, (R)0), (R)1);
+                    const V<R> x{herm3(Th, hn, y0.a, y1.a, f0.a, f1.a), herm3(Th, hn, y0.b, y1.b, f0.b, f1.b)};
+                    const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, j == 0 ? lam : Y1, h * __ldg(T + RKC_W + j), gw, lane);
+                    if (j == 0) {
+                        F0 = F;
+                        Y0 = lam;
+                        Y1 = V<R>{fma(mt1 * h, F0.a, lam.a), fma(mt1 * h, F0.b, lam.b)};
+                    } else {
+                        const R mu = __ldg(T + RKC_MU + j + 1), nu = __ldg(T + RKC_NU + j + 1), mt = __ldg(T + RKC_MT + j + 1),
+                                ga = __ldg(T + RKC_GA + j + 1);
+                        const R c0 = (R)1 - mu - nu;
+                        const V<R> Y2{fma(ga * h, F0.a, fma(mt * h, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * lam.a)))),
+                                      fma(ga * h, F0.b, fma(mt * h, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * lam.b))))};
+                        Y0 = Y1;
+                        Y1 = Y2;
+                    }
+                }
+                lam = Y1;
+                cur = ta;
+                if (isave >= 0 && fabs(ts - ta) <= eps) { jump(isave); --isave; }
+            }
         }
         if (p.grad_u0) stv(p.grad_u0 + n, N, lam, p.D, lane);
         loss = wsum(loss);

@@ -264,20 +264,22 @@ struct OperatorHost {
     // staged layout (operator_layout): odd leading dimensions, offsets, block sizes in elements
     int ld1, ld2, woff[5], soff[5], ldw[5], ops_elems, theta_elems, gstride;
     const void *ops;          // [64 loss weights | D1 (ld1 x M) | D2 (ld2 x D)], ops_elems elements
-    const void *theta, *rkc;  // the handle's theta, RKC2 tables
+    const void *theta, *rkc;  // the handle's theta, RKC2 tables (adaptive RKC2: one block per stage count 2..S)
+    const void *beta;         // adaptive RKC2: the real stability interval of s stages at index s (0..64)
+    double rho;               // adaptive RKC2: eigen_est, the bound of the spectral radius of df/du (desc.consts[0])
 };
 struct OperatorRun {
     const void *u0, *cot;
     void *out, *ustep, *dense, *usave, *grad_u0, *partial, *tgrid;
     int32_t *status;
-    int *nacc;
+    int *nacc, *sstep;        // adaptive: accepted steps; adaptive RKC2: the stage count of each [max_steps][N]
     int N, n_steps, save_every, n_save, max_steps, fused_l2, adaptive;
     double t0, dt, save_dt, abstol, reltol;
 };
 void operator_layout(OperatorHost &);                      // fills P and the staged layout from D, M, L, widths
 size_t operator_smem(const OperatorHost &, int warps);     // dynamic shared memory of a CTA (warps = 0: the forward kernels)
 int adj_rows_operator(int N, int warps);
-cudaError_t operator_static_smem(int dtype, size_t *bytes);   // the largest static shared memory of the dtype's six kernels (current device)
+cudaError_t operator_static_smem(int dtype, size_t *bytes);   // the largest static shared memory of the dtype's eight kernels (current device)
 cudaError_t launch_fwd_operator(const OperatorHost &, const OperatorRun &, cudaStream_t);
 cudaError_t launch_adj_operator(const OperatorHost &, const OperatorRun &, cudaStream_t, int *rows_out);
 

@@ -333,7 +333,11 @@ class RKC2:
     `ROCK2(eigen_est = ...)` (Climate/NeuralPDE/npde.jl:61,82; named by the north star for the stiff Fisher-KPP grid):
     same class of method (explicit, stability interval growing with the square of the stage count), closed-form
     coefficients (ROCK2's tables are not in the reference).  Give `stages`, or `eigen_est` (an upper bound of the spectral
-    radius of the RHS Jacobian, as the reference's ROCK2 call does) from which the stage count is chosen for the step."""
+    radius of the RHS Jacobian, as the reference's ROCK2 call does) from which the stage count is chosen for the step.
+
+    Adaptive (concrete_solve without dt) on an OperatorUDE: `eigen_est` is required; every step takes the fewest stages, up to
+    `stages` (default 64), whose stability interval covers 1.05 h eigen_est, and an embedded error estimate with a PI controller
+    picks h from abstol / reltol."""
     code = _lib.RKC2
 
     def __init__(self, stages=None, eigen_est=None):
@@ -442,11 +446,19 @@ class UDESolver:
         d.n_prefix = getattr(f, "trainable_rates", 0)
         d.n_suffix = getattr(f, "n_suffix", 0)
         cs = f.consts()
+        # adaptive RKC2 on the operator model: each step takes the fewest stages (up to `stages`, default 64) that are stable
+        # for its h * eigen_est, so eigen_est travels in consts[0] instead of fixing one stage count for dt
+        ark = bool(adaptive) and isinstance(alg, RKC2) and alg.eigen_est is not None and f.model == _lib.MODEL_OPERATOR
+        if ark:
+            cs = tuple(cs) + (float(alg.eigen_est),)
         d.n_consts = len(cs)
         for i, c in enumerate(cs):
             d.consts[i] = c
         d.solver = alg.code
-        d.n_stages = alg.n_stages(float(dt)) if isinstance(alg, RKC2) else 0
+        if ark:
+            d.n_stages = int(alg.stages) if alg.stages is not None else 64
+        else:
+            d.n_stages = alg.n_stages(float(dt)) if isinstance(alg, RKC2) else 0
         d.sensealg = sensealg.code
         d.t0, d.dt, d.n_steps, d.save_every = self.t0, self.dt, self.n_steps, self.save_every
         if loss_weights is not None:
@@ -728,7 +740,8 @@ def concrete_solve(prob, alg, u0=None, p=None, *, saveat=None, dt=None, adaptive
     `prob` may be an ODEProblem (u0[d] -> d x n_save, like Julia's Array(sol)) or an
     EnsembleProblem (u0s[d, N] -> n_save x d x N).  Differentiable w.r.t. p and u0.
     adaptive defaults to true when no dt is given (as in OrdinaryDiffEq): Tsit5 with the PI controller and
-    abstol / reltol (defaults 1e-6 / 1e-3); pass dt= for adaptive=false.
+    abstol / reltol (defaults 1e-6 / 1e-3), or on an OperatorUDE RKC2 / ROCK2(eigen_est=...) with the stage count of each
+    step chosen from eigen_est; pass dt= for adaptive=false.
     A ForcedNeuralODE takes its forcing coefficients [3J, N] as `forcing` and returns d + r rows per save.
     """
     ens = isinstance(prob, EnsembleProblem)
