@@ -8,8 +8,8 @@
 // (u0, out, cot, grad_u0) trajectory-fastest [row][point][trajectory]; tgrid [max_steps+1][N] and nacc [N] as in the other
 // adaptive kernels.
 //
-// The controller is the one of generic::adaptive_forward_kernel (PI, gamma 0.9, qmin 1/5, qmax 10, beta1 7/50, beta2 2/25, no
-// dead band, Hairer initial step, last step clipped to t1, saveat from the free interpolant).  The error norm -- and d0 / d1 / d2
+// The controller is PIControl<R, 5> (step_control.cuh: OrdinaryDiffEq's PI controller and Hairer initial step), the last step
+// clipped to t1, saveat from the free interpolant.  The error norm -- and d0 / d1 / d2
 // of the initial step -- is OrdinaryDiffEq's default norm over the whole trajectory, sqrt(sum_i (e_i / sc_i)^2 / Nx).  Every thread
 // of a trajectory sums the same Nx shared-memory terms in point order, so all of them hold the same bits, take the same
 // accept / reject decision and keep the same (t, dt, qold, nacc, isave); the result does not depend on which slot of the CTA the
@@ -130,7 +130,6 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
     const size_t N = (size_t)p.N, n = (size_t)(live ? traj : p.N - 1);
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)50, beta2 = (R)2 / (R)25;
     const R ttol = Prec<R>::clip;   // relative slack of the clip / save-time tests (as in the one-thread kernels)
     const R big = Prec<R>::huge;
     const int sx = Ops::P() - 5;
@@ -141,7 +140,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
         const R y = point_chain<Ops>(g);
         return fma(D0, fma(w1, gm, fma(w2, g, w3 * gp)), y);
     };
-    auto rms = [&](R v) { return sqrt(traj_sum(sE, slot, base, Nx, valid, v) / (R)Nx); };
+    auto rms = [&](R v) { return Prec<R>::sq(traj_sum(sE, slot, base, Nx, valid, v) / (R)Nx); };
     auto store_int = [&](R *b, int row, R v) { if (live) b[((size_t)row * N + n) * Nx + i] = v; };
     auto store_abi = [&](R *b, int row, R v) { if (live) b[((size_t)row * Nx + i) * N + n] = v; };
 
@@ -153,25 +152,22 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
     k[0] = rhs(u);
     store_int(p.dense, 0, k[0]);
     // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq, norms over the trajectory
-    R dt;
+    PIControl<R, 5> pi;
     {
         const R sk = abstol + reltol * fabs(u);
         const R d0 = rms((u / sk) * (u / sk));
         const R d1 = rms((k[0] / sk) * (k[0] / sk));
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         const R f1 = rhs(fma(dt0, k[0], u));
         const R e = (f1 - k[0]) / sk;
         const R d2 = rms(e * e) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : exp10(-((R)2 + log10(dm)) / (R)5);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     bool done = !live || isave >= p.n_save;   // uniform over the trajectory's threads
     while (__syncthreads_or(!done)) {
-        R h = done ? (R)0 : dt;
+        R h = done ? (R)0 : pi.dt;
         bool clipped = false;
         if (!done && t + h >= t1 - ttol * fabs(t1)) { h = t1 - t; clipped = true; }
         R un = u;
@@ -187,15 +183,13 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
         }
         R e = (R)0;
 #pragma unroll
-        for (int j = 0; j < 7; ++j) e = fma(generic::tsit5_btilde<R>(j), k[j], e);
+        for (int j = 0; j < 7; ++j) e = fma((R)Tsit5::bt(j), k[j], e);
         e *= h;
         const R sc = abstol + reltol * fmax(fabs(u), fabs(un));
         const R EEst = rms((e / sc) * (e / sc));
         if (done) continue;
         if (!(EEst <= big)) { bad = 1; done = true; continue; }   // NaN / Inf
-        const R q11 = pow(EEst, beta1);
-        const R q = fmin(fmax(q11 / pow(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= p.max_steps) { bad = 2; done = true; continue; }
             const R tn = clipped ? t1 : t + h;
             // dense record of this step: k_1..k_6 at rows nacc*6 + st, k_7 at (nacc+1)*6 (= k_1 of the next step)
@@ -204,17 +198,14 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
                 const R ts = t0 + p.save_dt * (R)isave;
                 if (ts > tn + ttol * fabs(tn)) break;
                 R bw[7];
-                generic::tsit5_bw_rt(fmin((ts - t) / h, (R)1), bw);
+                Tsit5::weights(fmin((ts - t) / h, (R)1), bw);
                 R acc = (R)0;
 #pragma unroll
                 for (int j = 0; j < 7; ++j) acc = fma(bw[j], k[j], acc);
                 store_abi(p.out, isave, fma(h, acc, u));
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq: no dead band
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = tn;
             ++nacc;
             if (live && i == 0) p.tgrid[(size_t)nacc * N + n] = t;
@@ -223,7 +214,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
             store_int(p.ustep, nacc, u);
             if (isave >= p.n_save) done = true;
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
         }
     }
     if (bad && live) {   // failed solve (non-finite error estimate / max_steps): the unreached save points are NaN
@@ -292,7 +283,7 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
                 R x = u_n;
                 if (act_s) {
                     R bw[7];
-                    generic::tsit5_bw_rt(fmin(fmax((cur - (R)Tsit5::c(st) * h - tn) / hn, (R)0), (R)1), bw);
+                    Tsit5::weights(fmin(fmax((cur - (R)Tsit5::c(st) * h - tn) / hn, (R)0), (R)1), bw);
                     R acc = (R)0;
 #pragma unroll
                     for (int j = 0; j < 7; ++j) acc = fma(bw[j], p.dense[((size_t)(sc_ * 6 + j) * N + n) * Nx + i], acc);

@@ -10,10 +10,9 @@
 // threads of a trajectory hold the same bits and take the same decisions.  The attempt loop of the forward and the step loop of
 // the adjoint run while any thread of the CTA still has work: every thread executes the same barrier sequence.
 //
-// Forward: the controller of generic::vern7_adaptive_forward_kernel (ude_generic.cuh) -- 10 stages, error
-// from btilde, PI with gamma 0.9, qmin 1/5, qmax 10, beta1 7/70, beta2 2/35, Hairer initial step with the order-7 exponent, no
-// FSAL (k_1 kept after a rejection), save times are tstops: a step is clipped to the next save time and out[isave] is the
-// step-end state.  The record is the one the discrete adjoint needs and nothing more: ustep [nacc+1][N][Nx] (point-fastest),
+// Forward: the stepping of generic::vern7_adaptive_forward_kernel (ude_generic.cuh) -- 10 stages, error from btilde,
+// PIControl<R, 7> (step_control.cuh), no FSAL (k_1 kept after a rejection), save times are tstops: a step is clipped to the
+// next save time and out[isave] is the step-end state.  The record is the one the discrete adjoint needs and nothing more: ustep [nacc+1][N][Nx] (point-fastest),
 // hstep [max_steps][N] (the h the step used: t_{n+1} - t_n is not bitwise h_n), tgrid [max_steps+1][N], nacc [N].
 //
 // Adjoint: the recurrence of discrete_adjoint.cuh per accepted step n, walking backwards --
@@ -85,7 +84,6 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
     const size_t N = (size_t)p.N, n = (size_t)(live ? traj : p.N - 1);
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)70, beta2 = (R)2 / (R)35;   // order 7
     const R ttol = Prec<R>::clip;   // relative slack of the clip test (as in the one-thread kernels)
     const R big = Prec<R>::huge;
     const int sx = Ops::P() - 5;
@@ -95,7 +93,7 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
         fkpp_adapt::exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
         return rhs_point<Ops>(g, gm, gp, w1, w2, w3, D0);
     };
-    auto rms = [&](R v) { return sqrt(fkpp_adapt::traj_sum(sE, slot, base, Nx, valid, v) / (R)Nx); };
+    auto rms = [&](R v) { return Prec<R>::sq(fkpp_adapt::traj_sum(sE, slot, base, Nx, valid, v) / (R)Nx); };
     auto store_int = [&](R *b, int row, R v) { if (live) b[((size_t)row * N + n) * Nx + i] = v; };
     auto store_abi = [&](R *b, int row, R v) { if (live) b[((size_t)row * Nx + i) * N + n] = v; };
 
@@ -106,27 +104,24 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
     R k[10];
     k[0] = rhs(u);
     // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq, order-7 exponent, norms over the trajectory
-    R dt;
+    PIControl<R, 7> pi;
     {
         const R sk = abstol + reltol * fabs(u);
         const R d0 = rms((u / sk) * (u / sk));
         const R d1 = rms((k[0] / sk) * (k[0] / sk));
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         const R f1 = rhs(fma(dt0, k[0], u));
         const R e = (f1 - k[0]) / sk;
         const R d2 = rms(e * e) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : exp10(-((R)2 + log10(dm)) / (R)7);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     bool done = !live || isave >= p.n_save;   // uniform over the trajectory's threads
     bool have_k1 = true;                      // not FSAL: k_1 = f(u) is re-evaluated after an accepted step
     while (__syncthreads_or(!done)) {
         const R tend = p.t0 + p.save_dt * (R)isave;
-        R h = done ? (R)0 : dt;
+        R h = done ? (R)0 : pi.dt;
         bool clipped = false;
         if (!done && t + h >= tend - ttol * fabs(tend)) { h = tend - t; clipped = true; }
         // CTA-uniform condition: a trajectory that still holds k_1 re-evaluates it to the same bits (u has not changed); a finished
@@ -152,9 +147,7 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
         const R EEst = rms((e / sc) * (e / sc));
         if (done) continue;
         if (!(EEst <= big)) { bad = 1; done = true; continue; }   // NaN / Inf
-        const R q11 = pow(EEst, beta1);
-        const R q = fmin(fmax(q11 / pow(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= p.max_steps) { bad = 2; done = true; continue; }
             if (live && i == 0) p.hstep[(size_t)nacc * N + n] = h;
             ++nacc;
@@ -162,10 +155,7 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
                 store_abi(p.out, isave, un);
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq: no dead band
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = clipped ? tend : t + h;
             if (live && i == 0) p.tgrid[(size_t)nacc * N + n] = t;
             store_int(p.ustep, nacc, un);
@@ -173,7 +163,7 @@ __global__ void __launch_bounds__(256) vern7_forward_kernel(Fwd<typename Ops::re
             have_k1 = false;
             if (isave >= p.n_save) done = true;
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
             have_k1 = true;
         }
     }

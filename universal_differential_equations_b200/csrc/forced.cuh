@@ -330,7 +330,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(Adj<typename B::real>
     for (int q = lane; q < P + 1; q += 32) dst[q] = gw[q];
 }
 
-// PI-controlled Tsit5 as generic::adaptive_forward_kernel (OrdinaryDiffEq's defaults, saves from the free interpolant), with the
+// PI-controlled Tsit5 as generic::adaptive_forward_kernel (PIControl, saves from the free interpolant), with the
 // stage times and the readout rows
 template <class B, int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename B::real> p, Adapt<typename B::real> ap)
@@ -346,7 +346,6 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
     f.load(p.forcing, J, p.fstride, n);
     const R t0 = ap.t0, t1 = ap.t0 + ap.save_dt * (R)(ap.n_save - 1);
     const R abstol = ap.abstol, reltol = ap.reltol;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)50, beta2 = (R)2 / (R)25;
     R u[MAXD], un[MAXD], g[MAXD], k[7][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     auto store = [&](R *base, int row, const R *v) {
@@ -358,7 +357,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
     ap.tgrid[n] = t0;
     rhs<B>(u, f(t0, J), k[0]);
     store(p.dense, 0, k[0]);
-    R dt;
+    PIControl<R, 5> pi;
     {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq (f at t0 + dt0 for the second derivative estimate)
         R d0 = 0, d1 = 0, d2 = 0;
         for (int c = 0; c < D; ++c) {
@@ -367,8 +366,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
             d1 += (k[0][c] / sk) * (k[0][c] / sk);
         }
         d0 = PR::sq(d0 / D); d1 = PR::sq(d1 / D);
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         for (int c = 0; c < D; ++c) g[c] = fma(dt0, k[0][c], u[c]);
         rhs<B>(g, f(t0 + dt0, J), un);
         for (int c = 0; c < D; ++c) {
@@ -377,14 +375,12 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
             d2 += e * e;
         }
         d2 = PR::sq(d2 / D) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)5);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     while (isave < ap.n_save) {
-        R h = dt;
+        R h = pi.dt;
         bool clipped = false;
         if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
 #pragma unroll
@@ -403,16 +399,14 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
         for (int c = 0; c < D; ++c) {
             R e = (R)0;
 #pragma unroll
-            for (int j = 0; j < 7; ++j) e = fma(generic::tsit5_btilde<R>(j), k[j][c], e);
+            for (int j = 0; j < 7; ++j) e = fma((R)Tsit5::bt(j), k[j][c], e);
             e *= h;
             const R sc = abstol + reltol * fmax(fabs(u[c]), fabs(un[c]));
             ee += (e / sc) * (e / sc);
         }
         const R EEst = PR::sq(ee / D);
         if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
-        const R q11 = PR::pw(EEst, beta1);
-        R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= ap.max_steps) { bad = 2; break; }
             const R tn = clipped ? t1 : t + h;
             for (int i = 1; i < 7; ++i) store(p.dense, nacc * 6 + i, k[i]);
@@ -420,7 +414,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
                 const R ts = t0 + ap.save_dt * (R)isave;
                 if (ts > tn + PR::clip * fabs(tn)) break;
                 R bw[7], us[MAXD];
-                generic::tsit5_bw_rt(fmin((ts - t) / h, (R)1), bw);
+                Tsit5::weights(fmin((ts - t) / h, (R)1), bw);
                 for (int c = 0; c < D; ++c) {
                     R acc = (R)0;
 #pragma unroll
@@ -431,16 +425,14 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(Fwd<typename
                 store(p.usave, isave, us);
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = tn;
             ++nacc;
             ap.tgrid[(size_t)nacc * N + n] = t;
             for (int c = 0; c < D; ++c) { u[c] = un[c]; k[0][c] = k[6][c]; }
             store(p.ustep, nacc, u);
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
         }
     }
     if (bad) {   // failed solve: the unreached save points are NaN, states and readout
@@ -515,7 +507,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_adjoint_kernel(Adj<typename
             for (int i = 0; i < 6; ++i) {
                 R bw[7];
                 const R Th = fmin(fmax((cur - (R)Tsit5::c(i) * h - tn) / hn, (R)0), (R)1);
-                generic::tsit5_bw_rt(Th, bw);
+                Tsit5::weights(Th, bw);
                 for (int c = 0; c < D; ++c) {
                     R acc = (R)0;
 #pragma unroll

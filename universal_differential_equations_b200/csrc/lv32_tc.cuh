@@ -15,6 +15,7 @@
 // discrete adjoint; gradient GEMM on the FMA pipe or on mma.sync).
 #pragma once
 #include "lv32_packed.cuh"
+#include "step_control.cuh"
 #include "ude_adjoint.cuh"
 
 namespace b200ude {
@@ -246,23 +247,11 @@ __global__ void __launch_bounds__(BLOCK, MINB) forward_kernel(FwdParams p)
 }
 
 // ---- adaptive forward kernel (abstol / reltol; scenario_1.jl:84-85, seir_exposure.jl:138-139 style calls) --------------
-// Tsit5 with OrdinaryDiffEq's PI controller and initial-step heuristic per trajectory (same algorithm as
-// generic::adaptive_forward_kernel / the oracle's ude_solve_adaptive), saveat by the free interpolant, and the record of
+// Tsit5 with OrdinaryDiffEq's PI controller and initial-step heuristic per trajectory (PIControl, step_control.cuh; the
+// oracle's ude_solve_adaptive), saveat by the free interpolant, and the record of
 // accepted steps (tgrid, ustep, the stage derivatives) that the replay adjoint reads.  The 32 x 32 sweeps are CTA-collective,
 // so the attempt loop is CTA-uniform: a trajectory that has reached the end keeps evaluating (results discarded) until the
 // slowest of the CTA's 128 trajectories is done.
-__device__ __forceinline__ float tsit5_btilde_rt(int j)
-{
-    return j == 0 ? -0.001780011052225777f : j == 1 ? -0.0008164344596567469f : j == 2 ? 0.007880878010261995f
-         : j == 3 ? -0.1447110071732629f : j == 4 ? 0.5823571654525552f : j == 5 ? -0.45808210592918697f : 0.015151515151515152f;
-}
-__device__ __forceinline__ void tsit5_weights_fwd(float Th, float (&bw)[7])
-{
-    bw[0] = Th * ((float)Tsit5::r(0, 1) + Th * ((float)Tsit5::r(0, 2) + Th * ((float)Tsit5::r(0, 3) + Th * (float)Tsit5::r(0, 4))));
-#pragma unroll
-    for (int j = 1; j < 7; ++j) bw[j] = Th * Th * ((float)Tsit5::r(j, 2) + Th * ((float)Tsit5::r(j, 3) + Th * (float)Tsit5::r(j, 4)));
-}
-
 template <int TM, int BLOCK, int MINB>
 __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams p, AdaptiveGrid ag)
 {
@@ -278,7 +267,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams
     const size_t n = live ? (size_t)gid : (size_t)(p.N - 1);   // padding threads shadow the last trajectory; stores masked
     const float t0 = ag.t0, t1 = ag.t0 + ag.save_dt * (float)(ag.n_save - 1);
     const float abstol = ag.abstol, reltol = ag.reltol;
-    const float gamma = 0.9f, qmin = 0.2f, qmax = 10.0f, beta1 = 7.0f / 50.0f, beta2 = 2.0f / 25.0f;
     float u0 = __ldg(p.u0 + n), u1 = __ldg(p.u0 + N + n);
     auto store2 = [&](float *base, int row, float v0, float v1) {
         if (live) {
@@ -293,35 +281,32 @@ __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams
     float k0[7], k1[7];
 #pragma unroll
     for (int j = 0; j < 7; ++j) { k0[j] = 0.f; k1[j] = 0.f; }
+    PIControl<float, 5> pi;
     {
         const float2 kk = rhs_tc<TM>(&c, sBhi, sBlo, u0, u1, 0);
         k0[0] = kk.x; k1[0] = kk.y;
     }
     store2(p.dense, 0, k0[0], k1[0]);
     // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
-    float dt;
     {
         const float s0 = abstol + reltol * fabsf(u0), s1 = abstol + reltol * fabsf(u1);
-        float d0 = sqrtf(0.5f * ((u0 / s0) * (u0 / s0) + (u1 / s1) * (u1 / s1)));
-        float d1 = sqrtf(0.5f * ((k0[0] / s0) * (k0[0] / s0) + (k1[0] / s1) * (k1[0] / s1)));
-        float dt0 = (d0 < 1e-5f || d1 < 1e-5f) ? 1e-6f : 0.01f * d0 / d1;
-        dt0 = fminf(dt0, t1 - t0);
+        float d0 = Prec<float>::sq(0.5f * ((u0 / s0) * (u0 / s0) + (u1 / s1) * (u1 / s1)));
+        float d1 = Prec<float>::sq(0.5f * ((k0[0] / s0) * (k0[0] / s0) + (k1[0] / s1) * (k1[0] / s1)));
+        const float dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         const float2 f1 = rhs_tc<TM>(&c, sBhi, sBlo, fmaf(dt0, k0[0], u0), fmaf(dt0, k1[0], u1), 1);
         const float e0 = (f1.x - k0[0]) / s0, e1 = (f1.y - k1[0]) / s1;
-        const float d2 = sqrtf(0.5f * (e0 * e0 + e1 * e1)) / dt0;
-        const float dm = fmaxf(d1, d2);
-        const float dt1 = dm <= 1e-15f ? fmaxf(1e-6f, dt0 * 1e-3f) : exp10f(-(2.0f + log10f(dm)) / 5.0f);
-        dt = fminf(fminf(100.0f * dt0, dt1), t1 - t0);
+        const float d2 = Prec<float>::sq(0.5f * (e0 * e0 + e1 * e1)) / dt0;
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    float t = t0, qold = 1e-4f;
+    float t = t0;
     int nacc = 0, isave = 1, bad = 0;
 #pragma unroll 1
     while (true) {
         const bool active = (isave < ag.n_save) && !bad;
         if (!__syncthreads_or(active ? 1 : 0)) break;
-        float h = dt;
+        float h = pi.dt;
         bool clipped = false;
-        if (t + h >= t1 - 1e-6f * fabsf(t1)) { h = t1 - t; clipped = true; }
+        if (t + h >= t1 - Prec<float>::clip * fabsf(t1)) { h = t1 - t; clipped = true; }
         if (!active) h = 0.0f;
         float un0 = u0, un1 = u1;
 #pragma unroll 1
@@ -359,16 +344,14 @@ __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams
         if (active) {
             float e0 = 0.0f, e1 = 0.0f;
 #pragma unroll
-            for (int j = 0; j < 7; ++j) { e0 = fmaf(tsit5_btilde_rt(j), k0[j], e0); e1 = fmaf(tsit5_btilde_rt(j), k1[j], e1); }
+            for (int j = 0; j < 7; ++j) { e0 = fmaf((float)Tsit5::bt(j), k0[j], e0); e1 = fmaf((float)Tsit5::bt(j), k1[j], e1); }
             e0 *= h; e1 *= h;
             const float c0 = abstol + reltol * fmaxf(fabsf(u0), fabsf(un0)), c1 = abstol + reltol * fmaxf(fabsf(u1), fabsf(un1));
-            const float EEst = sqrtf(0.5f * ((e0 / c0) * (e0 / c0) + (e1 / c1) * (e1 / c1)));
-            if (!(EEst <= 3.0e38f)) {
+            const float EEst = Prec<float>::sq(0.5f * ((e0 / c0) * (e0 / c0) + (e1 / c1) * (e1 / c1)));
+            if (!(EEst <= Prec<float>::huge)) {
                 bad = 1;   // NaN / Inf
             } else {
-                const float q11 = powf(EEst, beta1);
-                float q = fminf(fmaxf(q11 / powf(qold, beta2) / gamma, 1.0f / qmax), 1.0f / qmin);
-                if (EEst <= 1.0f) {
+                if (pi.judge(EEst)) {
                     if (nacc >= ag.max_steps) {
                         bad = 2;
                     } else {
@@ -379,19 +362,16 @@ __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams
 #undef B200UDE_ST
                         while (isave < ag.n_save) {
                             const float ts = t0 + ag.save_dt * (float)isave;
-                            if (ts > tn + 1e-6f * fabsf(tn)) break;
+                            if (ts > tn + Prec<float>::clip * fabsf(tn)) break;
                             float bw[7];
-                            tsit5_weights_fwd(fminf((ts - t) / h, 1.0f), bw);
+                            Tsit5::weights(fminf((ts - t) / h, 1.0f), bw);
                             float a0 = 0.0f, a1 = 0.0f;
 #pragma unroll
                             for (int j = 0; j < 7; ++j) { a0 = fmaf(bw[j], k0[j], a0); a1 = fmaf(bw[j], k1[j], a1); }
                             store2(p.out, isave, fmaf(h, a0, u0), fmaf(h, a1, u1));
                             ++isave;
                         }
-                        qold = fmaxf(EEst, 1e-4f);
-                        // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq (the 6/5 band is the implicit-solver default): no dead band
-                        if (!clipped || h >= dt) dt = h / q;
-                        else dt = fmaxf(dt, h / q);
+                        pi.accept(EEst, h, clipped);
                         t = tn;
                         ++nacc;
                         if (live) ag.tgrid[(size_t)nacc * N + n] = t;
@@ -400,17 +380,17 @@ __global__ void __launch_bounds__(BLOCK, MINB) adaptive_forward_kernel(FwdParams
                         store2(p.ustep, nacc, u0, u1);
                     }
                 } else {
-                    dt = h / fminf(1.0f / qmin, q11 / gamma);
+                    pi.reject(h);
                 }
             }
         }
     }
     if (bad) {   // failed solve: the unreached save points are NaN
-        for (int is = isave; is < ag.n_save; ++is) store2(p.out, is, __int_as_float(0x7fc00000), __int_as_float(0x7fc00000));
+        for (int is = isave; is < ag.n_save; ++is) store2(p.out, is, Prec<float>::nan(), Prec<float>::nan());
     }
     if (live) ag.nacc[n] = nacc;
     if (p.status && live) {
-        const bool ok = (fabsf(u0) <= 3.0e38f) && (fabsf(u1) <= 3.0e38f);
+        const bool ok = (fabsf(u0) <= Prec<float>::huge) && (fabsf(u1) <= Prec<float>::huge);
         p.status[n] = bad == 2 ? 2 : ((bad || !ok) ? 1 : 0);
     }
 }
@@ -425,14 +405,6 @@ struct __align__(16) WarpStageT {
     float SG[32 * 2];     // scaled, masked chain-output cotangent  [lane][m]
     float U[32 * 2];      // chain input                            [lane][m]
 };
-
-// weights b_j(Theta) of Tsit5's free 4th-order interpolant for a run-time Theta
-__device__ __forceinline__ void tsit5_weights(float Th, float (&bw)[7])
-{
-    bw[0] = Th * ((float)Tsit5::r(0, 1) + Th * ((float)Tsit5::r(0, 2) + Th * ((float)Tsit5::r(0, 3) + Th * (float)Tsit5::r(0, 4))));
-#pragma unroll
-    for (int j = 1; j < 7; ++j) bw[j] = Th * Th * ((float)Tsit5::r(j, 2) + Th * ((float)Tsit5::r(j, 3) + Th * (float)Tsit5::r(j, 4)));
-}
 
 // warp-level m16n8k8 TF32 MMA (legacy tensor-core path), D += A B
 __device__ __forceinline__ void mma_m16n8k8(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2])
@@ -779,7 +751,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) adjoint_kernel(AdjParams p, Adapt
                 {   // u at time cur - c_i h from the dense output of forward step sc_ (free 4th-order interpolant)
                     const float Th = fminf(fmaxf((cur - ci * h - tn) * inv_hn, 0.0f), 1.0f);
                     float bw[7];
-                    tsit5_weights(Th, bw);
+                    Tsit5::weights(Th, bw);
                     float a0 = 0.0f, a1 = 0.0f;
 #pragma unroll
                     for (int j = 0; j < 7; ++j) {

@@ -388,7 +388,7 @@ __global__ void __launch_bounds__(128) tsit5_adjoint_kernel(Run<R> p)
 }
 
 // ---- 3. adaptive Tsit5 forward: OrdinaryDiffEq's PI controller and initial step, saves from the free interpolant
-// (generic::adaptive_forward_kernel on one warp).  The norms are butterflies, so every decision is warp-uniform ----
+// (PIControl on one warp).  The norms are butterflies, so every decision is warp-uniform ----
 template <typename R>
 __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
 {
@@ -403,7 +403,6 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
     auto rec = [&](R *b, int row) { return b + ((size_t)row * N + n) * D; };
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol, Dr = (R)p.D;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)50, beta2 = (R)2 / (R)25;
     V<R> u = ldv(p.u0 + n, N, p.D, lane), un, k[7];
     stv(p.out + n, N, u, p.D, lane);
     stv(rec(p.usave, 0), 1, u, p.D, lane);
@@ -416,23 +415,20 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
         const R ea = xa / (abstol + reltol * sa), eb = xb / (abstol + reltol * sb);
         return (on_a ? ea * ea : (R)0) + (on_b ? eb * eb : (R)0);
     };
-    R dt;
+    PIControl<R, 5> pi;
     {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
         const R d0 = PR::sq(wsum(sq2(u.a, u.b, fabs(u.a), fabs(u.b))) / Dr);
         const R d1 = PR::sq(wsum(sq2(k[0].a, k[0].b, fabs(u.a), fabs(u.b))) / Dr);
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         const V<R> g{fma(dt0, k[0].a, u.a), fma(dt0, k[0].b, u.b)};
         un = rhs(p, sm.ops, sm.th, g, lane);
         const R d2 = PR::sq(wsum(sq2(un.a - k[0].a, un.b - k[0].b, fabs(u.a), fabs(u.b))) / Dr) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)5);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     while (isave < p.n_save) {
-        R h = dt;
+        R h = pi.dt;
         bool clipped = false;
         if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
 #pragma unroll
@@ -447,12 +443,10 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
         }
         R ea = (R)0, eb = (R)0;
 #pragma unroll
-        for (int j = 0; j < 7; ++j) { ea = fma(generic::tsit5_btilde<R>(j), k[j].a, ea); eb = fma(generic::tsit5_btilde<R>(j), k[j].b, eb); }
+        for (int j = 0; j < 7; ++j) { ea = fma((R)Tsit5::bt(j), k[j].a, ea); eb = fma((R)Tsit5::bt(j), k[j].b, eb); }
         const R EEst = PR::sq(wsum(sq2(h * ea, h * eb, fmax(fabs(u.a), fabs(un.a)), fmax(fabs(u.b), fabs(un.b)))) / Dr);
         if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
-        const R q11 = PR::pw(EEst, beta1);
-        const R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= p.max_steps) { bad = 2; break; }
             const R tn = clipped ? t1 : t + h;
             for (int i = 1; i < 7; ++i) stv(rec(p.dense, nacc * 6 + i), 1, k[i], p.D, lane);
@@ -460,7 +454,7 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
                 const R ts = t0 + p.save_dt * (R)isave;
                 if (ts > tn + PR::clip * fabs(tn)) break;
                 R bw[7];
-                generic::tsit5_bw_rt(fmin((ts - t) / h, (R)1), bw);
+                Tsit5::weights(fmin((ts - t) / h, (R)1), bw);
                 R aa = (R)0, ab = (R)0;
 #pragma unroll
                 for (int j = 0; j < 7; ++j) { aa = fma(bw[j], k[j].a, aa); ab = fma(bw[j], k[j].b, ab); }
@@ -469,9 +463,7 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
                 stv(rec(p.usave, isave), 1, us, p.D, lane);
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = tn;
             ++nacc;
             if (lane == 0) p.tgrid[(size_t)nacc * N + n] = t;
@@ -479,7 +471,7 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_forward_kernel(Run<R> p)
             k[0] = k[6];
             stv(rec(p.ustep, nacc), 1, u, p.D, lane);
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
         }
     }
     if (bad) {   // failed solve: the unreached save points are NaN
@@ -530,7 +522,7 @@ __global__ void __launch_bounds__(128) tsit5_adaptive_adjoint_kernel(Run<R> p)
 #pragma unroll
                 for (int i = 0; i < 6; ++i) {
                     R bw[7];
-                    generic::tsit5_bw_rt(fmin(fmax((cur - (R)Tsit5::c(i) * h - tn) / hn, (R)0), (R)1), bw);
+                    Tsit5::weights(fmin(fmax((cur - (R)Tsit5::c(i) * h - tn) / hn, (R)0), (R)1), bw);
                     R xa = (R)0, xb = (R)0, ga = (R)0, gb = (R)0;
 #pragma unroll
                     for (int j = 0; j < 7; ++j) {
@@ -654,8 +646,7 @@ __global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
     cta_reduce(p, sm.g);
 }
 
-// The adaptive RKC2 kernels below repeat the stage recurrence of kernels 5 / 6 and the controller of kernel 3 instead of
-// calling shared helpers: moving that code out of the existing kernels would recompile them, and their SASS stays as it was.
+// The adaptive RKC2 kernels below repeat the stage recurrence of kernels 5 / 6 instead of calling shared helpers.
 
 // the cubic Hermite interpolant on (a0, g0, a1, g1) over a step of length h at fraction Th (OrdinaryDiffEq's dense output of
 // the ROCK methods; kernel 6 writes the same expression inline)
@@ -668,7 +659,7 @@ __device__ __forceinline__ R herm3(R Th, R h, R a0, R a1, R g0, R g1)
 // ---- 7. adaptive RKC2 forward (ROCK2(eigen_est = rho) without dt, npde.jl:80-84,120-123).  Per attempt the fewest stages
 // s in 2..S with beta(s) >= 1.05 h rho (none: s = S and h = beta(S) / (1.05 rho)), the s-stage recurrence of kernel 5, the
 // error estimate of Sommeijer, Shampine and Verwer est = 0.8 (u_n - u_{n+1}) + 0.4 h (f(u_n) + f(u_{n+1})), kernel 3's PI
-// controller with the order-2 exponents (7/20, 1/5).  Saves from the cubic Hermite interpolant; f(u_{n+1}) is the next
+// controller with the order-2 exponents (7/20, 1/5) and the initial step's exponent 1/3.  Saves from the cubic Hermite interpolant; f(u_{n+1}) is the next
 // step's f(u_n), so an accepted step of s stages costs s right-hand sides.  Records u_n, f(u_n), t_n and s_n ----
 template <typename R>
 __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
@@ -684,7 +675,6 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
     auto rec = [&](R *b, int row) { return b + ((size_t)row * N + n) * D; };
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol, Dr = (R)p.D, rho = p.rho;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)20, beta2 = (R)1 / (R)5;
     V<R> u = ldv(p.u0 + n, N, p.D, lane), F0, un, F1;
     stv(p.out + n, N, u, p.D, lane);
     stv(rec(p.usave, 0), 1, u, p.D, lane);
@@ -696,23 +686,20 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
         const R ea = xa / (abstol + reltol * sa), eb = xb / (abstol + reltol * sb);
         return (on_a ? ea * ea : (R)0) + (on_b ? eb * eb : (R)0);
     };
-    R dt;
-    {   // initial step: kernel 3's heuristic at order 2
+    PIControl<R, 2, 3> pi;   // order-2 gains, initial-step exponent 1/3 (the Python reference divides by 3 too)
+    {   // initial step: kernel 3's heuristic
         const R d0 = PR::sq(wsum(sq2(u.a, u.b, fabs(u.a), fabs(u.b))) / Dr);
         const R d1 = PR::sq(wsum(sq2(F0.a, F0.b, fabs(u.a), fabs(u.b))) / Dr);
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         const V<R> g{fma(dt0, F0.a, u.a), fma(dt0, F0.b, u.b)};
         un = rhs(p, sm.ops, sm.th, g, lane);
         const R d2 = PR::sq(wsum(sq2(un.a - F0.a, un.b - F0.b, fabs(u.a), fabs(u.b))) / Dr) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)3);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     while (isave < p.n_save) {
-        R h = dt;
+        R h = pi.dt;
         bool clipped = false;
         if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
         const R hr = (R)1.05 * h * rho;
@@ -739,9 +726,7 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
         const R ea = fma((R)0.4 * h, F0.a + F1.a, (R)0.8 * (u.a - un.a)), eb = fma((R)0.4 * h, F0.b + F1.b, (R)0.8 * (u.b - un.b));
         const R EEst = PR::sq(wsum(sq2(ea, eb, fmax(fabs(u.a), fabs(un.a)), fmax(fabs(u.b), fabs(un.b)))) / Dr);
         if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
-        const R q11 = PR::pw(EEst, beta1);
-        const R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= p.max_steps) { bad = 2; break; }
             const R tn = clipped ? t1 : t + h;
             while (isave < p.n_save) {
@@ -753,9 +738,7 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
                 stv(rec(p.usave, isave), 1, us, p.D, lane);
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = tn;
             if (lane == 0) p.sstep[(size_t)nacc * N + n] = s;
             ++nacc;
@@ -765,7 +748,7 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
             stv(rec(p.ustep, nacc), 1, u, p.D, lane);
             stv(rec(p.dense, nacc), 1, F0, p.D, lane);
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
         }
     }
     if (bad) {   // failed solve: the unreached save points are NaN

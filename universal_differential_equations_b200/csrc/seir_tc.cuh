@@ -12,6 +12,7 @@
 #pragma once
 #include "vern7.cuh"
 #include "lv32_tc.cuh"
+#include "step_control.cuh"
 
 namespace b200ude {
 namespace seir {
@@ -290,7 +291,6 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
     const size_t n = live ? (size_t)gid : (size_t)(p.N - 1);
     const float t0 = ag.t0, t1 = ag.t0 + ag.save_dt * (float)(ag.n_save - 1);
     const float abstol = ag.abstol, reltol = ag.reltol;
-    const float gamma = 0.9f, qmin = 0.2f, qmax = 10.0f, beta1 = 7.0f / 50.0f, beta2 = 2.0f / 25.0f;
     State7 u;
 #pragma unroll
     for (int cc = 0; cc < D; ++cc) u.v[cc] = __ldg(p.u0 + (size_t)cc * N + n);
@@ -310,7 +310,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
         for (int cc = 0; cc < D; ++cc) k[j].v[cc] = 0.0f;
     k[0] = rhs_seir<TM>(&c, sWf_hi, sWf_lo, u, 0);
     store(p.dense, 0, k[0]);
-    float dt;
+    PIControl<float, 5> pi;
     {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
         float d0 = 0.f, d1 = 0.f, d2 = 0.f;
 #pragma unroll
@@ -319,9 +319,8 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
             d0 += (u.v[cc] / sk) * (u.v[cc] / sk);
             d1 += (k[0].v[cc] / sk) * (k[0].v[cc] / sk);
         }
-        d0 = sqrtf(d0 / D); d1 = sqrtf(d1 / D);
-        float dt0 = (d0 < 1e-5f || d1 < 1e-5f) ? 1e-6f : 0.01f * d0 / d1;
-        dt0 = fminf(dt0, t1 - t0);
+        d0 = Prec<float>::sq(d0 / D); d1 = Prec<float>::sq(d1 / D);
+        const float dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         State7 g;
 #pragma unroll
         for (int cc = 0; cc < D; ++cc) g.v[cc] = fmaf(dt0, k[0].v[cc], u.v[cc]);
@@ -332,20 +331,18 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
             const float e = (f1.v[cc] - k[0].v[cc]) / sk;
             d2 += e * e;
         }
-        d2 = sqrtf(d2 / D) / dt0;
-        const float dm = fmaxf(d1, d2);
-        const float dt1 = dm <= 1e-15f ? fmaxf(1e-6f, dt0 * 1e-3f) : exp10f(-(2.0f + log10f(dm)) / 5.0f);
-        dt = fminf(fminf(100.0f * dt0, dt1), t1 - t0);
+        d2 = Prec<float>::sq(d2 / D) / dt0;
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    float t = t0, qold = 1e-4f;
+    float t = t0;
     int nacc = 0, isave = 1, bad = 0;
 #pragma unroll 1
     while (true) {
         const bool active = (isave < ag.n_save) && !bad;
         if (!__syncthreads_or(active ? 1 : 0)) break;
-        float h = dt;
+        float h = pi.dt;
         bool clipped = false;
-        if (t + h >= t1 - 1e-6f * fabsf(t1)) { h = t1 - t; clipped = true; }
+        if (t + h >= t1 - Prec<float>::clip * fabsf(t1)) { h = t1 - t; clipped = true; }
         if (!active) h = 0.0f;
         State7 un = u;
 #pragma unroll 1
@@ -389,18 +386,16 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
             for (int cc = 0; cc < D; ++cc) {
                 float e = 0.0f;
 #pragma unroll
-                for (int j = 0; j < 7; ++j) e = fmaf(lv32::tc::tsit5_btilde_rt(j), k[j].v[cc], e);
+                for (int j = 0; j < 7; ++j) e = fmaf((float)Tsit5::bt(j), k[j].v[cc], e);
                 e *= h;
                 const float sc = abstol + reltol * fmaxf(fabsf(u.v[cc]), fabsf(un.v[cc]));
                 ee += (e / sc) * (e / sc);
             }
-            const float EEst = sqrtf(ee / D);
-            if (!(EEst <= 3.0e38f)) {
+            const float EEst = Prec<float>::sq(ee / D);
+            if (!(EEst <= Prec<float>::huge)) {
                 bad = 1;
             } else {
-                const float q11 = powf(EEst, beta1);
-                float q = fminf(fmaxf(q11 / powf(qold, beta2) / gamma, 1.0f / qmax), 1.0f / qmin);
-                if (EEst <= 1.0f) {
+                if (pi.judge(EEst)) {
                     if (nacc >= ag.max_steps) {
                         bad = 2;
                     } else {
@@ -409,9 +404,9 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
                         for (int i = 1; i < 7; ++i) store(p.dense, nacc * 6 + i, k[i]);
                         while (isave < ag.n_save) {
                             const float ts = t0 + ag.save_dt * (float)isave;
-                            if (ts > tn + 1e-6f * fabsf(tn)) break;
+                            if (ts > tn + Prec<float>::clip * fabsf(tn)) break;
                             float bw[7];
-                            lv32::tc::tsit5_weights_fwd(fminf((ts - t) / h, 1.0f), bw);
+                            Tsit5::weights(fminf((ts - t) / h, 1.0f), bw);
                             State7 o;
 #pragma unroll
                             for (int cc = 0; cc < D; ++cc) {
@@ -423,10 +418,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
                             store(p.out, isave, o);
                             ++isave;
                         }
-                        qold = fmaxf(EEst, 1e-4f);
-                        // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq (the 6/5 band is the implicit-solver default): no dead band
-                        if (!clipped || h >= dt) dt = h / q;
-                        else dt = fmaxf(dt, h / q);
+                        pi.accept(EEst, h, clipped);
                         t = tn;
                         ++nacc;
                         if (live) ag.tgrid[(size_t)nacc * N + n] = t;
@@ -435,7 +427,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
                         store(p.ustep, nacc, u);
                     }
                 } else {
-                    dt = h / fminf(1.0f / qmin, q11 / gamma);
+                    pi.reject(h);
                 }
             }
         }
@@ -443,13 +435,13 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(FwdParams p,
     if (bad && live) {   // failed solve: the unreached save points are NaN
         for (int is = isave; is < ag.n_save; ++is)
 #pragma unroll
-            for (int cc = 0; cc < D; ++cc) p.out[((size_t)is * D + cc) * N + n] = __int_as_float(0x7fc00000);
+            for (int cc = 0; cc < D; ++cc) p.out[((size_t)is * D + cc) * N + n] = Prec<float>::nan();
     }
     if (live) ag.nacc[n] = nacc;
     if (p.status && live) {
         bool ok = true;
 #pragma unroll
-        for (int cc = 0; cc < D; ++cc) ok = ok && (fabsf(u.v[cc]) <= 3.0e38f);
+        for (int cc = 0; cc < D; ++cc) ok = ok && (fabsf(u.v[cc]) <= Prec<float>::huge);
         p.status[n] = bad == 2 ? 2 : ((bad || !ok) ? 1 : 0);
     }
 }
@@ -770,7 +762,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(AdjParams p, Adaptive
                 {
                     const float Th = fminf(fmaxf((cur - ci * h - tn) * inv_hn, 0.0f), 1.0f);
                     float bw[7];
-                    lv32::tc::tsit5_weights(Th, bw);
+                    Tsit5::weights(Th, bw);
 #pragma unroll
                     for (int cc = 0; cc < D; ++cc) {
                         float acc2 = 0.0f;

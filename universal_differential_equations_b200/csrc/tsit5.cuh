@@ -48,6 +48,20 @@ struct Tsit5 {
         }
     }
     __host__ __device__ static constexpr double b(int j) { return a(6, j); }
+    // error weights b_j - btilde_j: err = dt * sum_j bt(j) k_j over the 7 stages
+    __host__ __device__ static constexpr double bt(int j)
+    {
+        switch (j) {
+        case 0: return -0.001780011052225777;
+        case 1: return -0.0008164344596567469;
+        case 2: return 0.007880878010261995;
+        case 3: return -0.1447110071732629;
+        case 4: return 0.5823571654525552;
+        case 5: return -0.45808210592918697;
+        case 6: return 0.015151515151515152;
+        default: return 0.0;
+        }
+    }
     // interpolant polynomial coefficients r_{j,p}: b_j(Th) = sum_p r(j,p) Th^p, p = 1..4
     __host__ __device__ static constexpr double r(int j, int p)
     {
@@ -85,6 +99,21 @@ struct Tsit5 {
     // weight of forward stage derivative k_j in u(t_{n+1} - c_i dt), the state the
     // backward (adjoint) stage i needs:  Theta_i = 1 - c_i
     __host__ __device__ static constexpr double bw(int i, int j) { return bTheta(j, 1.0 - c(i)); }
+    // b_j(Th) for a run-time Th, in the kernel's precision
+    template <typename R>
+    __device__ static __forceinline__ void weights(R Th, R (&w)[7])
+    {
+        w[0] = Th * ((R)r(0, 1) + Th * ((R)r(0, 2) + Th * ((R)r(0, 3) + Th * (R)r(0, 4))));
+#pragma unroll
+        for (int j = 1; j < 7; ++j) w[j] = Th * Th * ((R)r(j, 2) + Th * ((R)r(j, 3) + Th * (R)r(j, 4)));
+    }
 };
+
+// The fp32 kernels take (float)bt(j): each weight must round to the same float through double as from its decimal.
+static_assert((float)Tsit5::bt(0) == -0.001780011052225777f && (float)Tsit5::bt(1) == -0.0008164344596567469f &&
+                  (float)Tsit5::bt(2) == 0.007880878010261995f && (float)Tsit5::bt(3) == -0.1447110071732629f &&
+                  (float)Tsit5::bt(4) == 0.5823571654525552f && (float)Tsit5::bt(5) == -0.45808210592918697f &&
+                  (float)Tsit5::bt(6) == 0.015151515151515152f,
+              "Tsit5 error weights double-round in fp32");
 
 }  // namespace b200ude

@@ -28,36 +28,11 @@
 #include <stdint.h>
 
 #include "params.h"
+#include "step_control.cuh"
 #include "tsit5.cuh"
 #include "vern7.cuh"
 
 namespace b200ude {
-
-// per-precision margins and math of every kernel written over the real type
-template <typename R>
-struct Prec;
-template <>
-struct Prec<float> {
-    static constexpr float clip = 1e-6f;   // a step within clip |t1| of the end of tspan (or a save time) is stretched to it
-    static constexpr float eta = 1e-5f;    // a save time within eta h of a step end is that step end
-    static constexpr float huge = 3.0e38f;
-    static __device__ __forceinline__ float nan() { return __int_as_float(0x7fc00000); }
-    static __device__ __forceinline__ float pw(float a, float b) { return powf(a, b); }
-    static __device__ __forceinline__ float sq(float a) { return sqrtf(a); }
-    static __device__ __forceinline__ float lg(float a) { return log10f(a); }
-    static __device__ __forceinline__ float ex(float a) { return exp10f(a); }
-};
-template <>
-struct Prec<double> {
-    static constexpr double clip = 1e-12;
-    static constexpr double eta = 1e-10;
-    static constexpr double huge = 1.0e300;
-    static __device__ __forceinline__ double nan() { return __longlong_as_double(0x7ff8000000000000LL); }
-    static __device__ __forceinline__ double pw(double a, double b) { return pow(a, b); }
-    static __device__ __forceinline__ double sq(double a) { return sqrt(a); }
-    static __device__ __forceinline__ double lg(double a) { return log10(a); }
-    static __device__ __forceinline__ double ex(double a) { return exp10(a); }
-};
 
 namespace generic {
 
@@ -423,29 +398,12 @@ __global__ void __launch_bounds__(BLOCK, 1) adjoint_kernel(typename Ops::Adj p)
 
 // =====================================================================================================
 // Adaptive stepping (abstol / reltol as every reference call passes them: scenario_1.jl:85, seir_exposure.jl:139):
-// Tsit5 with OrdinaryDiffEq's default PI controller (gamma 0.9, qmin 1/5, qmax 10, beta1 7/50, beta2 2/25,
-// steady band [1, 1.2], Hairer initial step), one trajectory per thread with its own dt; saveat values come from
-// the free 4th-order interpolant and do not alter the steps.  Every ACCEPTED step is recorded
-// (tgrid, ustep, dense) so that the interpolating adjoint can replay the steps backwards, splitting them at
+// Tsit5 with OrdinaryDiffEq's default PI controller and initial step (PIControl, step_control.cuh), one trajectory per
+// thread with its own dt; saveat values come from the free 4th-order interpolant and do not alter the steps.  Every ACCEPTED
+// step is recorded (tgrid, ustep, dense) so that the interpolating adjoint can replay the steps backwards, splitting them at
 // the save times where the loss cotangent jumps in (oracle: ude_adjoint_replay; validated there against an
 // error-controlled backward solve of [lambda; mu]).  The step record is Ops::Adapt (AdaptiveGrid / Adapt64Host, params.h).
 // =====================================================================================================
-
-// weights of the free 4th-order interpolant at Th
-template <typename R>
-__device__ __forceinline__ void tsit5_bw_rt(R Th, R *bw)
-{
-    bw[0] = Th * ((R)Tsit5::r(0, 1) + Th * ((R)Tsit5::r(0, 2) + Th * ((R)Tsit5::r(0, 3) + Th * (R)Tsit5::r(0, 4))));
-#pragma unroll
-    for (int j = 1; j < 7; ++j) bw[j] = Th * Th * ((R)Tsit5::r(j, 2) + Th * ((R)Tsit5::r(j, 3) + Th * (R)Tsit5::r(j, 4)));
-}
-// error weights b - b* of Tsit5
-template <typename R>
-__device__ __forceinline__ R tsit5_btilde(int j)
-{
-    return j == 0 ? (R)-0.001780011052225777 : j == 1 ? (R)-0.0008164344596567469 : j == 2 ? (R)0.007880878010261995
-         : j == 3 ? (R)-0.1447110071732629 : j == 4 ? (R)0.5823571654525552 : j == 5 ? (R)-0.45808210592918697 : (R)0.015151515151515152;
-}
 
 template <class Ops, int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops::Fwd p, typename Ops::Adapt ap)
@@ -459,7 +417,6 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
     const size_t n = (size_t)gid;
     const R t0 = ap.t0, t1 = ap.t0 + ap.save_dt * (R)(ap.n_save - 1);
     const R abstol = ap.abstol, reltol = ap.reltol;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)50, beta2 = (R)2 / (R)25;
     R u[MAXD], un[MAXD], g[MAXD], k[7][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     auto store = [&](R *base, int row, const R *v) {
@@ -471,7 +428,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
     model_rhs<Ops>(u, k[0]);
     store(p.dense, 0, k[0]);
     // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
-    R dt;
+    PIControl<R, 5> pi;
     {
         R d0 = 0, d1 = 0, d2 = 0;
         for (int c = 0; c < D; ++c) {
@@ -480,8 +437,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
             d1 += (k[0][c] / sk) * (k[0][c] / sk);
         }
         d0 = PR::sq(d0 / D); d1 = PR::sq(d1 / D);
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         for (int c = 0; c < D; ++c) g[c] = fma(dt0, k[0][c], u[c]);
         model_rhs<Ops>(g, un);
         for (int c = 0; c < D; ++c) {
@@ -490,14 +446,12 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
             d2 += e * e;
         }
         d2 = PR::sq(d2 / D) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)5);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     while (isave < ap.n_save) {
-        R h = dt;
+        R h = pi.dt;
         bool clipped = false;
         if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
 #pragma unroll
@@ -516,16 +470,14 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
         for (int c = 0; c < D; ++c) {
             R e = (R)0;
 #pragma unroll
-            for (int j = 0; j < 7; ++j) e = fma(tsit5_btilde<R>(j), k[j][c], e);
+            for (int j = 0; j < 7; ++j) e = fma((R)Tsit5::bt(j), k[j][c], e);
             e *= h;
             const R sc = abstol + reltol * fmax(fabs(u[c]), fabs(un[c]));
             ee += (e / sc) * (e / sc);
         }
         const R EEst = PR::sq(ee / D);
         if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
-        const R q11 = PR::pw(EEst, beta1);
-        R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= ap.max_steps) { bad = 2; break; }
             const R tn = clipped ? t1 : t + h;
             // dense record of this step: k_1..k_6 at rows nacc*6 + i, k_7 at (nacc+1)*6 (= k_1 of the next step)
@@ -534,7 +486,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
                 const R ts = t0 + ap.save_dt * (R)isave;
                 if (ts > tn + PR::clip * fabs(tn)) break;
                 R bw[7];
-                tsit5_bw_rt(fmin((ts - t) / h, (R)1), bw);
+                Tsit5::weights(fmin((ts - t) / h, (R)1), bw);
                 for (int c = 0; c < D; ++c) {
                     R acc = (R)0;
 #pragma unroll
@@ -543,17 +495,14 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_forward_kernel(typename Ops
                 }
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq (the 6/5 band is the implicit-solver default): no dead band
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = tn;
             ++nacc;
             ap.tgrid[(size_t)nacc * N + n] = t;
             for (int c = 0; c < D; ++c) { u[c] = un[c]; k[0][c] = k[6][c]; }
             store(p.ustep, nacc, u);
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
         }
     }
     if (bad) {   // failed solve (non-finite error estimate / max_steps): the unreached save points are NaN, as a failed retcode would signal
@@ -586,7 +535,6 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
     const size_t n = (size_t)gid;
     const R t0 = ap.t0, t1 = ap.t0 + ap.save_dt * (R)(ap.n_save - 1);
     const R abstol = ap.abstol, reltol = ap.reltol;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)70, beta2 = (R)2 / (R)35;   // order 7
     const bool record = p.ustep != nullptr;
     R u[MAXD], un[MAXD], g[MAXD], k[10][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
@@ -596,7 +544,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
         for (int c = 0; c < D; ++c) p.ustep[(size_t)c * N + n] = u[c];
     }
     model_rhs<Ops>(u, k[0]);
-    R dt;
+    PIControl<R, 7> pi;
     {
         R d0 = 0, d1 = 0, d2 = 0;
         for (int c = 0; c < D; ++c) {
@@ -605,8 +553,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
             d1 += (k[0][c] / sk) * (k[0][c] / sk);
         }
         d0 = PR::sq(d0 / D); d1 = PR::sq(d1 / D);
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         for (int c = 0; c < D; ++c) g[c] = fma(dt0, k[0][c], u[c]);
         model_rhs<Ops>(g, un);
         for (int c = 0; c < D; ++c) {
@@ -615,16 +562,14 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
             d2 += e * e;
         }
         d2 = PR::sq(d2 / D) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)7);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     bool have_k1 = true;
     while (isave < ap.n_save) {
         const R tend = t0 + ap.save_dt * (R)isave;
-        R h = dt;
+        R h = pi.dt;
         bool clipped = false;
         if (t + h >= tend - PR::clip * fabs(tend)) { h = tend - t; clipped = true; }
         if (!have_k1) model_rhs<Ops>(u, k[0]);
@@ -654,9 +599,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
         }
         const R EEst = PR::sq(ee / D);
         if (!(EEst <= PR::huge)) { bad = 1; break; }
-        const R q11 = PR::pw(EEst, beta1);
-        R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= ap.max_steps) { bad = 2; break; }
             if (record) ap.hstep[(size_t)nacc * N + n] = h;
             ++nacc;
@@ -664,10 +607,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
                 for (int c = 0; c < D; ++c) p.out[((size_t)isave * D + c) * N + n] = un[c];
                 ++isave;
             }
-            qold = fmax(EEst, (R)1e-4);
-            // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq (the 6/5 band is the implicit-solver default): no dead band
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = clipped ? tend : t + h;
             if (record) {
                 ap.tgrid[(size_t)nacc * N + n] = t;
@@ -676,7 +616,7 @@ __global__ void __launch_bounds__(BLOCK, 1) vern7_adaptive_forward_kernel(typena
             for (int c = 0; c < D; ++c) u[c] = un[c];
             have_k1 = false;   // not FSAL
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
             have_k1 = true;    // k_1 = f(u) is still valid after a rejection
         }
     }
@@ -741,7 +681,7 @@ __global__ void __launch_bounds__(BLOCK, 1) adaptive_adjoint_kernel(typename Ops
             for (int i = 0; i < 6; ++i) {
                 R bw[7];
                 const R Th = fmin(fmax((cur - (R)Tsit5::c(i) * h - tn) / hn, (R)0), (R)1);
-                tsit5_bw_rt(Th, bw);
+                Tsit5::weights(Th, bw);
                 for (int c = 0; c < D; ++c) {
                     R acc = (R)0;
 #pragma unroll

@@ -299,7 +299,7 @@ struct Fwd {
     R t0, save_dt, abstol, reltol;
 };
 
-// adaptive Vern7 with OrdinaryDiffEq's PI controller (order 7: beta1 = 7/70, beta2 = 2/35), steps clipped at the end of tspan only,
+// adaptive Vern7 with OrdinaryDiffEq's PI controller (PIControl<R, 7>), steps clipped at the end of tspan only,
 // saveat by the interpolant
 template <class Ops, int BLOCK>
 __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::real> p)
@@ -314,7 +314,6 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
     const size_t n = (size_t)gid;
     const R t0 = p.t0, t1 = p.t0 + p.save_dt * (R)(p.n_save - 1);
     const R abstol = p.abstol, reltol = p.reltol;
-    const R gamma = (R)0.9, qmin = (R)0.2, qmax = (R)10, beta1 = (R)7 / (R)70, beta2 = (R)2 / (R)35;
     R u[MAXD], un[MAXD], g[MAXD], k[16][MAXD];
     for (int c = 0; c < D; ++c) u[c] = __ldg(p.u0 + (size_t)c * N + n);
     for (int c = 0; c < D; ++c) {
@@ -323,7 +322,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
     }
     p.tgrid[n] = t0;
     generic::model_rhs<Ops>(u, k[0]);
-    R dt;
+    PIControl<R, 7> pi;
     {   // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq
         R d0 = 0, d1 = 0, d2 = 0;
         for (int c = 0; c < D; ++c) {
@@ -332,8 +331,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
             d1 += (k[0][c] / sk) * (k[0][c] / sk);
         }
         d0 = PR::sq(d0 / D); d1 = PR::sq(d1 / D);
-        R dt0 = (d0 < (R)1e-5 || d1 < (R)1e-5) ? (R)1e-6 : (R)0.01 * d0 / d1;
-        dt0 = fmin(dt0, t1 - t0);
+        const R dt0 = pi.hnw_dt0(d0, d1, t1 - t0);
         for (int c = 0; c < D; ++c) g[c] = fma(dt0, k[0][c], u[c]);
         generic::model_rhs<Ops>(g, un);
         for (int c = 0; c < D; ++c) {
@@ -342,15 +340,13 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
             d2 += e * e;
         }
         d2 = PR::sq(d2 / D) / dt0;
-        const R dm = fmax(d1, d2);
-        const R dt1 = dm <= (R)1e-15 ? fmax((R)1e-6, dt0 * (R)1e-3) : PR::ex(-((R)2 + PR::lg(dm)) / (R)7);
-        dt = fmin(fmin((R)100 * dt0, dt1), t1 - t0);
+        pi.hnw(dt0, d1, d2, t1 - t0);
     }
-    R t = t0, qold = (R)1e-4;
+    R t = t0;
     int nacc = 0, isave = 1, bad = 0;
     bool have_k1 = true;
     while (isave < p.n_save) {
-        R h = dt;
+        R h = pi.dt;
         bool clipped = false;
         if (t + h >= t1 - PR::clip * fabs(t1)) { h = t1 - t; clipped = true; }
         if (!have_k1) generic::model_rhs<Ops>(u, k[0]);
@@ -378,9 +374,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
         }
         const R EEst = PR::sq(ee / D);
         if (!(EEst <= PR::huge)) { bad = 1; break; }
-        const R q11 = PR::pw(EEst, beta1);
-        const R q = fmin(fmax(q11 / PR::pw(qold, beta2) / gamma, (R)1 / qmax), (R)1 / qmin);
-        if (EEst <= (R)1) {
+        if (pi.judge(EEst)) {
             if (nacc >= p.max_steps) { bad = 2; break; }
             const R tn = clipped ? t1 : t + h;
             const R eps = PR::eta * (tn - t);
@@ -400,10 +394,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
             }
             p.hstep[(size_t)nacc * N + n] = h;
             ++nacc;
-            qold = fmax(EEst, (R)1e-4);
-            // qsteady_min = qsteady_max = 1 for explicit RK methods in OrdinaryDiffEq: no dead band
-            if (!clipped || h >= dt) dt = h / q;
-            else dt = fmax(dt, h / q);
+            pi.accept(EEst, h, clipped);
             t = tn;
             p.tgrid[(size_t)nacc * N + n] = t;
             for (int c = 0; c < D; ++c) {
@@ -412,7 +403,7 @@ __global__ void __launch_bounds__(BLOCK, 1) forward_kernel(Fwd<typename Ops::rea
             }
             have_k1 = false;   // not FSAL
         } else {
-            dt = h / fmin((R)1 / qmin, q11 / gamma);
+            pi.reject(h);
             have_k1 = true;    // k_1 = f(u) is still valid after a rejection
         }
     }
