@@ -469,6 +469,10 @@ int FN(ude_solve_adaptive)(const ude_model *m, const REAL *th, const REAL *u0, c
  * linear combination h sum_k w_k G_k of the stage integrands, with w from running the recurrence on unit vectors. */
 #ifndef UDE_RKC_TABLES_DEFINED
 #define UDE_RKC_TABLES_DEFINED
+#include <float.h>
+#if LDBL_MANT_DIG <= DBL_MANT_DIG
+#error "ude_rkc2_tables needs a long double wider than double (x86-64, aarch64 Linux) for fp64-accurate RKC2 tables"
+#endif
 #define UDE_RKC_MAX_STAGES 64
 typedef struct {
     int s;
@@ -481,26 +485,29 @@ typedef struct {
 
 static void ude_rkc2_tables(int s, ude_rkc_tables *t)
 {
-    const double eps = 2.0 / 13.0;
-    const double w0 = 1.0 + eps / ((double)s * s);
-    double T[UDE_RKC_MAX_STAGES + 1], dT[UDE_RKC_MAX_STAGES + 1], d2T[UDE_RKC_MAX_STAGES + 1], b[UDE_RKC_MAX_STAGES + 1] = {0};
+    /* T_j, T_j', T_j'' and b_j in long double: in double the relative error of the three-term recurrences grows like
+     * j^2 eps, which at s = 64 moves the tables' stability polynomial by ~1e-10 at the end of its interval */
+    const long double eps = 2.0L / 13.0L;
+    const long double w0 = 1.0L + eps / ((long double)s * s);
+    long double T[UDE_RKC_MAX_STAGES + 1], dT[UDE_RKC_MAX_STAGES + 1], d2T[UDE_RKC_MAX_STAGES + 1], b[UDE_RKC_MAX_STAGES + 1] = {0};
     T[0] = 1; T[1] = w0; dT[0] = 0; dT[1] = 1; d2T[0] = 0; d2T[1] = 0;
     for (int j = 2; j <= s; ++j) {
         T[j] = 2 * w0 * T[j - 1] - T[j - 2];
         dT[j] = 2 * T[j - 1] + 2 * w0 * dT[j - 1] - dT[j - 2];
         d2T[j] = 4 * dT[j - 1] + 2 * w0 * d2T[j - 1] - d2T[j - 2];
     }
-    const double w1 = dT[s] / d2T[s];
+    const long double w1 = dT[s] / d2T[s];
     for (int j = 2; j <= s; ++j) b[j] = d2T[j] / (dT[j] * dT[j]);
     b[0] = b[1] = b[2];
     t->s = s;
-    t->mt1 = b[1] * w1;
-    t->beta = (w0 + 1.0) * d2T[s] / dT[s];
+    t->mt1 = (double)(b[1] * w1);
+    t->beta = (double)((w0 + 1.0L) * d2T[s] / dT[s]);
     for (int j = 2; j <= s; ++j) {
-        t->mu[j] = 2 * b[j] * w0 / b[j - 1];
-        t->nu[j] = -b[j] / b[j - 2];
-        t->mt[j] = 2 * b[j] * w1 / b[j - 1];
-        t->ga[j] = -(1.0 - b[j - 1] * T[j - 1]) * t->mt[j];
+        const long double mt = 2 * b[j] * w1 / b[j - 1];
+        t->mu[j] = (double)(2 * b[j] * w0 / b[j - 1]);
+        t->nu[j] = (double)(-b[j] / b[j - 2]);
+        t->mt[j] = (double)mt;
+        t->ga[j] = (double)(-(1.0L - b[j - 1] * T[j - 1]) * mt);
     }
     /* abscissae and quadrature weights from the recurrence itself (y' = 1, and unit impulses in F_k) */
     double W[UDE_RKC_MAX_STAGES + 1][UDE_RKC_MAX_STAGES + 1];

@@ -7,6 +7,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cfloat>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -176,10 +177,15 @@ cudaError_t dalloc_real(b200ude_handle *h, void **p, size_t count) { return dall
 // RKC2 (Sommeijer, Shampine, Verwer 1998) recurrence coefficients, stage abscissae and the quadrature weights of the stage
 // integrands (from running the recurrence on unit impulses)
 // in double: mt1, then mu, nu, mt, ga, c, w with 65 entries each
+#if LDBL_MANT_DIG <= DBL_MANT_DIG
+#error "rkc2_tables64 needs a long double wider than double (x86-64, aarch64 Linux) for fp64-accurate RKC2 tables"
+#endif
 void rkc2_tables64(int s, double &mt1, double *mu, double *nu, double *mt, double *ga, double *c, double *w)
 {
-    const double eps = 2.0 / 13.0, w0 = 1.0 + eps / ((double)s * s);
-    double T[65], dT[65], d2T[65], b[65] = {0};
+    // T_j, T_j', T_j'' and b_j in long double (the oracle's ude_rkc2_tables): in double the relative error of the three-term
+    // recurrences grows like j^2 eps, which at s = 64 moves the tables' stability polynomial by ~1e-10 at the end of its interval
+    const long double eps = 2.0L / 13.0L, w0 = 1.0L + eps / ((long double)s * s);
+    long double T[65], dT[65], d2T[65], b[65] = {0};
     for (int j = 0; j < 65; ++j) mu[j] = nu[j] = mt[j] = ga[j] = c[j] = w[j] = 0;
     double W[65][65];   // 33 KB of stack, host side only
     T[0] = 1; T[1] = w0; dT[0] = 0; dT[1] = 1; d2T[0] = 0; d2T[1] = 0;
@@ -188,15 +194,16 @@ void rkc2_tables64(int s, double &mt1, double *mu, double *nu, double *mt, doubl
         dT[j] = 2 * T[j - 1] + 2 * w0 * dT[j - 1] - dT[j - 2];
         d2T[j] = 4 * dT[j - 1] + 2 * w0 * d2T[j - 1] - d2T[j - 2];
     }
-    const double w1 = dT[s] / d2T[s];
+    const long double w1 = dT[s] / d2T[s];
     for (int j = 2; j <= s; ++j) b[j] = d2T[j] / (dT[j] * dT[j]);
     b[0] = b[1] = b[2];
-    mt1 = b[1] * w1;
+    mt1 = (double)(b[1] * w1);
     for (int j = 2; j <= s; ++j) {
-        mu[j] = 2 * b[j] * w0 / b[j - 1];
-        nu[j] = -b[j] / b[j - 2];
-        mt[j] = 2 * b[j] * w1 / b[j - 1];
-        ga[j] = -(1.0 - b[j - 1] * T[j - 1]) * mt[j];
+        const long double mtj = 2 * b[j] * w1 / b[j - 1];
+        mu[j] = (double)(2 * b[j] * w0 / b[j - 1]);
+        nu[j] = (double)(-b[j] / b[j - 2]);
+        mt[j] = (double)mtj;
+        ga[j] = (double)(-(1.0L - b[j - 1] * T[j - 1]) * mtj);
     }
     memset(W, 0, sizeof W);
     c[0] = 0; c[1] = mt1; W[1][0] = mt1;

@@ -591,16 +591,17 @@ __global__ void __launch_bounds__(256) forward_rkc_kernel2(FwdParams p, Geom geo
     for (int s = 0; s < p.n_steps; ++s) {
         const float2 F0 = rhs(u, 0);
         store_int(p.dense, s, F0);   // row s of the record = f(u_s): with u_s, u_{s+1}, f(u_{s+1}) the cubic-Hermite dense output
-        float2 Y0 = u, Y1 = fma2(bc(c_rkc.mt1 * dt), F0, u);
+        // the stages as increments D_j = Y_j - u (operator.cuh kernel 5): O(h f), so their round-off is not amplified with |u|
+        float2 D0 = bc(0.0f), D1 = mul2(bc(c_rkc.mt1 * dt), F0);
 #pragma unroll 1
         for (int j = 2; j <= S; ++j) {
-            const float2 F = rhs(Y1, j);
+            const float2 F = rhs(add2(u, D1), j);
             const float mu = c_rkc.mu[j], nu = c_rkc.nu[j], mt = c_rkc.mt[j], ga = c_rkc.ga[j];
-            const float2 Y2 = fma2(bc(ga * dt), F0, fma2(bc(mt * dt), F, fma2(bc(nu), Y0, fma2(bc(mu), Y1, mul2(bc(1.0f - mu - nu), u)))));
-            Y0 = Y1;
-            Y1 = Y2;
+            const float2 D2 = fma2(bc(ga * dt), F0, fma2(bc(mt * dt), F, fma2(bc(nu), D0, mul2(bc(mu), D1))));
+            D0 = D1;
+            D1 = D2;
         }
-        u = Y1;
+        u = add2(u, D1);
         store_int(p.ustep, s + 1, u);
         if ((s + 1) % p.save_every == 0) { store_abi(p.out, isave, u); ++isave; }
     }
@@ -767,8 +768,10 @@ __global__ void __launch_bounds__(256) adjoint_kernel2(AdjParams p, Geom geo)
             else dxa = fma2(bc(wi), q1, dxa);
         }
         const float2 dx = mul2(add2(dxa, dxb), bc(isc));
-        // (J^T g)_i: w1 couples i+1 -> i, w3 couples i-1 -> i
-        const float2 kn = make_float2(dx.x + D0 * fmaf(w2, g.x, fmaf(w1, g.y, w3 * gl)), dx.y + D0 * fmaf(w2, g.y, fmaf(w1, gr, w3 * g.x)));
+        // (J^T g)_i: w1 couples i+1 -> i, w3 couples i-1 -> i.  The centre and one neighbour first, as the forward stencil does:
+        // for a smooth g, w2 g_i + g_{i-1} is exact and the sum rounds only after the cancellation (summing the two neighbours
+        // first rounds at |g| and costs eps |g| D0 per evaluation)
+        const float2 kn = make_float2(dx.x + D0 * fmaf(w1, g.y, fmaf(w2, g.x, w3 * gl)), dx.y + D0 * fmaf(w1, gr, fmaf(w2, g.y, w3 * g.x)));
         // stencil-weight and D0 gradients: point 0 has neighbours (xl, x.y), point 1 has (x.x, xr)
         a_s1 = fmaf(sg.x * D0, xl, fmaf(sg.y * D0, x.x, a_s1));
         a_s2 = fmaf(sg.x * D0, x.x, fmaf(sg.y * D0, x.y, a_s2));
@@ -832,28 +835,27 @@ __global__ void __launch_bounds__(256) adjoint_kernel2(AdjParams p, Geom geo)
     for (int s = p.n_steps - 1; s >= 0; --s) {
         const float2 y0 = ld2(p.ustep, (size_t)s), y1 = ld2(p.ustep, (size_t)s + 1), f0 = ld2(p.dense, (size_t)s), f1 = ld2(p.dense, (size_t)s + 1);
         const float2 dy = add2(y1, mul2(bc(-1.0f), y0));
-        float2 Y0 = lam, Y1 = lam, F0 = bc(0.0f);
+        float2 D0 = bc(0.0f), D1 = bc(0.0f), F0 = bc(0.0f);   // increments Y_j - lambda
 #pragma unroll 1
         for (int j = 0; j < S; ++j) {
             const float Th = 1.0f - c_rkc.c[j];
             // x = (1 - Th) y0 + Th y1 + Th (Th - 1) ((1 - 2 Th) (y1 - y0) + (Th - 1) dt f0 + Th dt f1)
             const float2 inner = fma2(bc(1.0f - 2.0f * Th), dy, fma2(bc((Th - 1.0f) * dt), f0, mul2(bc(Th * dt), f1)));
             const float2 x = fma2(bc(Th * (Th - 1.0f)), inner, fma2(bc(Th), dy, y0));
-            const float2 g = j == 0 ? lam : Y1;
+            const float2 g = add2(lam, D1);
             const float sc = dt * c_rkc.w[j], isc = 1.0f / sc;
             const float2 kn = eval_core(x, g, sc, isc, j);
             if (j == 0) {
                 F0 = kn;
-                Y0 = lam;
-                Y1 = fma2(bc(c_rkc.mt1 * dt), F0, lam);
+                D1 = mul2(bc(c_rkc.mt1 * dt), F0);
             } else {
                 const float mu = c_rkc.mu[j + 1], nu = c_rkc.nu[j + 1], mt = c_rkc.mt[j + 1], ga = c_rkc.ga[j + 1];
-                const float2 Y2 = fma2(bc(ga * dt), F0, fma2(bc(mt * dt), kn, fma2(bc(nu), Y0, fma2(bc(mu), Y1, mul2(bc(1.0f - mu - nu), lam)))));
-                Y0 = Y1;
-                Y1 = Y2;
+                const float2 D2 = fma2(bc(ga * dt), F0, fma2(bc(mt * dt), kn, fma2(bc(nu), D0, mul2(bc(mu), D1))));
+                D0 = D1;
+                D1 = D2;
             }
         }
-        lam = Y1;
+        lam = add2(lam, D1);
         if (s % p.save_every == 0) jump(s / p.save_every);
     }
     }

@@ -571,17 +571,18 @@ __global__ void __launch_bounds__(128) rkc2_forward_kernel(Run<R> p)
         const V<R> F0 = rhs(p, sm.ops, sm.th, u, lane);
         stv(rec(p.ustep, s), 1, u, p.D, lane);
         stv(rec(p.dense, s), 1, F0, p.D, lane);
-        V<R> Y0 = u, Y1{fma(mt1 * dt, F0.a, u.a), fma(mt1 * dt, F0.b, u.b)};
+        // the stages as increments D_j = Y_j - u: they are O(h f), so their round-off is not the recurrence's amplification of
+        // |u| (carried as Y_j, fp32 adaptive solves at 32..64 stages were 5.9e-5 off the fp64 reference; now 6.4e-7)
+        V<R> D0{(R)0, (R)0}, D1{mt1 * dt * F0.a, mt1 * dt * F0.b};
         for (int j = 2; j <= p.S; ++j) {
-            const V<R> F = rhs(p, sm.ops, sm.th, Y1, lane);
+            const V<R> F = rhs(p, sm.ops, sm.th, V<R>{u.a + D1.a, u.b + D1.b}, lane);
             const R mu = __ldg(p.rkc + RKC_MU + j), nu = __ldg(p.rkc + RKC_NU + j), mt = __ldg(p.rkc + RKC_MT + j), ga = __ldg(p.rkc + RKC_GA + j);
-            const R c0 = (R)1 - mu - nu;
-            const V<R> Y2{fma(ga * dt, F0.a, fma(mt * dt, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * u.a)))),
-                          fma(ga * dt, F0.b, fma(mt * dt, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * u.b))))};
-            Y0 = Y1;
-            Y1 = Y2;
+            const V<R> D2{fma(ga * dt, F0.a, fma(mt * dt, F.a, fma(nu, D0.a, mu * D1.a))),
+                          fma(ga * dt, F0.b, fma(mt * dt, F.b, fma(nu, D0.b, mu * D1.b)))};
+            D0 = D1;
+            D1 = D2;
         }
-        u = Y1;
+        u = V<R>{u.a + D1.a, u.b + D1.b};
         if ((s + 1) % p.save_every == 0) { stv(p.out + (size_t)isave * D * N + n, N, u, p.D, lane); ++isave; }
     }
     stv(rec(p.ustep, p.n_steps), 1, u, p.D, lane);
@@ -613,7 +614,7 @@ __global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
         for (int s = p.n_steps - 1; s >= 0; --s) {
             const V<R> y0 = ldv(rec(p.ustep, s), 1, p.D, lane), y1 = ldv(rec(p.ustep, s + 1), 1, p.D, lane);
             const V<R> f0 = ldv(rec(p.dense, s), 1, p.D, lane), f1 = ldv(rec(p.dense, s + 1), 1, p.D, lane);
-            V<R> Y0 = lam, Y1 = lam, F0{(R)0, (R)0};
+            V<R> D0{(R)0, (R)0}, D1{(R)0, (R)0}, F0{(R)0, (R)0};   // increments Y_j - lambda (kernel 5)
             for (int j = 0; j < p.S; ++j) {
                 const R Th = (R)1 - __ldg(p.rkc + RKC_C + j);
                 // x = (1 - Th) y0 + Th y1 + Th (Th - 1) ((1 - 2 Th) (y1 - y0) + (Th - 1) dt f0 + Th dt f1)
@@ -621,22 +622,20 @@ __global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
                     return ((R)1 - Th) * a0 + Th * a1 + Th * (Th - (R)1) * (((R)1 - (R)2 * Th) * (a1 - a0) + (Th - (R)1) * dt * g0 + Th * dt * g1);
                 };
                 const V<R> x{herm(y0.a, y1.a, f0.a, f1.a), herm(y0.b, y1.b, f0.b, f1.b)};
-                const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, j == 0 ? lam : Y1, dt * __ldg(p.rkc + RKC_W + j), gw, lane);
+                const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, V<R>{lam.a + D1.a, lam.b + D1.b}, dt * __ldg(p.rkc + RKC_W + j), gw, lane);
                 if (j == 0) {
                     F0 = F;
-                    Y0 = lam;
-                    Y1 = V<R>{fma(mt1 * dt, F0.a, lam.a), fma(mt1 * dt, F0.b, lam.b)};
+                    D1 = V<R>{mt1 * dt * F0.a, mt1 * dt * F0.b};
                 } else {
                     const R mu = __ldg(p.rkc + RKC_MU + j + 1), nu = __ldg(p.rkc + RKC_NU + j + 1), mt = __ldg(p.rkc + RKC_MT + j + 1),
                             ga = __ldg(p.rkc + RKC_GA + j + 1);
-                    const R c0 = (R)1 - mu - nu;
-                    const V<R> Y2{fma(ga * dt, F0.a, fma(mt * dt, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * lam.a)))),
-                                  fma(ga * dt, F0.b, fma(mt * dt, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * lam.b))))};
-                    Y0 = Y1;
-                    Y1 = Y2;
+                    const V<R> D2{fma(ga * dt, F0.a, fma(mt * dt, F.a, fma(nu, D0.a, mu * D1.a))),
+                                  fma(ga * dt, F0.b, fma(mt * dt, F.b, fma(nu, D0.b, mu * D1.b)))};
+                    D0 = D1;
+                    D1 = D2;
                 }
             }
-            lam = Y1;
+            lam = V<R>{lam.a + D1.a, lam.b + D1.b};
             if (s % p.save_every == 0) jump(s / p.save_every);
         }
         if (p.grad_u0) stv(p.grad_u0 + n, N, lam, p.D, lane);
@@ -711,19 +710,19 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_forward_kernel(Run<R> p)
         }
         const R *T = p.rkc + (size_t)(s - 2) * RKC_LEN;
         const R mt1 = __ldg(T);
-        V<R> Y0 = u, Y1{fma(mt1 * h, F0.a, u.a), fma(mt1 * h, F0.b, u.b)};
+        V<R> D0{(R)0, (R)0}, D1{mt1 * h * F0.a, mt1 * h * F0.b};   // increments Y_j - u (kernel 5)
         for (int j = 2; j <= s; ++j) {
-            const V<R> F = rhs(p, sm.ops, sm.th, Y1, lane);
+            const V<R> F = rhs(p, sm.ops, sm.th, V<R>{u.a + D1.a, u.b + D1.b}, lane);
             const R mu = __ldg(T + RKC_MU + j), nu = __ldg(T + RKC_NU + j), mt = __ldg(T + RKC_MT + j), ga = __ldg(T + RKC_GA + j);
-            const R c0 = (R)1 - mu - nu;
-            const V<R> Y2{fma(ga * h, F0.a, fma(mt * h, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * u.a)))),
-                          fma(ga * h, F0.b, fma(mt * h, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * u.b))))};
-            Y0 = Y1;
-            Y1 = Y2;
+            const V<R> D2{fma(ga * h, F0.a, fma(mt * h, F.a, fma(nu, D0.a, mu * D1.a))),
+                          fma(ga * h, F0.b, fma(mt * h, F.b, fma(nu, D0.b, mu * D1.b)))};
+            D0 = D1;
+            D1 = D2;
         }
-        un = Y1;
+        un = V<R>{u.a + D1.a, u.b + D1.b};
         F1 = rhs(p, sm.ops, sm.th, un, lane);
-        const R ea = fma((R)0.4 * h, F0.a + F1.a, (R)0.8 * (u.a - un.a)), eb = fma((R)0.4 * h, F0.b + F1.b, (R)0.8 * (u.b - un.b));
+        // u_n - u_{n+1} = -D_s
+        const R ea = fma((R)0.4 * h, F0.a + F1.a, (R)-0.8 * D1.a), eb = fma((R)0.4 * h, F0.b + F1.b, (R)-0.8 * D1.b);
         const R EEst = PR::sq(wsum(sq2(ea, eb, fmax(fabs(u.a), fabs(un.a)), fmax(fabs(u.b), fabs(un.b)))) / Dr);
         if (!(EEst <= PR::huge)) { bad = 1; break; }   // NaN / Inf
         if (pi.judge(EEst)) {
@@ -802,26 +801,24 @@ __global__ void __launch_bounds__(128) rkc2_adaptive_adjoint_kernel(Run<R> p)
                 const R ts = p.t0 + p.save_dt * (R)isave;
                 const R ta = (isave >= 0 && ts > tn + eps) ? ts : tn;
                 const R h = cur - ta;
-                V<R> Y0 = lam, Y1 = lam, F0{(R)0, (R)0};
+                V<R> D0{(R)0, (R)0}, D1{(R)0, (R)0}, F0{(R)0, (R)0};   // increments Y_j - lambda (kernel 5)
                 for (int j = 0; j < s; ++j) {
                     const R Th = fmin(fmax((cur - __ldg(T + RKC_C + j) * h - tn) / hn, (R)0), (R)1);
                     const V<R> x{herm3(Th, hn, y0.a, y1.a, f0.a, f1.a), herm3(Th, hn, y0.b, y1.b, f0.b, f1.b)};
-                    const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, j == 0 ? lam : Y1, h * __ldg(T + RKC_W + j), gw, lane);
+                    const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, V<R>{lam.a + D1.a, lam.b + D1.b}, h * __ldg(T + RKC_W + j), gw, lane);
                     if (j == 0) {
                         F0 = F;
-                        Y0 = lam;
-                        Y1 = V<R>{fma(mt1 * h, F0.a, lam.a), fma(mt1 * h, F0.b, lam.b)};
+                        D1 = V<R>{mt1 * h * F0.a, mt1 * h * F0.b};
                     } else {
                         const R mu = __ldg(T + RKC_MU + j + 1), nu = __ldg(T + RKC_NU + j + 1), mt = __ldg(T + RKC_MT + j + 1),
                                 ga = __ldg(T + RKC_GA + j + 1);
-                        const R c0 = (R)1 - mu - nu;
-                        const V<R> Y2{fma(ga * h, F0.a, fma(mt * h, F.a, fma(nu, Y0.a, fma(mu, Y1.a, c0 * lam.a)))),
-                                      fma(ga * h, F0.b, fma(mt * h, F.b, fma(nu, Y0.b, fma(mu, Y1.b, c0 * lam.b))))};
-                        Y0 = Y1;
-                        Y1 = Y2;
+                        const V<R> D2{fma(ga * h, F0.a, fma(mt * h, F.a, fma(nu, D0.a, mu * D1.a))),
+                                      fma(ga * h, F0.b, fma(mt * h, F.b, fma(nu, D0.b, mu * D1.b)))};
+                        D0 = D1;
+                        D1 = D2;
                     }
                 }
-                lam = Y1;
+                lam = V<R>{lam.a + D1.a, lam.b + D1.b};
                 cur = ta;
                 if (isave >= 0 && fabs(ts - ta) <= eps) { jump(isave); --isave; }
             }
