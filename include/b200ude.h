@@ -202,7 +202,12 @@ typedef struct b200ude_desc {
     double consts[16];    /* fixed physics constants */
     int32_t solver;       /* B200UDE_TSIT5 | B200UDE_VERN7 | B200UDE_RKC2 */
     int32_t sensealg;     /* B200UDE_INTERPOLATING_ADJOINT | B200UDE_DISCRETE_ADJOINT */
-    double t0;            /* tspan[1] */
+    double t0;            /* tspan[1], the absolute start time.  Every kernel runs on s = t - t0, so step and save times keep the
+                             float spacing of the span, whatever |t0| (at t0 = 1900, ulp(t) = 1.2e-4 in fp32).  The autonomous
+                             models (LV, SEIR, NODE, Fisher-KPP, operator) never read t: their results do not depend on t0, bit
+                             for bit.  B200UDE_MODEL_FORCED reads t in its forcing: b200ude_set_forcing folds w_j t0 into each
+                             phase, phi_j + w_j t0 reduced mod 2 pi in double, so gamma(t) = sum A_j cos(w_j s + phi_j') is the
+                             forcing at absolute t; with t0 = 0 the coefficients are used as given. */
     double dt;            /* fixed step (adaptive = false); saveat = t0 + i*save_every*dt */
     int32_t n_steps;      /* number of steps; tspan[2] = t0 + n_steps*dt */
     int32_t save_every;   /* save the state every this many steps (and at t0) */

@@ -344,10 +344,13 @@ Adj64Host adj_params(const b200ude_handle *h, const double *cot, double *grad_u0
     return Adj64Host{(const double *)h->d_ustep, (const double *)h->d_dense, cot, grad_u0, (double *)h->d_partial, (int)h->N, h->desc.n_steps,
                      h->desc.save_every, l2 ? 1 : 0, h->desc.dt};
 }
+// Every kernel runs on the time axis s = t - t0, so the origin it is given is 0.  The autonomous models never see t, and this
+// keeps the float spacing of their step and save times that of the span, not of |t0| (at t0 = 1900, ulp(t) = 1.2e-4 in fp32).
+// The forced model, the one model that reads t, has W t0 folded into its phases instead (b200ude_set_forcing).
 template <typename R>
 typename RealParams<R>::Adapt adapt(const b200ude_handle *h)
 {
-    return {(R)h->desc.t0, (R)(h->desc.dt * h->desc.save_every), (R)h->desc.abstol, (R)h->desc.reltol, h->n_save, h->desc.max_steps,
+    return {(R)0, (R)(h->desc.dt * h->desc.save_every), (R)h->desc.abstol, (R)h->desc.reltol, h->n_save, h->desc.max_steps,
             (R *)h->d_tgrid, h->d_nacc, (R *)h->d_hstep};
 }
 template <typename R>
@@ -702,7 +705,7 @@ ForcedRun forced_run(const b200ude_handle *h, size_t N)
     r.usave = h->d_usave;
     r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.adaptive = h->adaptive ? 1 : 0;
     r.n_save = h->n_save; r.max_steps = h->desc.max_steps; r.fstride = (int)h->cap;
-    r.t0 = h->desc.t0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;
+    r.t0 = 0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;   // s = t - t0 (adapt)
     return r;
 }
 
@@ -775,7 +778,7 @@ OperatorRun operator_run(const b200ude_handle *h, size_t N)
     r.sstep = h->d_sstep;
     r.N = (int)N; r.n_steps = h->desc.n_steps; r.save_every = h->desc.save_every; r.n_save = h->n_save; r.max_steps = h->desc.max_steps;
     r.adaptive = h->adaptive ? 1 : 0;
-    r.t0 = h->desc.t0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;
+    r.t0 = 0; r.dt = h->desc.dt; r.save_dt = h->desc.dt * h->desc.save_every; r.abstol = h->desc.abstol; r.reltol = h->desc.reltol;   // s = t - t0 (adapt)
     return r;
 }
 
@@ -1172,6 +1175,8 @@ int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32
     const size_t es = h->es();
     CUDA_TRY(h, cudaMemcpy2DAsync(h->d_forcing, es * h->cap, coef, es * N, es * N, (size_t)3 * h->fh.J,
                                   mem == B200UDE_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    // the kernels run on s = t - t0: cos(W t + F) = cos(W s + (F + W t0)).  t0 = 0 leaves the coefficients as given.
+    if (h->desc.t0 != 0) CUDA_TRY(h, launch_fold_forcing(h->fh.dtype, h->d_forcing, h->fh.J, (int)h->cap, (int)N, h->desc.t0, (cudaStream_t)stream));
     h->forcing_n = N;
     return B200UDE_OK;
 }

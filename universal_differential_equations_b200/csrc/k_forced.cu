@@ -116,6 +116,28 @@ static cudaError_t adj(const ForcedHost &h, const ForcedRun &r, cudaStream_t st,
     return cudaGetLastError();
 }
 
+// the forcing on the kernels' time axis s = t - t0: cos(w t + phi) = cos(w s + (phi + w t0)).  The sum is taken in double without
+// contraction (as  phi + w * t0  evaluates on the host) and reduced to [-pi, pi] exactly, then rounded once to R.
+template <typename R>
+__global__ void fold_forcing_kernel(R *coef, int J, int fstride, int N, double t0)
+{
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n >= N) return;
+    for (int j = 0; j < J; ++j) {
+        const double w = coef[(size_t)(3 * j + 1) * fstride + n];
+        R &phi = coef[(size_t)(3 * j + 2) * fstride + n];
+        phi = (R)remainder(__dadd_rn((double)phi, __dmul_rn(w, t0)), 6.283185307179586476925);
+    }
+}
+
+cudaError_t launch_fold_forcing(int dtype, void *forcing, int J, int fstride, int N, double t0, cudaStream_t st)
+{
+    const int grid = (N + 127) / 128;
+    if (dtype == 1) fold_forcing_kernel<double><<<grid, 128, 0, st>>>((double *)forcing, J, fstride, N, t0);
+    else fold_forcing_kernel<float><<<grid, 128, 0, st>>>((float *)forcing, J, fstride, N, t0);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_fwd_forced(const ForcedHost &h, const ForcedRun &r, cudaStream_t st)
 {
     return h.dtype == 1 ? fwd<forced::Ops64, FORCED_BLOCK64>(h, r, st) : fwd<forced::Ops32, FORCED_BLOCK32>(h, r, st);

@@ -247,11 +247,13 @@ struct ForcedRun {
     int32_t *status;
     int *nacc;
     int N, n_steps, save_every, fused_l2, adaptive, n_save, max_steps, fstride;
-    double t0, dt, save_dt, abstol, reltol;
+    double t0, dt, save_dt, abstol, reltol;   // t0: the origin of the kernels' time axis (0: they run on t - desc.t0)
 };
 int adj_rows_forced(int N, int dtype);
 cudaError_t launch_fwd_forced(const ForcedHost &, const ForcedRun &, cudaStream_t);
 cudaError_t launch_adj_forced(const ForcedHost &, const ForcedRun &, cudaStream_t, int *rows_out);
+// phi_j -> remainder(phi_j + w_j t0, 2 pi), in double, for the first N trajectories of the forcing [3J][fstride] (in place)
+cudaError_t launch_fold_forcing(int dtype, void *forcing, int J, int fstride, int N, double t0, cudaStream_t);
 
 // ---- wide-state operator UDE du = D1 NN(u) + D2 u (B200UDE_MODEL_OPERATOR; operator.cuh, k_operator.cu), fp32 and fp64 ----
 struct OperatorHost {
