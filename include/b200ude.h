@@ -169,6 +169,23 @@ extern "C" {
                                          without it.
                                        B200UDE_EUNSUPPORTED with the interpolating adjoint, together with B200UDE_FLAG_VERN7_DENSE,
                                        with Tsit5, RKC2 or the Fisher-KPP UPDE. */
+#define B200UDE_FLAG_CHECKPOINT 8u /* InterpolatingAdjoint(checkpointing = true): a checkpointed step record for adaptive Tsit5 with
+                                       the interpolating adjoint on the Fisher-KPP UPDE (B200UDE_MODEL_FKPP, adaptive = 1), fp32 and
+                                       fp64, every reaction chain and grid that configuration accepts (the 1-16-16-1 chain included).
+                                       - the forward runs the same steps and returns bitwise the same out and status; it keeps u_n
+                                         only every K accepted steps and the size of every accepted step, no stage derivatives;
+                                       - the adjoint takes the segments of K steps last to first, recomputes each one's states and
+                                         stages from its checkpoint with the recorded step sizes, and replays it as without the flag:
+                                         the gradients are bitwise those without the flag, for about one more evaluation of the
+                                         accepted steps' right-hand sides per adjoint.
+                                       K = max(1, round(sqrt(max_steps / 7))).  Record per trajectory, in reals:
+                                       (ceil(max_steps / K) + 1 + 7K + 2) * state_dim + (2 max_steps + 1) (checkpoints, scratch of one
+                                       segment, step sizes and step times) instead of (7 max_steps + 2) * state_dim + max_steps + 1;
+                                       b200ude_device_bytes reports it.  Deviation from SciMLSensitivity: its checkpointed adjoint
+                                       re-solves each interval between checkpoints with error control, so its gradient moves by about
+                                       the tolerance; here the forward's own accepted steps are replayed with their recorded sizes,
+                                       so nothing moves.  B200UDE_EUNSUPPORTED on every other configuration: fixed step, Vern7, RKC2,
+                                       the discrete adjoint, and every other model. */
 
 /* per-trajectory status words written by b200ude_forward */
 #define B200UDE_TRAJ_OK 0

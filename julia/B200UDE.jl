@@ -43,6 +43,7 @@ const INTERPOLATING_ADJOINT, DISCRETE_ADJOINT = Int32(0), Int32(1)
 const HOST, DEVICE = Int32(0), Int32(1)
 const FLAG_VERN7_DENSE = UInt32(2)
 const FLAG_DISCRETE_DENSE = UInt32(4)
+const FLAG_CHECKPOINT = UInt32(8)
 
 Base.@kwdef mutable struct Desc            # mirrors struct b200ude_desc
     struct_size::UInt32 = 0;  device::Int32 = 0;  dtype::Int32 = F32;  model::Int32 = 0

@@ -23,6 +23,7 @@ HOST, DEVICE = 0, 1
 FLAG_APPROX_TANH = 1
 FLAG_VERN7_DENSE = 2
 FLAG_DISCRETE_DENSE = 4
+FLAG_CHECKPOINT = 8
 OK, EINVAL, EUNSUPPORTED, ESTATE, ENOMEM, ENODEVICE = 0, -1, -2, -3, -4, -5
 MAX_LAYERS = 6
 

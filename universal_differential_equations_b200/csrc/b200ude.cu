@@ -96,7 +96,8 @@ struct b200ude_handle {
     // adaptive stepping
     bool adaptive = false;
     void *d_tgrid = nullptr, *d_cot = nullptr;
-    void *d_hstep = nullptr;   // discrete-adjoint Vern7: step sizes of the accepted steps
+    void *d_hstep = nullptr;   // discrete-adjoint Vern7, checkpointed Fisher-KPP: step sizes of the accepted steps
+    int seg = 0;               // B200UDE_FLAG_CHECKPOINT: accepted steps per checkpoint (d_ustep: checkpoints, d_dense: scratch), else 0
     float *d_block_loss = nullptr;
     int *d_nacc = nullptr;
     const void *last_out = nullptr;
@@ -424,7 +425,7 @@ cudaError_t launch_forward(b200ude_handle *h, const typename RealParams<R>::Fwd 
     if constexpr (is_f32<R>)
         if (fp32_only(h)) return forward32(h, p, N, solver, st);
     const auto ag = adapt<R>(h);
-    if (h->kid == K_FKPP) return RuntimeShape<R>::fwd_fkpp_adaptive(h->gen, tables<R>(h), p, ag, st);   // adaptive Tsit5 (b200ude_create)
+    if (h->kid == K_FKPP) return RuntimeShape<R>::fwd_fkpp_adaptive(h->gen, tables<R>(h), p, ag, h->seg, st);   // adaptive Tsit5 (b200ude_create)
     return RuntimeShape<R>::fwd(h->gen, tables<R>(h), p, solver, h->adaptive ? &ag : nullptr, st);
 }
 
@@ -436,7 +437,7 @@ cudaError_t launch_adjoint(b200ude_handle *h, const typename RealParams<R>::Adj 
     if constexpr (is_f32<R>)
         if (fp32_only(h)) return adjoint32(h, p, split, split_at, st, rows);
     const auto ag = adapt<R>(h);
-    if (h->kid == K_FKPP) return RuntimeShape<R>::adj_fkpp_adaptive(h->gen, tables<R>(h), p, ag, st, rows);
+    if (h->kid == K_FKPP) return RuntimeShape<R>::adj_fkpp_adaptive(h->gen, tables<R>(h), p, ag, h->seg, st, rows);
     return RuntimeShape<R>::adj(h->gen, tables<R>(h), p, h->adaptive ? &ag : nullptr, st, rows);
 }
 
@@ -957,6 +958,11 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (d->max_trajectories == 0 || d->max_trajectories > (1ull << 26)) return fail(nullptr, B200UDE_EINVAL, "create: max_trajectories out of range");
     const bool op = d->model == B200UDE_MODEL_OPERATOR, forced = d->model == B200UDE_MODEL_FORCED, want64 = d->dtype == B200UDE_F64;
     // the descriptor is validated before the device check, so that it is testable without a GPU
+    if ((d->flags & B200UDE_FLAG_CHECKPOINT) &&
+        !(d->model == B200UDE_MODEL_FKPP && d->adaptive && d->solver == B200UDE_TSIT5 && d->sensealg == B200UDE_INTERPOLATING_ADJOINT))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_FLAG_CHECKPOINT applies to adaptive Tsit5 with the interpolating adjoint on the Fisher-KPP UPDE; not to "
+                    "fixed step, Vern7, RKC2, the discrete adjoint or other models");
     KernelId kid = K_OPERATOR;
     int32_t rc = op ? operator_check(d) : select_kernel(d, &kid);
     if (rc) return rc;
@@ -1039,11 +1045,17 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     // a discrete-adjoint or dense-output Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead when adaptive
     const bool disc_vern7 = (h->var.discrete && d->solver == B200UDE_VERN7) || h->vern7_dense;
     const size_t dense_rows = oh.rkc2 ? rec + 1 : rec * 6 + 1;   // operator RKC2: f(u_n); Tsit5: the stages
+    // B200UDE_FLAG_CHECKPOINT (adaptive Tsit5 Fisher-KPP only, checked above): u_n every K accepted steps in place of ustep, the
+    // adjoint's scratch area for one segment (6K + 1 stage rows, K + 1 state rows) in place of dense, the step sizes.  K minimises
+    // max_steps / K + 7K, the rows of both
+    if (d->flags & B200UDE_FLAG_CHECKPOINT) h->seg = std::max(1, (int)std::lround(std::sqrt((double)d->max_steps / 7.0)));
+    const size_t seg = (size_t)h->seg;
+    const size_t ustep_rows = seg ? (rec + seg - 1) / seg + 1 : rec + 1, dense_alloc = seg ? 7 * seg + 2 : dense_rows;
     // theta: the fp32 runtime-shape and tuned kernels read it as float4
     const size_t theta_n = want64 || forced || op ? (size_t)P + 1 : (size_t)((P + 3) / 4) * 4;
     h->partial_blocks = partial_rows(h);
-    bool ok = dalloc_real(h, &h->d_theta, theta_n) == cudaSuccess && dalloc_real(h, &h->d_ustep, (rec + 1) * D * N) == cudaSuccess &&
-              (disc_vern7 || dalloc_real(h, &h->d_dense, dense_rows * D * N) == cudaSuccess) &&
+    bool ok = dalloc_real(h, &h->d_theta, theta_n) == cudaSuccess && dalloc_real(h, &h->d_ustep, ustep_rows * D * N) == cudaSuccess &&
+              (disc_vern7 || dalloc_real(h, &h->d_dense, dense_alloc * D * N) == cudaSuccess) &&
               dalloc_real(h, &h->d_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess;
     if (!want64) ok = ok && dalloc(h, &h->d_grad, (size_t)P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
     if (h->adaptive) {
@@ -1052,7 +1064,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
             ok = ok && dalloc_real(h, &h->d_usave, (size_t)h->n_save * D * N) == cudaSuccess;
         else   // the cotangent of the fused L2 and, in fp32, its per-block losses
             ok = ok && dalloc_real(h, &h->d_cot, (size_t)h->n_save * D * N) == cudaSuccess &&
-                 (!disc_vern7 || dalloc_real(h, &h->d_hstep, rec * N) == cudaSuccess) &&
+                 (!(disc_vern7 || seg) || dalloc_real(h, &h->d_hstep, rec * N) == cudaSuccess) &&
                  (want64 || dalloc(h, &h->d_block_loss, (size_t)L2_BLOCKS) == cudaSuccess);
     }
     if (forced) ok = ok && dalloc_real(h, &h->d_forcing, 3 * (size_t)d->consts[1] * N) == cudaSuccess;

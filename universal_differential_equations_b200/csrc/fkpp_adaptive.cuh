@@ -19,6 +19,14 @@
 //
 // `Ops` is the precision of the runtime-shape model layer (ude_generic.cuh): k_generic.cu: fp32 over the constant bank (Ops32);
 // k_f64.cu: fp64 over the handle's theta (Ops64).
+//
+// CKPT (B200UDE_FLAG_CHECKPOINT, InterpolatingAdjoint(checkpointing = true)): the forward keeps u_n only at n = 0, K, 2K, ...
+// (`ustep` holds those checkpoints) and the step size h_n of every accepted step (`hstep`), no `dense` record.  The adjoint takes
+// the segments of K accepted steps from the last to the first: it recomputes a segment's u_n and k_1..k_7 from its checkpoint and
+// the recorded h_n into a per-trajectory scratch area, with the stage code of the forward (tsit5_stages), and replays the segment
+// from there exactly as the full-record adjoint replays it from `ustep` / `dense`.  The recomputed record is bitwise the forward's,
+// so the gradients are bitwise those of the full record.  K = max(1, round(sqrt(max_steps / 7))) (b200ude_create) makes the
+// checkpoint rows (max_steps / K + 1) plus the scratch rows (7K + 2) smallest.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -61,6 +69,9 @@ struct Fwd {
     int *nacc;          // [N]
     int N, Nx, tpc, n_save, max_steps;
     R t0, save_dt, abstol, reltol;
+    // CKPT only: ustep is then [ceil(max_steps/seg)+1][N][Nx], u_n at n = 0, seg, 2 seg, ...; dense is not written
+    R *hstep;           // [max_steps][N] h_n of every accepted step
+    int seg;            // K, accepted steps per checkpoint
 };
 
 template <typename R>
@@ -72,6 +83,10 @@ struct Adj {
     R *partial;         // [gridDim.x * nwarps][P+1]
     int N, Nx, tpc, n_save;
     R t0, save_dt;
+    // CKPT only: ustep holds the forward's checkpoints, dense is not read
+    const R *hstep;     // [max_steps][N]
+    R *scratch;         // [6 seg + 1][N][Nx] stage derivatives, then [seg + 1][N][Nx] u_n, of the segment being replayed
+    int seg;
 };
 
 // the chain at one grid point (one input, one output), and its VJP: returns dx, this warp's gradient vector += w (dchain/dtheta)^T dy
@@ -101,6 +116,45 @@ __device__ __forceinline__ void exchange(R *sU, int slot, int base, int i, int N
     __syncthreads();
 }
 
+// the right-hand side at the trajectory's point i (two barriers: every thread of the CTA calls it)
+template <class Ops>
+struct PointRhs {
+    using R = typename Ops::real;
+    R *sU;
+    int slot, base, i, Nx;
+    bool valid;
+    R w1, w2, w3, D0;
+    __device__ __forceinline__ R operator()(R g) const
+    {
+        R gm, gp;
+        exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
+        const R y = point_chain<Ops>(g);
+        return fma(D0, fma(w1, gm, fma(w2, g, w3 * gp)), y);
+    }
+};
+
+// stages 2..7 of one Tsit5 step of size h from u, k[0] = f(u): fills k[1..6] and returns the step's end state (the 7th stage's
+// argument).  The forward's attempts and the checkpointed adjoint's recomputation of the accepted steps both run this code, so the
+// recomputed stages are bitwise the forward's.
+template <class Ops>
+__device__ __forceinline__ typename Ops::real tsit5_stages(const PointRhs<Ops> &rhs, typename Ops::real u, typename Ops::real h,
+                                                           typename Ops::real (&k)[7])
+{
+    using R = typename Ops::real;
+    R un = u;
+#pragma unroll
+    for (int st = 1; st < 7; ++st) {
+        R acc = (R)0;
+#pragma unroll
+        for (int j = 0; j < st; ++j)
+            if (Tsit5::a(st, j) != 0.0) acc = fma((R)Tsit5::a(st, j), k[j], acc);
+        const R g = fma(h, acc, u);
+        if (st == 6) un = g;
+        k[st] = rhs(g);
+    }
+    return un;
+}
+
 // sum of v over the trajectory's Nx points, in point order; every thread of the trajectory returns the same value
 template <typename R>
 __device__ __forceinline__ R traj_sum(R *sE, int slot, int base, int Nx, bool valid, R v)
@@ -113,7 +167,7 @@ __device__ __forceinline__ R traj_sum(R *sE, int slot, int base, int Nx, bool va
     return acc;
 }
 
-template <class Ops>
+template <class Ops, bool CKPT>
 __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
 {
     using R = typename Ops::real;
@@ -134,12 +188,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
     const R big = Prec<R>::huge;
     const int sx = Ops::P() - 5;
     const R w1 = Ops::theta(sx), w2 = Ops::theta(sx + 1), w3 = Ops::theta(sx + 2), D0 = Ops::theta(sx + 4);
-    auto rhs = [&](R g) {
-        R gm, gp;
-        exchange(sU, slot, base, i, Nx, valid, g, gm, gp);
-        const R y = point_chain<Ops>(g);
-        return fma(D0, fma(w1, gm, fma(w2, g, w3 * gp)), y);
-    };
+    const PointRhs<Ops> rhs{sU, slot, base, i, Nx, valid, w1, w2, w3, D0};
     auto rms = [&](R v) { return Prec<R>::sq(traj_sum(sE, slot, base, Nx, valid, v) / (R)Nx); };
     auto store_int = [&](R *b, int row, R v) { if (live) b[((size_t)row * N + n) * Nx + i] = v; };
     auto store_abi = [&](R *b, int row, R v) { if (live) b[((size_t)row * Nx + i) * N + n] = v; };
@@ -150,7 +199,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
     if (live && i == 0) p.tgrid[n] = t0;
     R k[7];
     k[0] = rhs(u);
-    store_int(p.dense, 0, k[0]);
+    if (!CKPT) store_int(p.dense, 0, k[0]);
     // initial step: Hairer-Norsett-Wanner as in OrdinaryDiffEq, norms over the trajectory
     PIControl<R, 5> pi;
     {
@@ -170,17 +219,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
         R h = done ? (R)0 : pi.dt;
         bool clipped = false;
         if (!done && t + h >= t1 - ttol * fabs(t1)) { h = t1 - t; clipped = true; }
-        R un = u;
-#pragma unroll
-        for (int st = 1; st < 7; ++st) {
-            R acc = (R)0;
-#pragma unroll
-            for (int j = 0; j < st; ++j)
-                if (Tsit5::a(st, j) != 0.0) acc = fma((R)Tsit5::a(st, j), k[j], acc);
-            const R g = fma(h, acc, u);
-            if (st == 6) un = g;
-            k[st] = rhs(g);
-        }
+        const R un = tsit5_stages(rhs, u, h, k);
         R e = (R)0;
 #pragma unroll
         for (int j = 0; j < 7; ++j) e = fma((R)Tsit5::bt(j), k[j], e);
@@ -192,8 +231,13 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
         if (pi.judge(EEst)) {
             if (nacc >= p.max_steps) { bad = 2; done = true; continue; }
             const R tn = clipped ? t1 : t + h;
-            // dense record of this step: k_1..k_6 at rows nacc*6 + st, k_7 at (nacc+1)*6 (= k_1 of the next step)
-            for (int st = 1; st < 7; ++st) store_int(p.dense, nacc * 6 + st, k[st]);
+            // dense record of this step: k_1..k_6 at rows nacc*6 + st, k_7 at (nacc+1)*6 (= k_1 of the next step); checkpointed:
+            // the step size, from which the adjoint recomputes them (t_{n+1} - t_n is not h_n bitwise)
+            if (CKPT) {
+                if (live && i == 0) p.hstep[(size_t)nacc * N + n] = h;
+            } else {
+                for (int st = 1; st < 7; ++st) store_int(p.dense, nacc * 6 + st, k[st]);
+            }
             while (isave < p.n_save) {
                 const R ts = t0 + p.save_dt * (R)isave;
                 if (ts > tn + ttol * fabs(tn)) break;
@@ -211,7 +255,8 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
             if (live && i == 0) p.tgrid[(size_t)nacc * N + n] = t;
             u = un;
             k[0] = k[6];
-            store_int(p.ustep, nacc, u);
+            if (!CKPT) store_int(p.ustep, nacc, u);
+            else if (nacc % p.seg == 0) store_int(p.ustep, nacc / p.seg, u);
             if (isave >= p.n_save) done = true;
         } else {
             pi.reject(h);
@@ -228,7 +273,7 @@ __global__ void __launch_bounds__(256) forward_kernel(Fwd<typename Ops::real> p)
     }
 }
 
-template <class Ops>
+template <class Ops, bool CKPT>
 __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
 {
     using R = typename Ops::real;
@@ -262,14 +307,15 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
     int isave = p.n_save - 1;
     if (live) lam += cot(isave);
     --isave;
-    for (int s = nmax - 1; s >= 0; --s) {
-        // trajectories past their own record shadow step 0 (their initial state) with weight 0
+    // the replay of accepted step s, whose u_n and k_1..k_7 are rows r and 6r..6r+6 of ust / den
+    auto replay = [&](int s, const R *ust, const R *den, int r) {
+        // trajectories past their own record shadow step 0 (their initial state, row 0 of the record) with weight 0
         const bool act_s = live && s < nacc;
-        const int sc_ = act_s ? s : 0;
+        const int sc_ = act_s ? s : 0, rc = act_s ? r : 0;
         const R tn = act_s ? p.tgrid[(size_t)sc_ * N + n] : (R)0;
         const R tn1 = act_s ? p.tgrid[(size_t)(sc_ + 1) * N + n] : (R)0;
         const R hn = tn1 - tn, eps = eps_rel * hn;
-        const R u_n = p.ustep[((size_t)sc_ * N + n) * Nx + i];
+        const R u_n = (act_s ? ust : p.ustep)[((size_t)rc * N + n) * Nx + i];
         R cur = tn1;
         while (true) {
             const bool has = act_s && cur > tn + eps;   // uniform over the trajectory
@@ -286,7 +332,7 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
                     Tsit5::weights(fmin(fmax((cur - (R)Tsit5::c(st) * h - tn) / hn, (R)0), (R)1), bw);
                     R acc = (R)0;
 #pragma unroll
-                    for (int j = 0; j < 7; ++j) acc = fma(bw[j], p.dense[((size_t)(sc_ * 6 + j) * N + n) * Nx + i], acc);
+                    for (int j = 0; j < 7; ++j) acc = fma(bw[j], den[((size_t)(rc * 6 + j) * N + n) * Nx + i], acc);
                     x = fma(hn, acc, u_n);
                 }
                 R a2 = (R)0;
@@ -314,6 +360,38 @@ __global__ void __launch_bounds__(256) adjoint_kernel(Adj<typename Ops::real> p)
                 cur = ta;
                 if (isave >= 0 && fabs(ts - ta) <= eps) { lam += cot(isave); --isave; }
             }
+        }
+    };
+    if constexpr (!CKPT) {
+        for (int s = nmax - 1; s >= 0; --s) replay(s, p.ustep, p.dense, s);
+    } else {
+        // segments [s0, s0 + len) of K accepted steps, last first; len is CTA-uniform (nmax), so is every barrier of the recomputation
+        const int K = p.seg;
+        const PointRhs<Ops> rhs{sU, slot, base, i, Nx, valid, w1, w2, w3, D0};
+        R *sk = p.scratch, *su = p.scratch + (size_t)(6 * K + 1) * N * Nx;
+        auto store = [&](R *b, int row, R v) { if (live) b[((size_t)row * N + n) * Nx + i] = v; };
+        for (int s0 = nmax > 0 ? (nmax - 1) / K * K : -1; s0 >= 0; s0 -= K) {
+            const int len = min(K, nmax - s0);
+            // 1. the segment's u_n and stages from its checkpoint and the recorded h_n; a trajectory past its own record steps
+            // with h = 0 and stores nothing
+            const bool act0 = live && s0 < nacc;
+            R u = p.ustep[((size_t)(act0 ? s0 / K : 0) * N + n) * Nx + i];
+            R k[7];
+            k[0] = rhs(u);   // = the forward's k_7 of step s0 - 1 (FSAL)
+            if (act0) { store(su, 0, u); store(sk, 0, k[0]); }
+            for (int j = 0; j < len; ++j) {
+                const bool act = live && s0 + j < nacc;
+                const R h = act ? p.hstep[(size_t)(s0 + j) * N + n] : (R)0;
+                const R un = tsit5_stages(rhs, u, h, k);
+                if (act) {
+                    for (int st = 1; st < 7; ++st) store(sk, j * 6 + st, k[st]);
+                    store(su, j + 1, un);
+                }
+                u = un;
+                k[0] = k[6];
+            }
+            // 2. its replay, read from the scratch area (each thread reads back only what it wrote)
+            for (int s = s0 + len - 1; s >= s0; --s) replay(s, su, sk, s - s0);
         }
     }
     if (p.grad_u0 && live) p.grad_u0[(size_t)i * N + n] = lam;

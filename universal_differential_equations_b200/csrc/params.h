@@ -105,7 +105,7 @@ struct AdaptiveGrid {
     int n_save, max_steps;
     float *tgrid;   // [max_steps+1][N]
     int *nacc;      // [N]
-    float *hstep;   // [max_steps][N] step sizes (discrete-adjoint Vern7 handles only, else nullptr)
+    float *hstep;   // [max_steps][N] step sizes (discrete-adjoint Vern7 and checkpointed Fisher-KPP handles only, else nullptr)
 };
 constexpr int L2_BLOCKS = 296;
 
@@ -179,7 +179,7 @@ struct Adapt64Host {
     int n_save, max_steps;
     double *tgrid;
     int *nacc;
-    double *hstep;   // discrete-adjoint Vern7 handles only, else nullptr
+    double *hstep;   // discrete-adjoint Vern7 and checkpointed Fisher-KPP handles only, else nullptr
 };
 template <typename R>
 struct RealParams;
@@ -220,9 +220,10 @@ struct RuntimeShape {
     // discrete adjoint of that adaptive forward through its interpolated saves (vern7_dense_discrete.cuh, B200UDE_FLAG_DISCRETE_DENSE)
     static cudaError_t adj_vern7_dense_discrete(const GenericShape &, const Tab &, const Adj &, const Adapt &, const R *saved, cudaStream_t,
                                                 int *rows_out);
-    // adaptive Tsit5 of the Fisher-KPP UPDE (fkpp_adaptive.cuh)
-    static cudaError_t fwd_fkpp_adaptive(const GenericShape &, const Tab &, const Fwd &, const Adapt &, cudaStream_t);
-    static cudaError_t adj_fkpp_adaptive(const GenericShape &, const Tab &, const Adj &, const Adapt &, cudaStream_t, int *rows_out);
+    // adaptive Tsit5 of the Fisher-KPP UPDE (fkpp_adaptive.cuh).  seg = 0: the full step record (p.ustep, p.dense); seg = K
+    // (B200UDE_FLAG_CHECKPOINT): p.ustep holds u_n every K accepted steps, ag.hstep the step sizes, p.dense the adjoint's scratch area
+    static cudaError_t fwd_fkpp_adaptive(const GenericShape &, const Tab &, const Fwd &, const Adapt &, int seg, cudaStream_t);
+    static cudaError_t adj_fkpp_adaptive(const GenericShape &, const Tab &, const Adj &, const Adapt &, int seg, cudaStream_t, int *rows_out);
     // adaptive Vern7 of the Fisher-KPP UPDE with the discrete adjoint (fkpp_vern7_discrete.cuh): same geometry and shared memory as
     // adaptive Tsit5; the record is p.ustep / ag.tgrid / ag.hstep / ag.nacc; p.fused_l2 reads the recorded step-end states
     static cudaError_t fwd_fkpp_vern7(const GenericShape &, const Tab &, const Fwd &, const Adapt &, cudaStream_t);

@@ -145,7 +145,7 @@ cudaError_t RuntimeShape<R>::adj_vern7_dense_discrete(const GenericShape &g, con
 }
 
 template <typename R>
-cudaError_t RuntimeShape<R>::fwd_fkpp_adaptive(const GenericShape &g, const Tab &t, const Fwd &p, const Adapt &ag, cudaStream_t st)
+cudaError_t RuntimeShape<R>::fwd_fkpp_adaptive(const GenericShape &g, const Tab &t, const Fwd &p, const Adapt &ag, int seg, cudaStream_t st)
 {
     using U = ShapeUnit<R>;
     cudaError_t e = U::upload(g, t, st);
@@ -156,11 +156,14 @@ cudaError_t RuntimeShape<R>::fwd_fkpp_adaptive(const GenericShape &g, const Tab 
     q.u0 = p.u0; q.out = p.out; q.ustep = p.ustep; q.dense = p.dense; q.status = p.status; q.tgrid = ag.tgrid; q.nacc = ag.nacc;
     q.N = p.N; q.Nx = g.D; q.n_save = ag.n_save; q.max_steps = ag.max_steps;
     q.t0 = ag.t0; q.save_dt = ag.save_dt; q.abstol = ag.abstol; q.reltol = ag.reltol;
-    return shape_launch::fkpp(fkpp_adapt::forward_kernel<typename U::Ops>, q, th, fkpp_adapt::fwd_smem(g.D, sizeof(R)), st, nullptr);
+    q.hstep = ag.hstep; q.seg = seg;
+    const size_t smem = fkpp_adapt::fwd_smem(g.D, sizeof(R));
+    if (seg) return shape_launch::fkpp(fkpp_adapt::forward_kernel<typename U::Ops, true>, q, th, smem, st, nullptr);
+    return shape_launch::fkpp(fkpp_adapt::forward_kernel<typename U::Ops, false>, q, th, smem, st, nullptr);
 }
 
 template <typename R>
-cudaError_t RuntimeShape<R>::adj_fkpp_adaptive(const GenericShape &g, const Tab &t, const Adj &p, const Adapt &ag, cudaStream_t st,
+cudaError_t RuntimeShape<R>::adj_fkpp_adaptive(const GenericShape &g, const Tab &t, const Adj &p, const Adapt &ag, int seg, cudaStream_t st,
                                                int *rows_out)
 {
     using U = ShapeUnit<R>;
@@ -171,7 +174,11 @@ cudaError_t RuntimeShape<R>::adj_fkpp_adaptive(const GenericShape &g, const Tab 
     fkpp_adapt::cta_geometry(g.D, &q.tpc, &th);
     q.ustep = p.ustep; q.dense = p.dense; q.tgrid = ag.tgrid; q.nacc = ag.nacc; q.cot = p.cot; q.grad_u0 = p.grad_u0; q.partial = p.partial;
     q.N = p.N; q.Nx = g.D; q.n_save = ag.n_save; q.t0 = ag.t0; q.save_dt = ag.save_dt;
-    return shape_launch::fkpp(fkpp_adapt::adjoint_kernel<typename U::Ops>, q, th, fkpp_adapt::adj_smem(g.D, g.P, sizeof(R)), st, rows_out);
+    // checkpointed: the handle's dense buffer is the adjoint's scratch area
+    q.hstep = ag.hstep; q.scratch = seg ? const_cast<R *>(p.dense) : nullptr; q.seg = seg;
+    const size_t smem = fkpp_adapt::adj_smem(g.D, g.P, sizeof(R));
+    if (seg) return shape_launch::fkpp(fkpp_adapt::adjoint_kernel<typename U::Ops, true>, q, th, smem, st, rows_out);
+    return shape_launch::fkpp(fkpp_adapt::adjoint_kernel<typename U::Ops, false>, q, th, smem, st, rows_out);
 }
 
 template <typename R>

@@ -381,7 +381,16 @@ class ZygoteVJP:
 
 @dataclass
 class InterpolatingAdjoint:
+    """InterpolatingAdjoint(autojacvec = ReverseDiffVJP()) of seir_exposure.jl:71,140 and Fisher-KPP-CNN.jl:136.
+
+    checkpointing=True (SciMLSensitivity's keyword; adaptive Tsit5 on the Fisher-KPP UPDE only, float32 and float64,
+    B200UDE_FLAG_CHECKPOINT): the forward keeps the state every K accepted steps and the size of every step instead of the whole
+    step record, K = max(1, round(sqrt(max_steps / 7))), and the adjoint recomputes each segment of K steps before it replays it.
+    The record shrinks by about sqrt(max_steps / 7) / 2 times (55x at max_steps = 2048), for one more evaluation of the accepted
+    steps' right-hand sides per adjoint.  Unlike SciMLSensitivity, which re-solves each interval with error control, the
+    forward's own steps are replayed with their recorded sizes, so the gradient is bitwise that of checkpointing=False."""
     autojacvec: object = field(default_factory=ReverseDiffVJP)
+    checkpointing: bool = False
     code = _lib.INTERPOLATING_ADJOINT
 
 
@@ -473,6 +482,8 @@ class UDESolver:
                 d.flags |= _lib.FLAG_DISCRETE_DENSE if adaptive else 0
             else:
                 d.flags |= _lib.FLAG_VERN7_DENSE
+        if isinstance(sensealg, InterpolatingAdjoint) and sensealg.checkpointing:
+            d.flags |= _lib.FLAG_CHECKPOINT
         # adaptive = true: OrdinaryDiffEq's defaults abstol = 1e-6, reltol = 1e-3 when the kwargs are omitted (Fisher-KPP-CNN.jl:136)
         d.adaptive = 1 if adaptive else 0
         d.abstol, d.reltol, d.max_steps = float(abstol), float(reltol), int(max_steps)
@@ -762,7 +773,8 @@ def concrete_solve(prob, alg, u0=None, p=None, *, saveat=None, dt=None, adaptive
     abstol = 1e-6 if abstol is None else abstol
     reltol = 1e-3 if reltol is None else reltol
     key = (id(base.f), t0, dtv, n_steps, save_every, type(alg).__name__, getattr(alg, "stages", None), getattr(alg, "eigen_est", None),
-           getattr(alg, "dense", None), type(sensealg).__name__ if sensealg is not None else None, dev.index, tuple(loss_weights) if loss_weights else None,
+           getattr(alg, "dense", None), type(sensealg).__name__ if sensealg is not None else None,
+           bool(getattr(sensealg, "checkpointing", False)), dev.index, tuple(loss_weights) if loss_weights else None,
            bool(adaptive), abstol, reltol, max_steps, str(dtype))
     solver = _SOLVERS.get(key)
     if solver is None or solver.capacity < N:
