@@ -1,6 +1,6 @@
 """The chain shapes at the edges of the runtime-shape kernels' envelope (1 to 5 dense layers, widths 1 to 64, identity / tanh /
 RBF in any layer, NODE state dimension 1 to 8, fp32 theta up to the 12 288-float constant bank), none of them one that
-pick_kernel() sends to a tuned kernel, with their inputs.
+resolve() routes to a tuned kernel, with their inputs.
 
     id          form          widths                 acts                          P
     node1_lin   NODE d = 1    1-1                    id                            2      one layer, d = 1, closed form

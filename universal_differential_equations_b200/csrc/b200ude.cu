@@ -28,37 +28,55 @@ namespace {
 
 thread_local std::string g_create_error;
 
-// kernel families compiled into this build (one translation unit each, see k_*.cu); a handle's dtype picks the precision
-//   K_LV32   LV 2 -> 32 -> 32 -> 2 tanh                      BASELINE config 2
-//   K_LV5Px  LV 2 -> 5 -> 5 -> 5 -> 2, per-layer activations, x trainable linear rates
-//            scenario_1.jl:62-73 (x=0), scenario_2.jl:79-98 (x=1), hudson_bay.jl:77-91 (x=2)
-//   K_GENERIC  any LV / SEIR / SEIR_NODE / NODE form with chain widths <= 64 and <= 5 layers (k_generic.cu fp32, k_f64.cu fp64):
-//            functional coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned; also Vern7, the adaptive path of untuned chains
-//            and the discrete adjoint of every form but the tuned LV chains (discrete_adjoint.cuh; through Vern7's interpolated
-//            saves: vern7_dense_discrete.cuh)
-//   K_FKPP     Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126); fixed step
-//            (fp32), adaptive Tsit5 (fkpp_adaptive.cuh) and adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
-//   K_SEIR64   SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu)      BASELINE config 3
-//   K_FKPP16   Fisher-KPP UPDE with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu)                BASELINE config 4
-//   K_FORCED   forced neural ODE with a readout network (FENEP.jl:41-62) (k_forced.cu)
-//   K_OPERATOR wide-state operator UDE du = D1 NN(u) + D2 u (npde.jl:75-78), warp per trajectory (k_operator.cu)
-// The fp64 handles are K_GENERIC, K_FKPP, K_FORCED and K_OPERATOR; the others are fp32 only.
-enum KernelId { K_NONE = 0, K_LV32, K_LV5P0, K_LV5P1, K_LV5P2, K_GENERIC, K_FKPP, K_SEIR64, K_FKPP16, K_FORCED, K_OPERATOR };
+// The route of a handle: the forward / adjoint kernel pair it runs, chosen once by resolve() at create.  The forward, the adjoint,
+// the Tsit5 re-solve, num_params, partial_rows and the buffers of create read the route, not the descriptor's model, solver or
+// flag bits; within a route the dtype, fixed or adaptive stepping and the ensemble size are data the launchers take.  Routes
+// marked fp32 are fp32 only; the others take both dtypes.
+//   R_LV32            LV 2 -> 32 -> 32 -> 2 tanh, fixed-step Tsit5, interpolating adjoint (fp32)             BASELINE config 2
+//                     (k_lv32_*.cu): warp-collective or one trajectory per thread, chosen per call from the ensemble size
+//   R_LV32_DISCRETE   the same forward, the discrete adjoint on one trajectory per thread (fp32)
+//   R_LV32_ADAPTIVE   adaptive Tsit5: tensor-core kernels with CTA-uniform attempt loops (fp32)
+//   R_LV5             LV 2 -> 5 -> 5 -> 5 -> 2, per-layer activations, n_prefix = 0, 1, 2 trainable linear rates (k_lv5.cu):
+//                     scenario_1.jl:62-73, scenario_2.jl:79-98, hudson_bay.jl:77-91; fixed-step Tsit5, either adjoint (fp32)
+//   R_SEIR64          SEIR exposure UDE 3 -> 64 -> 64 -> 1 tanh, tensor-core kernels (k_seir.cu), fixed-step Tsit5 (fp32)   BASELINE config 3
+//   R_SEIR64_VERN7    its fixed-step Vern7; the interpolating adjoint runs over a Tsit5 re-solve, launched by the first adjoint (fp32)
+//   R_SEIR64_ADAPTIVE its adaptive Tsit5, CTA-uniform attempt loops (fp32)
+//   R_FKPP_FIXED      Fisher-KPP UPDE: pointwise chain 1 -> ... -> 1 + 3-tap periodic stencil (Fisher-KPP-CNN.jl:111-126), fixed-step
+//                     Tsit5 (fp32)
+//   R_FKPP16          Fisher-KPP with the 1 -> 16 -> 16 -> 1 tanh reaction chain (k_fkpp.cu), fixed-step Tsit5 (fp32)   BASELINE config 4
+//   R_FKPP16_RKC2     the same chain on even grids, fixed-step RKC2 (fp32)
+//   R_FKPP_ADAPTIVE   Fisher-KPP adaptive Tsit5, grid per CTA, any chain (fkpp_adaptive.cuh), full step record
+//   R_FKPP_CHECKPOINT the same with B200UDE_FLAG_CHECKPOINT: u_n every `seg` accepted steps and the step sizes
+//   R_FKPP_VERN7_DISCRETE  Fisher-KPP adaptive Vern7 with the discrete adjoint (fkpp_vern7_discrete.cuh)
+//   runtime-shape kernels (RuntimeShape<R>: k_generic.cu fp32, k_f64.cu fp64): any LV / SEIR / SEIR_NODE / NODE form with chain
+//   widths <= 64 and <= 5 layers, fixed step or adaptive -- functional coverage (seir_exposure.jl:52-64,114-130 shapes), not tuned
+//   R_TSIT5           Tsit5, interpolating adjoint
+//   R_VERN7           Vern7; the interpolating adjoint runs over a Tsit5 re-solve from the same u0, launched by the first adjoint
+//   R_DISCRETE_TSIT5  fixed-step Tsit5, discrete adjoint (discrete_adjoint.cuh)
+//   R_DISCRETE_VERN7  Vern7, discrete adjoint; saves at step ends (B200UDE_FLAG_DISCRETE_DENSE on a fixed grid lands here too)
+//   R_VERN7_DENSE     Vern7 with its lazy dense output, interpolating adjoint over it (vern7_dense.cuh; B200UDE_FLAG_VERN7_DENSE)
+//   R_VERN7_DENSE_DISCRETE  adaptive Vern7 saving through its interpolant, discrete adjoint through it (vern7_dense_discrete.cuh;
+//                     B200UDE_FLAG_DISCRETE_DENSE)
+//   R_FORCED          forced neural ODE with a readout network (FENEP.jl:41-62) (k_forced.cu), Tsit5
+//   R_OPERATOR        wide-state operator UDE du = D1 NN(u) + D2 u (npde.jl:75-78), warp per trajectory (k_operator.cu), Tsit5 or RKC2
+enum Route {
+    R_LV32, R_LV32_DISCRETE, R_LV32_ADAPTIVE, R_LV5, R_SEIR64, R_SEIR64_VERN7, R_SEIR64_ADAPTIVE, R_FKPP_FIXED, R_FKPP16, R_FKPP16_RKC2,
+    R_FKPP_ADAPTIVE, R_FKPP_CHECKPOINT, R_FKPP_VERN7_DISCRETE, R_TSIT5, R_VERN7, R_DISCRETE_TSIT5, R_DISCRETE_VERN7, R_VERN7_DENSE,
+    R_VERN7_DENSE_DISCRETE, R_FORCED, R_OPERATOR
+};
 
 // parameters of a handle: the tuned chains' fixed counts, else n_prefix + the dense layers + n_suffix.  The forced model's f0 and f1
 // lie back to back in `widths`: its layers l >= L0 read one entry further on
-int num_params(const b200ude_desc *d, KernelId k)
+int num_params(const b200ude_desc *d, Route r)
 {
-    switch (k) {
-    case K_LV32: return 2 * 32 + 32 + 32 * 32 + 32 + 32 * 2 + 2;
-    case K_SEIR64: return 3 * 64 + 64 + 64 * 64 + 64 + 64 + 1;
-    case K_FKPP16: return 16 + 16 + 256 + 16 + 16 + 1 + 5;
-    case K_LV5P0: return 87;
-    case K_LV5P1: return 88;
-    case K_LV5P2: return 89;
+    switch (r) {
+    case R_LV32: case R_LV32_DISCRETE: case R_LV32_ADAPTIVE: return 2 * 32 + 32 + 32 * 32 + 32 + 32 * 2 + 2;
+    case R_SEIR64: case R_SEIR64_VERN7: case R_SEIR64_ADAPTIVE: return 3 * 64 + 64 + 64 * 64 + 64 + 64 + 1;
+    case R_FKPP16: case R_FKPP16_RKC2: return 16 + 16 + 256 + 16 + 16 + 1 + 5;
+    case R_LV5: return 87 + d->n_prefix;
     default: break;
     }
-    const int L0 = k == K_FORCED ? (int)d->consts[0] : d->n_layers;
+    const int L0 = r == R_FORCED ? (int)d->consts[0] : d->n_layers;
     int P = d->n_prefix + d->n_suffix;
     for (int l = 0; l < d->n_layers; ++l) {
         const int a = l < L0 ? l : l + 1;
@@ -73,7 +91,7 @@ std::atomic<uint64_t> g_serial{0};   // handles may be created from several host
 
 struct b200ude_handle {
     b200ude_desc desc;
-    KernelId kid = K_NONE;
+    Route route = R_TSIT5;
     bool f64 = false;   // dtype = B200UDE_F64: every real-valued device array of the handle and of the callers is double
     Variant var;
     ConstTables tab;    // fp32 runtime-shape and tuned kernels
@@ -97,7 +115,7 @@ struct b200ude_handle {
     bool adaptive = false;
     void *d_tgrid = nullptr, *d_cot = nullptr;
     void *d_hstep = nullptr;   // discrete-adjoint Vern7, checkpointed Fisher-KPP: step sizes of the accepted steps
-    int seg = 0;               // B200UDE_FLAG_CHECKPOINT: accepted steps per checkpoint (d_ustep: checkpoints, d_dense: scratch), else 0
+    int seg = 0;               // R_FKPP_CHECKPOINT: accepted steps per checkpoint (d_ustep: checkpoints, d_dense: scratch), else 0
     float *d_block_loss = nullptr;
     int *d_nacc = nullptr;
     const void *last_out = nullptr;
@@ -108,25 +126,23 @@ struct b200ude_handle {
     cudaStream_t own_stream = nullptr;
     cudaStream_t copy_stream = nullptr;   // host-buffer path: the data upload overlaps the forward kernel
     cudaEvent_t data_ready = nullptr, data_ready2 = nullptr;
-    RkcHost rkc;                    // solver = B200UDE_RKC2: recurrence tables for desc.n_stages
+    RkcHost rkc;                    // R_FKPP16_RKC2: recurrence tables for desc.n_stages
     // fused reduce + all-reduce over NVLink peer memory (b200ude_peer_*)
     void *d_peer_buf = nullptr;     // this rank's exchange buffer (cudaMalloc, exported with CUDA IPC)
     PeerLinks peer;                 // every rank's buffer as mapped here
     bool peer_attached = false;
     // on-device optimiser (b200ude_adam_*, b200ude_train_adam)
     void *d_u0_keep = nullptr, *d_aux_out = nullptr;   // Vern7: u0 of the last forward, saved states of the Tsit5 re-solve
-    bool vern7_pending = false;
-    bool vern7_dense = false;   // B200UDE_FLAG_VERN7_DENSE: saveat and the interpolating adjoint through Vern7's own dense output
-    bool discrete_dense = false;   // B200UDE_FLAG_DISCRETE_DENSE on an adaptive grid: saveat through the interpolant, discrete adjoint through it
+    bool vern7_pending = false;   // R_VERN7, R_SEIR64_VERN7: the Tsit5 re-solve the adjoint runs over is still to be launched
     float *d_adam_m = nullptr, *d_adam_v = nullptr, *d_train_out = nullptr;
     int *d_adam_t = nullptr;
     int adam_t = 0;   // host mirror of the step counter
-    // forced neural ODE (K_FORCED): shape, the forcing coefficients [3J][cap], the last forward's out
+    // forced neural ODE (R_FORCED): shape, the forcing coefficients [3J][cap], the last forward's out
     ForcedHost fh{};
     void *d_forcing = nullptr;
     size_t forcing_n = 0;   // trajectories of the last b200ude_set_forcing
     void *d_usave = nullptr;   // adaptive: the saved states of the last forward [n_save][D][cap], read by the replay adjoint
-    // operator UDE (K_OPERATOR): shape, the padded operator block, the RKC2 tables (handle dtype); it shares d_usave (as
+    // operator UDE (R_OPERATOR): shape, the padded operator block, the RKC2 tables (handle dtype); it shares d_usave (as
     // [n_save][cap][D]) and the record buffers with the forced model
     bool ops_set = false;
     OperatorHost oh{};
@@ -278,29 +294,6 @@ bool generic_ok(const b200ude_desc &d)
 // kernel family of the LV 2-32-32-2 chain for an ensemble of N: mode 1 = always warp-collective, 0 = never, -1 = by size
 bool use_wm(int mode, size_t N, size_t n_max) { return mode > 0 || (mode < 0 && N <= n_max); }
 
-KernelId pick_kernel(const b200ude_desc &d)
-{
-    if (d.model == B200UDE_MODEL_LV && d.state_dim == 2 && d.acts[d.n_layers - 1] == B200UDE_ACT_IDENTITY) {
-        if (d.n_layers == 3 && d.widths[0] == 2 && d.widths[1] == 32 && d.widths[2] == 32 && d.widths[3] == 2 &&
-            d.acts[0] == B200UDE_ACT_TANH && d.acts[1] == B200UDE_ACT_TANH && d.n_prefix == 0)
-            return K_LV32;
-        if (d.n_layers == 4 && d.widths[0] == 2 && d.widths[1] == 5 && d.widths[2] == 5 && d.widths[3] == 5 && d.widths[4] == 2) {
-            if (d.n_prefix == 0) return K_LV5P0;
-            if (d.n_prefix == 1) return K_LV5P1;
-            if (d.n_prefix == 2) return K_LV5P2;
-        }
-    }
-    if (!generic_ok(d)) return K_NONE;
-    if (d.model == B200UDE_MODEL_SEIR && d.n_layers == 3 && d.widths[1] == 64 && d.widths[2] == 64 && d.acts[0] == B200UDE_ACT_TANH &&
-        d.acts[1] == B200UDE_ACT_TANH && d.acts[2] == B200UDE_ACT_IDENTITY && d.n_suffix == 0 && env_int("B200UDE_SEIR_TC", 1))
-        return K_SEIR64;
-    if (d.model == B200UDE_MODEL_FKPP && d.n_layers == 3 && d.widths[1] == 16 && d.widths[2] == 16 && d.acts[0] == B200UDE_ACT_TANH &&
-        d.acts[1] == B200UDE_ACT_TANH && d.acts[2] == B200UDE_ACT_IDENTITY && env_int("B200UDE_FKPP_TUNED", 1))
-        return K_FKPP16;
-    return d.model == B200UDE_MODEL_FKPP ? K_FKPP : K_GENERIC;
-}
-
-
 template <typename R>
 constexpr bool is_f32 = std::is_same<R, float>::value;
 
@@ -309,15 +302,6 @@ int32_t do_forward_forced(b200ude_handle *h, const void *u0, size_t N, void *out
 int32_t do_adjoint_forced(b200ude_handle *h, bool l2, const void *cot, void *grad_u0, cudaStream_t st, int *rows);
 int32_t do_forward_operator(b200ude_handle *h, const void *u0, size_t N, void *out, int32_t *status, cudaStream_t st);
 int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *grad_u0, cudaStream_t st, int *rows);
-
-// the fp32-only kernels: the tuned families (LV 2-32-32-2, LV 2-5-5-5-2, SEIR 3-64-64-1 -- its fixed-step Vern7 included --,
-// Fisher-KPP 1-16-16-1, the only one with RKC2) and fixed-step Fisher-KPP.  Every other handle, fp32 or fp64, runs on the
-// runtime-shape kernels (RuntimeShape<R>).
-bool fp32_only(const b200ude_handle *h)
-{
-    return h->kid == K_LV32 || h->kid == K_LV5P0 || h->kid == K_LV5P1 || h->kid == K_LV5P2 || h->kid == K_SEIR64 || h->kid == K_FKPP16 ||
-           (h->kid == K_FKPP && !h->adaptive);
-}
 
 // the kernels' parameter structs of each precision
 FwdParams fwd_params(const b200ude_handle *h, const float *u0, float *out, void *ustep, void *dense, int32_t *status, size_t N)
@@ -361,92 +345,46 @@ const typename RealParams<R>::Tab &tables(const b200ude_handle *h)
     else return h->tab64;
 }
 
-// forward of the fp32-only kernels; solver 1: the SEIR chain's fixed-step Vern7
-cudaError_t forward32(b200ude_handle *h, const FwdParams &p, size_t N, int solver, cudaStream_t st)
+// the forward kernel of the handle's route.  tsit5: the Tsit5 re-solve of a Vern7 route (R_VERN7, R_SEIR64_VERN7) that its
+// interpolating adjoint runs over.  The fp32-only routes exist in the fp32 instantiation only.
+template <typename R>
+cudaError_t launch_forward(b200ude_handle *h, const typename RealParams<R>::Fwd &p, size_t N, bool tsit5, cudaStream_t st)
 {
-    if (solver == 1) return launch_fwd_seir_vern7(h->var, h->tab, p, st);   // tensor-core kernels (seir_tc.cuh)
-    if (h->adaptive)   // the headline chains: tensor-core kernels with CTA-uniform attempt loops
-        return h->kid == K_LV32 ? launch_fwd_lv32_adaptive(h->var, h->tab, p, adapt<float>(h), st)
-                                : launch_fwd_seir_adaptive(h->var, h->tab, p, adapt<float>(h), st);
-    if (h->desc.solver == B200UDE_RKC2) return launch_fwd_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st);
-    switch (h->kid) {
-    case K_LV32:
+    using RS = RuntimeShape<R>;
+    const auto &t = tables<R>(h);
+    const auto ag = adapt<R>(h);
+    const auto *agp = h->adaptive ? &ag : nullptr;
+    switch (h->route) {
+    case R_LV32:
+    case R_LV32_DISCRETE:
         // small / medium ensembles: the warp-collective family (latency per stage ~4x lower); large ones: one trajectory per thread
-        return use_wm(h->var.fwd_wm, N, h->wm_fwd_max) ? launch_fwd_lv32_wm(h->var, h->tab, p, st) : launch_fwd_lv32(h->var, h->tab, p, st);
-    case K_LV5P0: return launch_fwd_lv5(0, h->var, h->tab, p, st);
-    case K_LV5P1: return launch_fwd_lv5(1, h->var, h->tab, p, st);
-    case K_LV5P2: return launch_fwd_lv5(2, h->var, h->tab, p, st);
-    case K_FKPP: return launch_fwd_fkpp(h->gen, h->tab, p, st);
-    case K_SEIR64: return launch_fwd_seir(h->var, h->tab, p, st);
-    default: return launch_fwd_fkpp16(h->var, h->tab, p, h->D, st);   // K_FKPP16
+        if constexpr (is_f32<R>)
+            return use_wm(h->var.fwd_wm, N, h->wm_fwd_max) ? launch_fwd_lv32_wm(h->var, h->tab, p, st) : launch_fwd_lv32(h->var, h->tab, p, st);
+        break;
+    case R_LV32_ADAPTIVE: if constexpr (is_f32<R>) return launch_fwd_lv32_adaptive(h->var, h->tab, p, ag, st); break;
+    case R_LV5: if constexpr (is_f32<R>) return launch_fwd_lv5(h->desc.n_prefix, h->var, h->tab, p, st); break;
+    case R_SEIR64: if constexpr (is_f32<R>) return launch_fwd_seir(h->var, h->tab, p, st); break;
+    case R_SEIR64_VERN7:
+        if constexpr (is_f32<R>) return tsit5 ? launch_fwd_seir(h->var, h->tab, p, st) : launch_fwd_seir_vern7(h->var, h->tab, p, st);
+        break;
+    case R_SEIR64_ADAPTIVE: if constexpr (is_f32<R>) return launch_fwd_seir_adaptive(h->var, h->tab, p, ag, st); break;
+    case R_FKPP_FIXED: if constexpr (is_f32<R>) return launch_fwd_fkpp(h->gen, h->tab, p, st); break;
+    case R_FKPP16: if constexpr (is_f32<R>) return launch_fwd_fkpp16(h->var, h->tab, p, h->D, st); break;
+    case R_FKPP16_RKC2: if constexpr (is_f32<R>) return launch_fwd_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st); break;
+    case R_FKPP_ADAPTIVE:
+    case R_FKPP_CHECKPOINT: return RS::fwd_fkpp_adaptive(h->gen, t, p, ag, h->seg, st);
+    case R_FKPP_VERN7_DISCRETE: return RS::fwd_fkpp_vern7(h->gen, t, p, ag, st);
+    case R_TSIT5:
+    case R_DISCRETE_TSIT5: return RS::fwd(h->gen, t, p, 0, agp, st);
+    case R_VERN7: return RS::fwd(h->gen, t, p, tsit5 ? 0 : 1, agp, st);
+    case R_DISCRETE_VERN7: return RS::fwd(h->gen, t, p, 1, agp, st);
+    // an adaptive solve saves through the interpolant; a fixed grid saves at step ends, as without the flag
+    case R_VERN7_DENSE: return h->adaptive ? RS::fwd_vern7_dense(h->gen, t, p, ag, st) : RS::fwd(h->gen, t, p, 1, nullptr, st);
+    case R_VERN7_DENSE_DISCRETE: return RS::fwd_vern7_dense(h->gen, t, p, ag, st);
+    case R_FORCED:
+    case R_OPERATOR: break;   // do_forward_forced, do_forward_operator
     }
-}
-
-// adjoint of the fp32-only kernels.  split: the two data-ready events of the host-buffer path, under which the warp-collective LV
-// adjoint runs as two sub-range launches (the first one under the second half's upload), or nullptr
-cudaError_t adjoint32(b200ude_handle *h, const AdjParams &p, const cudaEvent_t *split, size_t split_at, cudaStream_t st, int *rows)
-{
-    if (h->adaptive)
-        return h->kid == K_LV32 ? launch_adj_lv32_adaptive(h->var, h->tab, p, adapt<float>(h), st, rows)
-                                : launch_adj_seir_adaptive(h->var, h->tab, p, adapt<float>(h), st, rows);
-    if (h->desc.solver == B200UDE_RKC2) return launch_adj_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st, rows);
-    switch (h->kid) {
-    case K_LV32:
-        if (split) {
-            int g0 = 0, g1 = 0;
-            AdjParams q = p;
-            q.n0 = 0; q.n_cnt = (int)split_at; q.row0 = 0;
-            cudaError_t e = cudaStreamWaitEvent(st, split[0], 0);
-            if (e == cudaSuccess) e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g0);
-            if (e == cudaSuccess) {
-                q.n0 = (int)split_at; q.n_cnt = (int)(h->N - split_at); q.row0 = g0;
-                e = cudaStreamWaitEvent(st, split[1], 0);
-                if (e == cudaSuccess) e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g1);
-            }
-            *rows = g0 + g1;
-            return e;
-        }
-        return (!h->var.discrete && use_wm(h->var.adj_wm, h->N, h->wm_adj_max)) ? launch_adj_lv32_wm(h->var, h->tab, p, st, rows)
-                                                                                : launch_adj_lv32(h->var, h->tab, p, st, rows);
-    case K_LV5P0: return launch_adj_lv5(0, h->var, h->tab, p, st, rows);
-    case K_LV5P1: return launch_adj_lv5(1, h->var, h->tab, p, st, rows);
-    case K_LV5P2: return launch_adj_lv5(2, h->var, h->tab, p, st, rows);
-    case K_FKPP: return launch_adj_fkpp(h->gen, h->tab, p, st, rows);
-    case K_SEIR64: return launch_adj_seir(h->var, h->tab, p, st, rows);
-    default: return launch_adj_fkpp16(h->var, h->tab, p, h->D, st, rows);   // K_FKPP16
-    }
-}
-
-// Tsit5 (solver 0) or Vern7 (solver 1) forward of a runtime-shape or fp32-only handle; the Tsit5 solve writes the dense record
-// (stage derivatives) the interpolating adjoint reads
-template <typename R>
-cudaError_t launch_forward(b200ude_handle *h, const typename RealParams<R>::Fwd &p, size_t N, int solver, cudaStream_t st)
-{
-    if constexpr (is_f32<R>)
-        if (fp32_only(h)) return forward32(h, p, N, solver, st);
-    const auto ag = adapt<R>(h);
-    if (h->kid == K_FKPP) return RuntimeShape<R>::fwd_fkpp_adaptive(h->gen, tables<R>(h), p, ag, h->seg, st);   // adaptive Tsit5 (b200ude_create)
-    return RuntimeShape<R>::fwd(h->gen, tables<R>(h), p, solver, h->adaptive ? &ag : nullptr, st);
-}
-
-// the interpolating adjoint of that Tsit5 solve (the replay of an adaptive one)
-template <typename R>
-cudaError_t launch_adjoint(b200ude_handle *h, const typename RealParams<R>::Adj &p, const cudaEvent_t *split, size_t split_at, cudaStream_t st,
-                           int *rows)
-{
-    if constexpr (is_f32<R>)
-        if (fp32_only(h)) return adjoint32(h, p, split, split_at, st, rows);
-    const auto ag = adapt<R>(h);
-    if (h->kid == K_FKPP) return RuntimeShape<R>::adj_fkpp_adaptive(h->gen, tables<R>(h), p, ag, h->seg, st, rows);
-    return RuntimeShape<R>::adj(h->gen, tables<R>(h), p, h->adaptive ? &ag : nullptr, st, rows);
-}
-
-template <typename R>
-int32_t tsit5_forward(b200ude_handle *h, const R *u0, size_t N, R *out, int32_t *status, cudaStream_t st)
-{
-    CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, u0, out, h->d_ustep, h->d_dense, status, N), N, 0, st));
-    h->last_out = out;
-    return B200UDE_OK;
+    return cudaErrorNotSupported;
 }
 
 template <typename R>
@@ -456,28 +394,15 @@ int32_t do_forward(b200ude_handle *h, const R *u0, size_t N, R *out, int32_t *st
     if (!h->have_theta) return fail(h, B200UDE_ESTATE, "forward: set_params has not been called");
     if (N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "forward: N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     if (!u0 || !out) return fail(h, B200UDE_EINVAL, "forward: null pointer");
-    if (h->kid == K_FORCED) return do_forward_forced(h, u0, N, out, status, st);
-    if (h->kid == K_OPERATOR) return do_forward_operator(h, u0, N, out, status, st);
-    if (h->desc.solver == B200UDE_VERN7 && (h->var.discrete || h->vern7_dense)) {
-        // discrete adjoint, or the interpolating adjoint over Vern7's dense output: the forward records u_n of every (accepted)
-        // step, which the adjoint recomputes the stages from.  With either dense flag an adaptive solve saves through the
-        // interpolant; a fixed grid saves at step ends either way
-        using RS = RuntimeShape<R>;
-        const auto p = fwd_params(h, u0, out, h->d_ustep, nullptr, status, N);
-        const auto ag = adapt<R>(h);
-        if (h->kid == K_FKPP) CUDA_TRY(h, RS::fwd_fkpp_vern7(h->gen, tables<R>(h), p, ag, st));   // adaptive only (b200ude_create)
-        else if (h->adaptive && (h->vern7_dense || h->discrete_dense)) CUDA_TRY(h, RS::fwd_vern7_dense(h->gen, tables<R>(h), p, ag, st));
-        else CUDA_TRY(h, RS::fwd(h->gen, tables<R>(h), p, 1, h->adaptive ? &ag : nullptr, st));
-        h->last_out = out;
-        h->N = N;
-        h->have_forward = true;
-        return B200UDE_OK;
-    }
-    if (h->desc.solver == B200UDE_VERN7) {
-        // Vern7 writes the saved states only.  Its lazy dense output is not available (SURVEY.md App. A.3), so the
-        // interpolating adjoint of a Vern7 solve runs over a Tsit5 re-solve from the same u0 with the same step /
-        // tolerances, launched by the first adjoint call (do_adjoint); u0 is kept for that.
-        CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, u0, out, nullptr, nullptr, status, N), N, 1, st));
+    switch (h->route) {
+    case R_FORCED: return do_forward_forced(h, u0, N, out, status, st);
+    case R_OPERATOR: return do_forward_operator(h, u0, N, out, status, st);
+    case R_VERN7:
+    case R_SEIR64_VERN7:
+        // Vern7 writes the saved states only.  Its lazy dense output is not used here (R_VERN7_DENSE uses it), so the interpolating
+        // adjoint runs over a Tsit5 re-solve from the same u0 with the same step / tolerances, launched by the first adjoint call
+        // (do_adjoint); u0 is kept for that.
+        CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, u0, out, nullptr, nullptr, status, N), N, false, st));
         if (!h->d_u0_keep && dalloc_real(h, &h->d_u0_keep, (size_t)h->D * h->cap) != cudaSuccess)
             return fail(h, B200UDE_ENOMEM, "forward: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
         CUDA_TRY(h, cudaMemcpyAsync(h->d_u0_keep, u0, sizeof(R) * (size_t)h->D * N, cudaMemcpyDeviceToDevice, st));
@@ -485,12 +410,15 @@ int32_t do_forward(b200ude_handle *h, const R *u0, size_t N, R *out, int32_t *st
         h->have_forward = false;
         h->vern7_pending = true;
         return B200UDE_OK;
+    default:
+        // the Tsit5 and RKC2 solves write the dense record (stage derivatives) the interpolating adjoint reads; the routes that
+        // recompute the stages from u_n (discrete adjoint of Vern7, Vern7's dense output) have none (d_dense = nullptr)
+        CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, u0, out, h->d_ustep, h->d_dense, status, N), N, false, st));
+        h->last_out = out;
+        h->N = N;
+        h->have_forward = true;
+        return B200UDE_OK;
     }
-    int32_t rc = tsit5_forward(h, u0, N, out, status, st);
-    if (rc) return rc;
-    h->N = N;
-    h->have_forward = true;
-    return B200UDE_OK;
 }
 
 // partial rows -> grad_theta and the loss (nullptr: not written): fp64 reduce, fp32 reduce fused with the all-reduce over the
@@ -513,65 +441,100 @@ int32_t do_adjoint(b200ude_handle *h, bool l2, const R *cot, R *loss, R *grad_th
     if (peer && !h->peer_attached) return fail(h, B200UDE_ESTATE, "adjoint_l2_allreduce: b200ude_peer_attach has not been called");
     if (peer && h->adaptive) return fail(h, B200UDE_EUNSUPPORTED, "adjoint_l2_allreduce: not available with adaptive stepping (all-reduce the result of b200ude_adjoint_l2 instead)");
     // an fp64 operator handle names its missing operators before the missing forward solution
-    if (h->f64 && h->kid == K_OPERATOR && !h->ops_set)
+    if (h->f64 && h->route == R_OPERATOR && !h->ops_set)
         return fail(h, B200UDE_ESTATE, "adjoint: B200UDE_MODEL_OPERATOR needs its operators (call b200ude_set_operators first)");
-    if (h->desc.solver == B200UDE_VERN7 && h->vern7_pending) {
+    if (h->vern7_pending) {
         if (!h->d_aux_out && dalloc_real(h, &h->d_aux_out, (size_t)h->n_save * (size_t)h->D * h->cap) != cudaSuccess)
             return fail(h, B200UDE_ENOMEM, "adjoint: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-        int32_t rc = tsit5_forward(h, (const R *)h->d_u0_keep, h->N, (R *)h->d_aux_out, nullptr, st);
-        if (rc) return rc;
+        CUDA_TRY(h, launch_forward<R>(h, fwd_params(h, (const R *)h->d_u0_keep, (R *)h->d_aux_out, h->d_ustep, h->d_dense, nullptr, h->N),
+                                      h->N, true, st));
+        h->last_out = h->d_aux_out;
         h->vern7_pending = false;
         h->have_forward = true;
     }
     if (!h->have_forward) return fail(h, B200UDE_ESTATE, "adjoint: no stored forward solution (call b200ude_forward first)");
     if (!cot || !grad_theta) return fail(h, B200UDE_EINVAL, "adjoint: null pointer");
-    const bool split_ok = split && h->kid == K_LV32 && !h->adaptive && h->desc.solver != B200UDE_RKC2 && !h->var.discrete &&
-                          use_wm(h->var.adj_wm, h->N, h->wm_adj_max) && split_at > 0 && split_at < h->N;
+    const bool split_ok = split && h->route == R_LV32 && use_wm(h->var.adj_wm, h->N, h->wm_adj_max) && split_at > 0 && split_at < h->N;
     if (split && !split_ok) {   // every other kernel family reads the whole data array
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[0], 0));
         CUDA_TRY(h, cudaStreamWaitEvent(st, split[1], 0));
     }
-    int rows = 0;
-    if (h->kid == K_FORCED || h->kid == K_OPERATOR) {
-        const int32_t rc = h->kid == K_FORCED ? do_adjoint_forced(h, l2, cot, grad_u0, st, &rows) : do_adjoint_operator(h, l2, cot, grad_u0, st, &rows);
-        return rc ? rc : reduce_partials(h, rows, grad_theta, loss, peer, st);
-    }
     using RS = RuntimeShape<R>;
     const auto &t = tables<R>(h);
     const auto ag = adapt<R>(h);
+    const auto *agp = h->adaptive ? &ag : nullptr;
     auto p = adj_params(h, cot, grad_u0, l2);
-    const R *saved = (const R *)h->last_out;
+    const R *saved = (const R *)h->last_out;   // the states the forward returned (after a Vern7 forward: the Tsit5 re-solve's)
     R *reduce_loss = loss;
     bool finish_l2 = false;   // fp32 two-stage L2 cotangent: its loss follows the reduce
-    if (h->vern7_dense) {
-        // interpolating adjoint over the Vern7 solve's own dense output; the fused L2 reads the states the forward returned
-        CUDA_TRY(h, RS::adj_vern7_dense(h->gen, t, p, h->adaptive ? &ag : nullptr, saved, st, &rows));
-    } else if (h->discrete_dense) {
-        // discrete adjoint of the free-stepping Vern7 solve through its interpolated saves; the fused L2 reads the states the forward
-        // returned
-        CUDA_TRY(h, RS::adj_vern7_dense_discrete(h->gen, t, p, ag, saved, st, &rows));
-    } else if (h->var.discrete && h->kid == K_FKPP) {
-        // discrete adjoint of an adaptive Vern7 Fisher-KPP solve (grid-per-CTA kernels)
-        CUDA_TRY(h, RS::adj_fkpp_vern7(h->gen, t, p, ag, st, &rows));
-    } else if (h->var.discrete && h->kid == K_GENERIC) {
-        // discrete adjoint of a runtime-shape Tsit5 / Vern7 solve over its recorded steps; the fused L2 reads the recorded step-end states
-        CUDA_TRY(h, RS::adj_discrete(h->gen, t, p, h->desc.solver == B200UDE_VERN7 ? 1 : 0, h->adaptive ? &ag : nullptr, st, &rows));
-    } else {
-        if (h->adaptive && l2) {
-            // form the cotangent 2 w (out - data) from the interpolated saved states of the last forward: in fp32 in two stages (the
-            // loss follows the reduce), in fp64 in one CTA that writes the loss itself
-            if constexpr (is_f32<R>) {
-                CUDA_TRY(h, launch_l2_cot(h->tab, saved, cot, (float *)h->d_cot, h->d_block_loss, h->D, h->N, h->n_save, st));
-                finish_l2 = loss != nullptr;
-            } else {
-                CUDA_TRY(h, launch_l2_cot_f64(h->tab64, saved, cot, (double *)h->d_cot, loss, h->D, h->N, h->n_save, st));
-                reduce_loss = nullptr;
-            }
-            p.cot = (const R *)h->d_cot;
-            p.fused_l2 = 0;
+    const Route r = h->route;
+    if (h->adaptive && l2 && (r == R_LV32_ADAPTIVE || r == R_SEIR64_ADAPTIVE || r == R_FKPP_ADAPTIVE || r == R_FKPP_CHECKPOINT ||
+                              r == R_TSIT5 || r == R_VERN7)) {
+        // the replay of an adaptive Tsit5 solve: form the cotangent 2 w (out - data) from the interpolated saved states of the last
+        // forward, in fp32 in two stages (the loss follows the reduce), in fp64 in one CTA that writes the loss itself
+        if constexpr (is_f32<R>) {
+            CUDA_TRY(h, launch_l2_cot(h->tab, saved, cot, (float *)h->d_cot, h->d_block_loss, h->D, h->N, h->n_save, st));
+            finish_l2 = loss != nullptr;
+        } else {
+            CUDA_TRY(h, launch_l2_cot_f64(h->tab64, saved, cot, (double *)h->d_cot, loss, h->D, h->N, h->n_save, st));
+            reduce_loss = nullptr;
         }
-        CUDA_TRY(h, launch_adjoint<R>(h, p, split_ok ? split : nullptr, split_at, st, &rows));
+        p.cot = (const R *)h->d_cot;
+        p.fused_l2 = 0;
     }
+    int rows = 0;
+    cudaError_t e = cudaErrorNotSupported;
+    switch (r) {
+    case R_LV32:
+        if constexpr (is_f32<R>) {
+            if (!split_ok) {
+                e = use_wm(h->var.adj_wm, h->N, h->wm_adj_max) ? launch_adj_lv32_wm(h->var, h->tab, p, st, &rows)
+                                                              : launch_adj_lv32(h->var, h->tab, p, st, &rows);
+                break;
+            }
+            int g0 = 0, g1 = 0;
+            AdjParams q = p;
+            q.n0 = 0; q.n_cnt = (int)split_at; q.row0 = 0;
+            e = cudaStreamWaitEvent(st, split[0], 0);
+            if (e == cudaSuccess) e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g0);
+            if (e == cudaSuccess) {
+                q.n0 = (int)split_at; q.n_cnt = (int)(h->N - split_at); q.row0 = g0;
+                e = cudaStreamWaitEvent(st, split[1], 0);
+                if (e == cudaSuccess) e = launch_adj_lv32_wm(h->var, h->tab, q, st, &g1);
+            }
+            rows = g0 + g1;
+        }
+        break;
+    case R_LV32_DISCRETE: if constexpr (is_f32<R>) e = launch_adj_lv32(h->var, h->tab, p, st, &rows); break;
+    case R_LV32_ADAPTIVE: if constexpr (is_f32<R>) e = launch_adj_lv32_adaptive(h->var, h->tab, p, ag, st, &rows); break;
+    case R_LV5: if constexpr (is_f32<R>) e = launch_adj_lv5(h->desc.n_prefix, h->var, h->tab, p, st, &rows); break;
+    case R_SEIR64:
+    case R_SEIR64_VERN7: if constexpr (is_f32<R>) e = launch_adj_seir(h->var, h->tab, p, st, &rows); break;
+    case R_SEIR64_ADAPTIVE: if constexpr (is_f32<R>) e = launch_adj_seir_adaptive(h->var, h->tab, p, ag, st, &rows); break;
+    case R_FKPP_FIXED: if constexpr (is_f32<R>) e = launch_adj_fkpp(h->gen, h->tab, p, st, &rows); break;
+    case R_FKPP16: if constexpr (is_f32<R>) e = launch_adj_fkpp16(h->var, h->tab, p, h->D, st, &rows); break;
+    case R_FKPP16_RKC2: if constexpr (is_f32<R>) e = launch_adj_fkpp16_rkc(h->var, h->tab, h->rkc, p, h->D, st, &rows); break;
+    case R_FKPP_ADAPTIVE:
+    case R_FKPP_CHECKPOINT: e = RS::adj_fkpp_adaptive(h->gen, t, p, ag, h->seg, st, &rows); break;
+    // grid-per-CTA kernels
+    case R_FKPP_VERN7_DISCRETE: e = RS::adj_fkpp_vern7(h->gen, t, p, ag, st, &rows); break;
+    case R_TSIT5:
+    case R_VERN7: e = RS::adj(h->gen, t, p, agp, st, &rows); break;
+    // over the recorded steps; the fused L2 reads the recorded step-end states
+    case R_DISCRETE_TSIT5: e = RS::adj_discrete(h->gen, t, p, 0, agp, st, &rows); break;
+    case R_DISCRETE_VERN7: e = RS::adj_discrete(h->gen, t, p, 1, agp, st, &rows); break;
+    // over Vern7's own dense output / through its interpolated saves; the fused L2 reads the states the forward returned
+    case R_VERN7_DENSE: e = RS::adj_vern7_dense(h->gen, t, p, agp, saved, st, &rows); break;
+    case R_VERN7_DENSE_DISCRETE: e = RS::adj_vern7_dense_discrete(h->gen, t, p, ag, saved, st, &rows); break;
+    case R_FORCED:
+    case R_OPERATOR: {
+        const int32_t rc = r == R_FORCED ? do_adjoint_forced(h, l2, cot, grad_u0, st, &rows) : do_adjoint_operator(h, l2, cot, grad_u0, st, &rows);
+        if (rc) return rc;
+        e = cudaSuccess;
+        break;
+    }
+    }
+    CUDA_TRY(h, e);
     const int32_t rc = reduce_partials(h, rows, grad_theta, reduce_loss, peer, st);
     if (rc) return rc;
     if constexpr (is_f32<R>) {
@@ -803,98 +766,110 @@ int32_t do_adjoint_operator(b200ude_handle *h, bool l2, const void *cot, void *g
     return B200UDE_OK;
 }
 
-// the descriptor checks of every model but the operator UDE (operator_check), and the kernel family that runs the descriptor
-int32_t select_kernel(const b200ude_desc *d, KernelId *kid_out)
+// The descriptor checks and the route that runs the descriptor.  The refusals keep this order: the first check a descriptor fails
+// names it.  The kernel-selection knobs (B200UDE_SEIR_TC, _FKPP_TUNED, _SEIR_VERN7_TC, _ADAPTIVE_TC, _FKPP_PACKED; default 1) are
+// read here, so they take effect per handle at create.
+int32_t resolve(const b200ude_desc &d, Route *route)
 {
-    const bool forced = d->model == B200UDE_MODEL_FORCED;
-    if (forced) {
-        const int32_t rc = forced_check(d);
-        if (rc) return rc;
+    const bool disc = d.sensealg == B200UDE_DISCRETE_ADJOINT, want64 = d.dtype == B200UDE_F64, adaptive = d.adaptive != 0;
+    const bool fkpp = d.model == B200UDE_MODEL_FKPP;
+    if ((d.flags & B200UDE_FLAG_CHECKPOINT) && !(fkpp && adaptive && d.solver == B200UDE_TSIT5 && d.sensealg == B200UDE_INTERPOLATING_ADJOINT))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: B200UDE_FLAG_CHECKPOINT applies to adaptive Tsit5 with the interpolating adjoint on the Fisher-KPP UPDE; not to "
+                    "fixed step, Vern7, RKC2, the discrete adjoint or other models");
+    if (d.model == B200UDE_MODEL_OPERATOR) {
+        *route = R_OPERATOR;
+        return operator_check(&d);
     }
-    if (!forced && d->n_loss_weights != 0 && d->n_loss_weights != d->state_dim) return fail(nullptr, B200UDE_EINVAL, "create: n_loss_weights must be 0 or state_dim");
-    KernelId kid = pick_kernel(*d);
-    const bool want64 = d->dtype == B200UDE_F64;
-    const bool disc = d->sensealg == B200UDE_DISCRETE_ADJOINT;
+    if (d.model == B200UDE_MODEL_FORCED) {
+        *route = R_FORCED;
+        return forced_check(&d);
+    }
+    if (d.n_loss_weights != 0 && d.n_loss_weights != d.state_dim) return fail(nullptr, B200UDE_EINVAL, "create: n_loss_weights must be 0 or state_dim");
+    // the tuned chains
+    const bool shape_ok = generic_ok(d);   // the runtime-shape envelope
+    const bool lv_out = d.model == B200UDE_MODEL_LV && d.state_dim == 2 && d.acts[d.n_layers - 1] == B200UDE_ACT_IDENTITY;
+    const bool lv32 = lv_out && d.n_layers == 3 && d.widths[0] == 2 && d.widths[1] == 32 && d.widths[2] == 32 && d.widths[3] == 2 &&
+                      d.acts[0] == B200UDE_ACT_TANH && d.acts[1] == B200UDE_ACT_TANH && d.n_prefix == 0;
+    const bool lv5 = lv_out && d.n_layers == 4 && d.widths[0] == 2 && d.widths[1] == 5 && d.widths[2] == 5 && d.widths[3] == 5 &&
+                     d.widths[4] == 2 && d.n_prefix >= 0 && d.n_prefix <= 2;
+    const bool tanh64 = d.n_layers == 3 && d.acts[0] == B200UDE_ACT_TANH && d.acts[1] == B200UDE_ACT_TANH && d.acts[2] == B200UDE_ACT_IDENTITY;
+    const bool seir64 = shape_ok && tanh64 && d.model == B200UDE_MODEL_SEIR && d.widths[1] == 64 && d.widths[2] == 64 && d.n_suffix == 0 &&
+                        env_int("B200UDE_SEIR_TC", 1);
+    const bool fkpp16 = shape_ok && tanh64 && fkpp && d.widths[1] == 16 && d.widths[2] == 16 && env_int("B200UDE_FKPP_TUNED", 1);
     // discrete adjoint: the tuned LV kernels (fixed-step Tsit5 on 2-32-32-2 / 2-5-5-5-2, fp32), the runtime-shape kernels of
     // discrete_adjoint.cuh and, for the Fisher-KPP UPDE, the grid-per-CTA adaptive Vern7 kernels of fkpp_vern7_discrete.cuh.
     // Adaptive Tsit5 saves through its free interpolant, which an exact discrete adjoint would also have to differentiate;
     // fixed-step Fisher-KPP and RKC2 have no such kernels.
     // B200UDE_FLAG_DISCRETE_DENSE: the discrete adjoint of the Vern7 solve that saves through its lazy interpolant
     // (vern7_dense_discrete.cuh); on a fixed grid the saves are step ends and the flag selects nothing
-    const bool disc_dense = (d->flags & B200UDE_FLAG_DISCRETE_DENSE) != 0;
-    if (disc_dense && (d->solver != B200UDE_VERN7 || !disc || d->model == B200UDE_MODEL_FKPP || (d->flags & B200UDE_FLAG_VERN7_DENSE)))
+    const bool disc_dense = (d.flags & B200UDE_FLAG_DISCRETE_DENSE) != 0;
+    if (disc_dense && (d.solver != B200UDE_VERN7 || !disc || fkpp || (d.flags & B200UDE_FLAG_VERN7_DENSE)))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: B200UDE_FLAG_DISCRETE_DENSE applies to Vern7 with the discrete adjoint on the LV / SEIR / SEIR_NODE / NODE forms; "
                     "not to the interpolating adjoint (B200UDE_FLAG_VERN7_DENSE is its flag, and the two exclude each other), Tsit5, RKC2 or "
                     "the Fisher-KPP UPDE");
-    const bool fkpp_v7 = d->model == B200UDE_MODEL_FKPP && d->adaptive && d->solver == B200UDE_VERN7;
-    if (disc && ((d->model == B200UDE_MODEL_FKPP && !fkpp_v7) || d->solver == B200UDE_RKC2 || (d->adaptive && d->solver == B200UDE_TSIT5)))
+    const bool fkpp_v7 = fkpp && adaptive && d.solver == B200UDE_VERN7;
+    if (disc && ((fkpp && !fkpp_v7) || d.solver == B200UDE_RKC2 || (adaptive && d.solver == B200UDE_TSIT5)))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: the discrete adjoint (ForwardDiffSensitivity) has kernels for fixed-step Tsit5 and for fixed-step or adaptive Vern7 on the "
                     "LV / SEIR / SEIR_NODE / NODE forms (chain widths <= 64), and for adaptive Vern7 on the Fisher-KPP UPDE, fp32 and fp64; "
                     "not for adaptive Tsit5, fixed-step Fisher-KPP or RKC2");
     // Vern7's lazy dense output (vern7_dense.cuh): saveat through the interpolant and the interpolating adjoint over it.  The
     // discrete adjoint through an interpolated save has its own flag (above)
-    const bool v7dense = (d->flags & B200UDE_FLAG_VERN7_DENSE) != 0;
-    if (v7dense && (d->solver != B200UDE_VERN7 || d->sensealg != B200UDE_INTERPOLATING_ADJOINT || d->model == B200UDE_MODEL_FKPP))
+    const bool v7dense = (d.flags & B200UDE_FLAG_VERN7_DENSE) != 0;
+    if (v7dense && (d.solver != B200UDE_VERN7 || d.sensealg != B200UDE_INTERPOLATING_ADJOINT || fkpp))
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: B200UDE_FLAG_VERN7_DENSE applies to Vern7 with the interpolating adjoint on the LV / SEIR / SEIR_NODE / NODE forms; "
                     "not to the discrete adjoint, Tsit5, RKC2 or the Fisher-KPP UPDE");
-    if (want64 && !forced) {
+    const bool tol_ok = d.abstol > 0 && d.reltol > 0 && d.max_steps >= 1;
+    if (want64) {
         // fp64: the runtime-shape one-trajectory-per-thread kernels (ude_generic.cuh in fp64, k_f64.cu): LV / SEIR / NODE forms, Tsit5 and Vern7,
         // fixed step and adaptive, interpolating or discrete adjoint; the Fisher-KPP UPDE with adaptive Tsit5 (fkpp_adaptive.cuh)
-        if (!generic_ok(*d) || d->solver == B200UDE_RKC2)
+        if (!shape_ok || d.solver == B200UDE_RKC2)
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: B200UDE_F64 kernels exist for the LV / SEIR / NODE forms (chain widths <= 64), Tsit5 / Vern7, and the Fisher-KPP UPDE "
                         "with adaptive Tsit5 and the interpolating adjoint");
-        if (d->model == B200UDE_MODEL_FKPP && (!d->adaptive || !(d->solver == B200UDE_TSIT5 || (fkpp_v7 && disc))))
+        if (fkpp && (!adaptive || !(d.solver == B200UDE_TSIT5 || (fkpp_v7 && disc))))
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: B200UDE_F64 Fisher-KPP runs adaptive Tsit5 (interpolating adjoint) and adaptive Vern7 with the discrete adjoint "
                         "only; fixed-step Fisher-KPP is fp32");
-        if (d->adaptive && (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1))
-            return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
-        kid = d->model == B200UDE_MODEL_FKPP ? K_FKPP : K_GENERIC;
+        if (adaptive && !tol_ok) return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
     }
-    if (!want64 && d->solver == B200UDE_VERN7) {
-        if (!generic_ok(*d) || (d->model == B200UDE_MODEL_FKPP && !(fkpp_v7 && disc)))
-            return fail(nullptr, B200UDE_EUNSUPPORTED,
-                        "create: Vern7 kernels exist for the LV / SEIR / NODE forms, and for the Fisher-KPP UPDE adaptive with the discrete adjoint");
-        // fixed-step Vern7 of the SEIR 3-64-64-1 chain runs on the tensor-core kernels (and so does the Tsit5 re-solve its
-        // adjoint uses); every other Vern7 configuration on the runtime-shape kernels
-        // (the discrete adjoint of a Vern7 solve and the dense-output flag run on the runtime-shape kernels only)
-        if (disc || v7dense || !(kid == K_SEIR64 && !d->adaptive && env_int("B200UDE_SEIR_VERN7_TC", 1))) kid = K_GENERIC;
-    }
-    if (!want64 && d->adaptive && !forced) {
-        if (!(d->abstol > 0) || !(d->reltol > 0) || d->max_steps < 1)
-            return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
-        if (!generic_ok(*d))
+    if (!want64 && d.solver == B200UDE_VERN7 && (!shape_ok || (fkpp && !(fkpp_v7 && disc))))
+        return fail(nullptr, B200UDE_EUNSUPPORTED,
+                    "create: Vern7 kernels exist for the LV / SEIR / NODE forms, and for the Fisher-KPP UPDE adaptive with the discrete adjoint");
+    if (!want64 && adaptive) {
+        if (!tol_ok) return fail(nullptr, B200UDE_EINVAL, "create: adaptive stepping needs abstol > 0, reltol > 0, max_steps >= 1");
+        if (!shape_ok)
             return fail(nullptr, B200UDE_EUNSUPPORTED, "create: adaptive stepping is implemented for the LV / SEIR / NODE forms and the Fisher-KPP UPDE (chain widths <= 64)");
-        if (d->model == B200UDE_MODEL_FKPP) {
-            // Fisher-KPP: runtime-shape grid-per-CTA kernels (fkpp_adaptive.cuh; fkpp_vern7_discrete.cuh for Vern7 with the discrete
-            // adjoint), the tuned 1-16-16-1 chain included
-            if (d->solver != B200UDE_TSIT5 && !(fkpp_v7 && disc))
-                return fail(nullptr, B200UDE_EUNSUPPORTED,
-                            "create: adaptive stepping of the Fisher-KPP UPDE is implemented for Tsit5, and for Vern7 with the discrete adjoint");
-            kid = K_FKPP;
-        } else if (!((kid == K_LV32 || kid == K_SEIR64) && d->solver == B200UDE_TSIT5 && env_int("B200UDE_ADAPTIVE_TC", 1))) {
-            // adaptive solves run on the runtime-shape kernels, except the headline chain (tensor-core kernels with CTA-uniform attempt loops)
-            kid = K_GENERIC;
-        }
+        if (fkpp && d.solver != B200UDE_TSIT5 && !(fkpp_v7 && disc))
+            return fail(nullptr, B200UDE_EUNSUPPORTED,
+                        "create: adaptive stepping of the Fisher-KPP UPDE is implemented for Tsit5, and for Vern7 with the discrete adjoint");
     }
-    if (d->solver == B200UDE_RKC2) {
-        if (d->n_stages < 2 || d->n_stages > 64) return fail(nullptr, B200UDE_EINVAL, "create: RKC2 needs 2 <= n_stages <= 64 (stability interval ~ 0.65 n_stages^2 >= dt * spectral radius)");
-        if (kid != K_FKPP16 || d->state_dim % 2 != 0 || d->adaptive || d->sensealg != B200UDE_INTERPOLATING_ADJOINT || !env_int("B200UDE_FKPP_PACKED", 1))
+    if (d.solver == B200UDE_RKC2) {
+        if (d.n_stages < 2 || d.n_stages > 64) return fail(nullptr, B200UDE_EINVAL, "create: RKC2 needs 2 <= n_stages <= 64 (stability interval ~ 0.65 n_stages^2 >= dt * spectral radius)");
+        if (!fkpp16 || d.state_dim % 2 != 0 || adaptive || d.sensealg != B200UDE_INTERPOLATING_ADJOINT || !env_int("B200UDE_FKPP_PACKED", 1))
             return fail(nullptr, B200UDE_EUNSUPPORTED,
                         "create: RKC2 has kernels for the Fisher-KPP UPDE with the 1-16-16-1 chain on even grids (fixed step, interpolating adjoint)");
     }
-    // fixed-step Tsit5 with the discrete adjoint: LV 2-32-32-2 / 2-5-5-5-2 keep their tuned kernels, every other form runs on the
-    // runtime-shape ones (the SEIR tensor-core kernels have no discrete adjoint)
-    if (disc && !want64 && kid != K_NONE && !(kid == K_LV32 || kid == K_LV5P0 || kid == K_LV5P1 || kid == K_LV5P2 || kid == K_FKPP)) kid = K_GENERIC;
-    if (forced) kid = K_FORCED;
-    if (kid == K_NONE)
+    if (!shape_ok && !lv32 && !lv5)
         return fail(nullptr, B200UDE_EUNSUPPORTED,
                     "create: no sm_90a kernel for this model/chain (built: LV 2-32-32-2 tanh; LV 2-5-5-5-2; generic LV/SEIR/NODE chains with widths <= 64, <= 5 layers)");
-    *kid_out = kid;
+    // every check passed: the tuned fp32 kernels where they exist, the runtime-shape kernels for the rest.  The Fisher-KPP UPDE runs
+    // adaptive on grid-per-CTA kernels (fkpp_adaptive.cuh; fkpp_vern7_discrete.cuh for Vern7), the tuned 1-16-16-1 chain included
+    const bool tsit5 = d.solver == B200UDE_TSIT5;
+    if (fkpp && adaptive) *route = !tsit5 ? R_FKPP_VERN7_DISCRETE : (d.flags & B200UDE_FLAG_CHECKPOINT) ? R_FKPP_CHECKPOINT : R_FKPP_ADAPTIVE;
+    else if (fkpp) *route = !fkpp16 ? R_FKPP_FIXED : tsit5 ? R_FKPP16 : R_FKPP16_RKC2;
+    // fixed-step Tsit5 with the discrete adjoint: LV 2-32-32-2 / 2-5-5-5-2 keep their tuned kernels (the SEIR tensor-core kernels have none)
+    else if (!want64 && tsit5 && !adaptive && (lv32 || lv5 || (seir64 && !disc))) *route = lv32 ? (disc ? R_LV32_DISCRETE : R_LV32) : lv5 ? R_LV5 : R_SEIR64;
+    // adaptive: the headline chains on tensor-core kernels with CTA-uniform attempt loops
+    else if (!want64 && tsit5 && adaptive && (lv32 || seir64) && env_int("B200UDE_ADAPTIVE_TC", 1)) *route = lv32 ? R_LV32_ADAPTIVE : R_SEIR64_ADAPTIVE;
+    // fixed-step Vern7 of the SEIR 3-64-64-1 chain (and the Tsit5 re-solve its adjoint uses) on the tensor-core kernels
+    else if (!want64 && d.solver == B200UDE_VERN7 && seir64 && !adaptive && !disc && !v7dense && env_int("B200UDE_SEIR_VERN7_TC", 1)) *route = R_SEIR64_VERN7;
+    else if (tsit5) *route = disc ? R_DISCRETE_TSIT5 : R_TSIT5;
+    else if (v7dense) *route = R_VERN7_DENSE;
+    else *route = !disc ? R_VERN7 : adaptive && disc_dense ? R_VERN7_DENSE_DISCRETE : R_DISCRETE_VERN7;
     return B200UDE_OK;
 }
 
@@ -915,15 +890,15 @@ int32_t probe_device(const b200ude_desc *d, cudaDeviceProp *prop)
 size_t partial_rows(const b200ude_handle *h)
 {
     const int N = (int)h->cap;
-    switch (h->kid) {
-    case K_OPERATOR: return (size_t)adj_rows_operator(N, h->oh.warps);
-    case K_FORCED: return (size_t)adj_rows_forced(N, h->f64 ? 1 : 0);
-    case K_GENERIC: return (size_t)(h->f64 ? RuntimeShape<double>::adj_rows(N) : RuntimeShape<float>::adj_rows(N));
-    case K_FKPP: return (size_t)adj_rows_fkpp(N, h->D);
-    case K_LV32: return (size_t)std::max(adj_grid_lv32(N), adj_rows_lv32_wm(N));
-    case K_SEIR64: return (size_t)adj_rows_seir(N);
-    case K_FKPP16: return (size_t)adj_rows_fkpp16(N, h->D);
-    default: return (size_t)adj_grid_lv5(N);
+    switch (h->route) {
+    case R_OPERATOR: return (size_t)adj_rows_operator(N, h->oh.warps);
+    case R_FORCED: return (size_t)adj_rows_forced(N, h->f64 ? 1 : 0);
+    case R_LV32: case R_LV32_DISCRETE: case R_LV32_ADAPTIVE: return (size_t)std::max(adj_grid_lv32(N), adj_rows_lv32_wm(N));
+    case R_LV5: return (size_t)adj_grid_lv5(N);
+    case R_SEIR64: case R_SEIR64_VERN7: case R_SEIR64_ADAPTIVE: return (size_t)adj_rows_seir(N);
+    case R_FKPP16: case R_FKPP16_RKC2: return (size_t)adj_rows_fkpp16(N, h->D);
+    case R_FKPP_FIXED: case R_FKPP_ADAPTIVE: case R_FKPP_CHECKPOINT: case R_FKPP_VERN7_DISCRETE: return (size_t)adj_rows_fkpp(N, h->D);
+    default: return (size_t)(h->f64 ? RuntimeShape<double>::adj_rows(N) : RuntimeShape<float>::adj_rows(N));
     }
 }
 
@@ -956,16 +931,11 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     if (!(d->dt > 0) || d->n_steps < 1 || d->save_every < 1 || d->n_steps % d->save_every != 0)
         return fail(nullptr, B200UDE_EINVAL, "create: need dt>0, n_steps>=1, save_every>=1 dividing n_steps");
     if (d->max_trajectories == 0 || d->max_trajectories > (1ull << 26)) return fail(nullptr, B200UDE_EINVAL, "create: max_trajectories out of range");
-    const bool op = d->model == B200UDE_MODEL_OPERATOR, forced = d->model == B200UDE_MODEL_FORCED, want64 = d->dtype == B200UDE_F64;
     // the descriptor is validated before the device check, so that it is testable without a GPU
-    if ((d->flags & B200UDE_FLAG_CHECKPOINT) &&
-        !(d->model == B200UDE_MODEL_FKPP && d->adaptive && d->solver == B200UDE_TSIT5 && d->sensealg == B200UDE_INTERPOLATING_ADJOINT))
-        return fail(nullptr, B200UDE_EUNSUPPORTED,
-                    "create: B200UDE_FLAG_CHECKPOINT applies to adaptive Tsit5 with the interpolating adjoint on the Fisher-KPP UPDE; not to "
-                    "fixed step, Vern7, RKC2, the discrete adjoint or other models");
-    KernelId kid = K_OPERATOR;
-    int32_t rc = op ? operator_check(d) : select_kernel(d, &kid);
+    Route route;
+    int32_t rc = resolve(*d, &route);
     if (rc) return rc;
+    const bool op = route == R_OPERATOR, forced = route == R_FORCED, want64 = d->dtype == B200UDE_F64;
     OperatorHost oh{};
     if (op) {
         oh.dtype = want64 ? 1 : 0; oh.D = d->state_dim; oh.M = d->widths[d->n_layers]; oh.L = d->n_layers;
@@ -979,8 +949,8 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     cudaDeviceProp prop;
     rc = probe_device(d, &prop);
     if (rc) return rc;
-    const int P = op ? oh.P : num_params(d, kid);
-    if (d->model == B200UDE_MODEL_FKPP && d->adaptive) {
+    const int P = op ? oh.P : num_params(d, route);
+    if (route == R_FKPP_ADAPTIVE || route == R_FKPP_CHECKPOINT || route == R_FKPP_VERN7_DISCRETE) {
         // the adjoint keeps one gradient vector (P + 1 entries) per warp in shared memory: refuse here what could not launch
         const size_t smem = fkpp_adaptive_smem(d->state_dim, P, want64 ? (int)sizeof(double) : (int)sizeof(float)) + 16;   // + static
         if (smem > prop.sharedMemPerBlockOptin)
@@ -1004,14 +974,17 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
                         "(%zu B dynamic + %zu B static; device limit %zu B)",
                         oh.D, oh.M, oh.P, operator_smem(oh, 1) + stat, operator_smem(oh, 1), stat, (size_t)prop.sharedMemPerBlockOptin);
     }
-    if (!want64 && (kid == K_GENERIC || kid == K_FKPP || kid == K_FORCED) && P > 12288)
+    // the fp32 runtime-shape, Fisher-KPP and forced kernels read theta from the constant bank
+    const bool tuned = route == R_LV32 || route == R_LV32_DISCRETE || route == R_LV32_ADAPTIVE || route == R_LV5 || route == R_SEIR64 ||
+                       route == R_SEIR64_VERN7 || route == R_SEIR64_ADAPTIVE || route == R_FKPP16 || route == R_FKPP16_RKC2;
+    if (!want64 && !tuned && !op && P > 12288)
         return fail(nullptr, B200UDE_EUNSUPPORTED, "create: %d parameters exceed the constant-bank budget", P);
 
     b200ude_handle *h = new (std::nothrow) b200ude_handle();
     if (!h) return fail(nullptr, B200UDE_ENOMEM, "create: out of host memory");
     const uint64_t serial = ++g_serial;   // taken once: the shape and the tables must agree
     h->desc = *d;
-    h->kid = kid;
+    h->route = route;
     h->f64 = want64;
     h->D = h->DR = d->state_dim;
     h->n_save = d->n_steps / d->save_every + 1;
@@ -1022,9 +995,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
     h->oh = oh;
     h->var.approx_tanh = (d->flags & B200UDE_FLAG_APPROX_TANH) ? 1 : 0;
     h->var.discrete = d->sensealg == B200UDE_DISCRETE_ADJOINT ? 1 : 0;
-    h->vern7_dense = (d->flags & B200UDE_FLAG_VERN7_DENSE) != 0;
-    h->discrete_dense = (d->flags & B200UDE_FLAG_DISCRETE_DENSE) && d->adaptive;
-    if (d->solver == B200UDE_RKC2) rkc2_tables(d->n_stages, &h->rkc);
+    if (route == R_FKPP16_RKC2) rkc2_tables(d->n_stages, &h->rkc);
     // tuning knobs for experiments (defaults are the measured-best variant, see DESIGN.md)
     h->var.fwd_smem = env_int("B200UDE_FWD_SMEM", 0);
     // default: tensor-core (3xTF32 mma.sync) kernels; B200UDE_FWD_TC=0 / B200UDE_ADJ_TC=0 select the packed CUDA-core kernels
@@ -1042,20 +1013,20 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
 
     const size_t N = h->cap, D = (size_t)h->D, es = h->es();
     const size_t rec = h->adaptive ? (size_t)d->max_steps : (size_t)d->n_steps;   // capacity of the step record
-    // a discrete-adjoint or dense-output Vern7 handle recomputes the stages from u_n: no dense record, the step sizes instead when adaptive
-    const bool disc_vern7 = (h->var.discrete && d->solver == B200UDE_VERN7) || h->vern7_dense;
+    // the discrete adjoint of Vern7 and Vern7's dense output recompute the stages from u_n: no dense record, the step sizes instead
+    // when adaptive
+    const bool from_un = route == R_DISCRETE_VERN7 || route == R_VERN7_DENSE || route == R_VERN7_DENSE_DISCRETE || route == R_FKPP_VERN7_DISCRETE;
     const size_t dense_rows = oh.rkc2 ? rec + 1 : rec * 6 + 1;   // operator RKC2: f(u_n); Tsit5: the stages
-    // B200UDE_FLAG_CHECKPOINT (adaptive Tsit5 Fisher-KPP only, checked above): u_n every K accepted steps in place of ustep, the
-    // adjoint's scratch area for one segment (6K + 1 stage rows, K + 1 state rows) in place of dense, the step sizes.  K minimises
-    // max_steps / K + 7K, the rows of both
-    if (d->flags & B200UDE_FLAG_CHECKPOINT) h->seg = std::max(1, (int)std::lround(std::sqrt((double)d->max_steps / 7.0)));
+    // R_FKPP_CHECKPOINT: u_n every K accepted steps in place of ustep, the adjoint's scratch area for one segment (6K + 1 stage
+    // rows, K + 1 state rows) in place of dense, the step sizes.  K minimises max_steps / K + 7K, the rows of both
+    if (route == R_FKPP_CHECKPOINT) h->seg = std::max(1, (int)std::lround(std::sqrt((double)d->max_steps / 7.0)));
     const size_t seg = (size_t)h->seg;
     const size_t ustep_rows = seg ? (rec + seg - 1) / seg + 1 : rec + 1, dense_alloc = seg ? 7 * seg + 2 : dense_rows;
     // theta: the fp32 runtime-shape and tuned kernels read it as float4
     const size_t theta_n = want64 || forced || op ? (size_t)P + 1 : (size_t)((P + 3) / 4) * 4;
     h->partial_blocks = partial_rows(h);
     bool ok = dalloc_real(h, &h->d_theta, theta_n) == cudaSuccess && dalloc_real(h, &h->d_ustep, ustep_rows * D * N) == cudaSuccess &&
-              (disc_vern7 || dalloc_real(h, &h->d_dense, dense_alloc * D * N) == cudaSuccess) &&
+              (from_un || dalloc_real(h, &h->d_dense, dense_alloc * D * N) == cudaSuccess) &&
               dalloc_real(h, &h->d_partial, h->partial_blocks * (size_t)(P + 1)) == cudaSuccess;
     if (!want64) ok = ok && dalloc(h, &h->d_grad, (size_t)P) == cudaSuccess && dalloc(h, &h->d_loss, 1) == cudaSuccess;
     if (h->adaptive) {
@@ -1064,7 +1035,7 @@ int32_t b200ude_create(const b200ude_desc *d, b200ude_handle **out)
             ok = ok && dalloc_real(h, &h->d_usave, (size_t)h->n_save * D * N) == cudaSuccess;
         else   // the cotangent of the fused L2 and, in fp32, its per-block losses
             ok = ok && dalloc_real(h, &h->d_cot, (size_t)h->n_save * D * N) == cudaSuccess &&
-                 (!(disc_vern7 || seg) || dalloc_real(h, &h->d_hstep, rec * N) == cudaSuccess) &&
+                 (!(from_un || seg) || dalloc_real(h, &h->d_hstep, rec * N) == cudaSuccess) &&
                  (want64 || dalloc(h, &h->d_block_loss, (size_t)L2_BLOCKS) == cudaSuccess);
     }
     if (forced) ok = ok && dalloc_real(h, &h->d_forcing, 3 * (size_t)d->consts[1] * N) == cudaSuccess;
@@ -1181,7 +1152,7 @@ int32_t b200ude_set_params(b200ude_handle *h, const void *theta, size_t P, int32
 int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32_t mem, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid != K_FORCED) return fail(h, B200UDE_EUNSUPPORTED, "set_forcing: only B200UDE_MODEL_FORCED handles take a forcing (this handle: model %d)", h->desc.model);
+    if (h->route != R_FORCED) return fail(h, B200UDE_EUNSUPPORTED, "set_forcing: only B200UDE_MODEL_FORCED handles take a forcing (this handle: model %d)", h->desc.model);
     if (!coef || N == 0 || N > h->cap) return fail(h, B200UDE_EINVAL, "set_forcing: null pointer or N=%zu outside (0, max_trajectories=%zu]", N, h->cap);
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
     const size_t es = h->es();
@@ -1196,7 +1167,7 @@ int32_t b200ude_set_forcing(b200ude_handle *h, const void *coef, size_t N, int32
 int32_t b200ude_set_operators(b200ude_handle *h, const void *D1, const void *D2, int32_t mem, void *stream)
 {
     if (!h) return B200UDE_EINVAL;
-    if (h->kid != K_OPERATOR) return fail(h, B200UDE_EUNSUPPORTED, "set_operators: only B200UDE_MODEL_OPERATOR handles take operators (this handle: model %d)", h->desc.model);
+    if (h->route != R_OPERATOR) return fail(h, B200UDE_EUNSUPPORTED, "set_operators: only B200UDE_MODEL_OPERATOR handles take operators (this handle: model %d)", h->desc.model);
     if (!D1) return fail(h, B200UDE_EINVAL, "set_operators: D1 is a null pointer");
     CUDA_TRY(h, cudaSetDevice(h->desc.device));
     const OperatorHost &o = h->oh;
