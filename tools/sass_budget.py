@@ -3,9 +3,11 @@
 
 Compiles k_lv32_wm.cu for sm_90a with the library's flags into a temporary directory (or reads a given object), then for the
 default forward and adjoint instantiations at N = 65 536 prints the registers, the spill traffic, and the opcode counts of
-the stage loop: the smallest loop of the kernel that holds all of its tensor-core instructions (HMMA counted by shape:
-m16n8k16 fp16, m16n8k8 fp16, m16n8k8 TF32).  Loops nested in the stage
-loop, and the loop around it (the per-step code), are listed too.  Also counts the instructions of one tanh_quad_z.
+the stage loop (the smallest loop that holds a tensor-core instruction; HMMA counted by shape: m16n8k16 fp16, m16n8k8 fp16,
+m16n8k8 TF32) and of the step loop around it, and the instructions one step issues: the stage loop times its trip count
+plus the rest of the step loop (branches taken once per solve or on rare rescales included).  The forward's stage loop runs
+6 times per step; the adjoint's runs stages 1..4, and stage 5 with the next step's stage 0 (the state they share) is step
+code.  Also counts the instructions of one tanh_quad_z.
 
     python tools/sass_budget.py                   # compile the working tree's k_lv32_wm.cu
     python tools/sass_budget.py --obj k_lv32_wm.o # read a compiled object (spills then come from LDL/STL counts only)
@@ -123,16 +125,19 @@ def row(label, c):
     return f"  {label:34s} {c['total']:6d} " + " ".join(f"{c[col]:>7d}" for col, _ in COLUMNS)
 
 
-def report(fname, funcs, res, spills):
+STAGE_TRIPS = {"forward": 6, "adjoint": 4}   # stage-loop iterations per step
+
+
+def report(fname, funcs, res, spills, trips):
     insns, labels = funcs[fname]
     hm = [a for a, op, _ in insns if op.startswith("HMMA")]
     ls = loops(insns, labels)
-    stage = next((l for l in ls if l[0] <= min(hm) and max(hm) <= l[1]), None) if hm else None
+    stage = next((l for l in ls if any(l[0] <= a <= l[1] for a in hm)), None)
     print(f"{fname}")
     print(f"  registers {res.get('REG', '?')}, local memory {res.get('LOCAL', '?')} B, {spills}")
     print(f"  {'region':34s} {'insns':>6s} " + " ".join(f"{col:>7s}" for col, _ in COLUMNS))
     if stage is None:
-        print("  (no loop holds every HMMA)")
+        print("  (no loop holds an HMMA)")
         return
     print(row("stage loop", count(insns, *stage)))
     for l in ls:
@@ -140,7 +145,10 @@ def report(fname, funcs, res, spills):
             print(row(f"  nested loop {l[0]:#x}..{l[1]:#x}", count(insns, *l)))
     outer = next((l for l in ls if l[0] <= stage[0] and stage[1] <= l[1] and l != stage), None)
     if outer:
-        print(row("step loop (stage loop included)", count(insns, *outer)))
+        cs, co = count(insns, *stage), count(insns, *outer)
+        print(row("step loop (stage loop included)", co))
+        per_step = collections.Counter({k: trips * cs[k] + co[k] - cs[k] for k in co})
+        print(row(f"per step: {trips} x stage loop + rest", per_step))
     print(row("whole kernel", count(insns, 0, 1 << 40)))
 
 
@@ -209,7 +217,7 @@ def main():
         insns = funcs[fname][0]
         sp = spills.get(fname) or f"{sum(1 for _, op, _ in insns if op.startswith(('STL', 'LDL')))} LDL/STL instructions"
         print(f"== {what}: ", end="")
-        report(fname, funcs, res.get(fname, {}), sp)
+        report(fname, funcs, res.get(fname, {}), sp, STAGE_TRIPS[what])
     if tanh is not None:
         fp = tanh["FP32"] + tanh["MUFU"]
         print(f"== tanh_quad_z<0> (four values): {fp} instructions: {tanh['MUFU']} MUFU, {tanh['FP32']} FFMA/FMUL/FADD/FMNMX")

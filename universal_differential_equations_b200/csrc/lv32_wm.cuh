@@ -439,6 +439,15 @@ constexpr int stage_headroom()
 constexpr int STAGE_HEADROOM = stage_headroom();
 static_assert(STAGE_HEADROOM == 6, "Tsit5: max |b_i| / b_0 = 34.1");
 
+// the lambda-free part of a backward stage at one state: what the cotangent products of that point read
+template <int R>
+struct ChainRows {
+    float xo;                           // own component of the state (its rows are gathered where they are used)
+    float2 om1[R][4];                   // 1 - h1^2
+    uint32_t h1hi[R][4], h1lo[R][4];    // h1 split once: A operand of layer 2, (transposed) B operand of dW2
+    float2 h2[R][4];                    // tanh of layer 2
+};
+
 template <int TM, int R, int WPC, int MINB>
 __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Consts cs)
 {
@@ -493,23 +502,128 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
         }
     };
 
-    // one backward stage: xo = own component of u(t), go = own component of the stage's lambda argument, sc = dt b_i;
-    // first = the first stage since macc was flushed
-    auto eval = [&](float xo, float go, float sc, float isc, bool first) -> float {
-        float x[1][R][2], sg[R][2];
+    // A backward stage is three parts: the chain forward at its state (lambda-free), the VJP of its lambda argument (the
+    // cotangent rows sg = dt b_i lambda-argument give q2, W2^T q2, q1 and the stage's k) and the theta sums, linear in sg.
+    // Where two stages share a state, the chain forward runs once and dW3 once, on the summed rows.
+
+    // the chain forward at the state whose own component is xo
+    auto chain = [&](float xo, ChainRows<R> &c) {
+        float x[1][R][2];
         gather4<R>(L, xo, x[0]);
-        const float sgo = lv * sc * go;
-        gather4<R>(L, sgo, sg);
-        gb3 += sgo;
-        // Every cotangent row q2[t][.] is scaled by a power of two into fp16's range for the W2^T q2 product (|q2[t][j]| <=
-        // max|W3| (|sg_t0| + |sg_t1|) =: B_t; scale 2^(127 - e_t), e_t = biased exponent of B_t, undone on the product -- both exact)
-        uint32_t eb[R];   // e_t
+        c.xo = xo;
+        float2 h1[1][R][4];
+        layer1<TM, 1, R>(w, L, x, h1);
+        split_rows<R>(h1[0], c.h1hi, c.h1lo);
+        float d[4][4];
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+            const float2 bias = lds2(w.b2 + 8 * nt + 2 * L.tig);
+            d[nt][0] = bias.x; d[nt][1] = bias.y; d[nt][2] = bias.x; d[nt][3] = bias.y;
+        }
+        gemm32h_w<R>(w.w2h_hi, w.w2h_lo, L, c.h1hi, c.h1lo, d);
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            float2 v[4];
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) v[nt] = make_float2(d[nt][2 * r], d[nt][2 * r + 1]);
+            tanh_quad_z<TM>(v[0], v[1]);
+            tanh_quad_z<TM>(v[2], v[3]);
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                c.h2[r][nt] = v[nt];
+                const float2 hh = h1[0][r][nt];
+                c.om1[r][nt] = fma2(make_float2(-hh.x, -hh.y), hh, bc(1.0f));
+            }
+        }
+    };
+    // Every cotangent row q2[t][.] is scaled by a power of two into fp16's range for the W2^T q2 product (|q2[t][j]| <=
+    // max|W3| (|sg_t0| + |sg_t1|) =: B_t; scale 2^(127 - e_t), e_t = biased exponent of B_t, undone on the product -- both exact)
+    auto row_exp = [&](const float (&sg)[R][2], uint32_t (&eb)[R]) {
 #pragma unroll
         for (int r = 0; r < R; ++r) eb[r] = (__float_as_uint(wt.w3max * (fabsf(sg[r][0]) + fabsf(sg[r][1]))) >> 23) & 0xFFu;
+    };
+    // the scaled rows 2^(127 - e_t) q2 as fp16 hi/lo words: operand of W2^T q2 and (transposed) of dW2
+    auto split_q2 = [&](const float2 (&q2)[R][4], const uint32_t (&eb)[R], uint32_t (&hi)[R][4], uint32_t (&lo)[R][4]) {
+        float2 q2s[R][4];
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const float2 sc2 = bc(__uint_as_float((254u - eb[r]) << 23));
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) q2s[r][nt] = mul2(q2[r][nt], sc2);
+        }
+        split_rows<R>(q2s, hi, lo);
+    };
+    // q2 = (W3^T sg) (1 - h2^2) of cotangent rows sg; db2 += q2
+    auto q2_rows = [&](const ChainRows<R> &c, const float (&sg)[R][2], float2 (&q2)[R][4]) {
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const float2 s0 = bc(sg[r][0]), s1 = bc(sg[r][1]);
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                const float2 w3a = lds2(w.w3a + 8 * nt + 2 * L.tig), w3b = lds2(w.w3b + 8 * nt + 2 * L.tig);
+                const float2 t = fma2(w3b, s1, mul2(w3a, s0));
+                const float2 v = c.h2[r][nt];
+                const float2 om = fma2(make_float2(-v.x, -v.y), v, bc(1.0f));
+                q2[r][nt] = mul2(t, om);
+                gB2[nt] = add2(gB2[nt], q2[r][nt]);
+            }
+        }
+    };
+    // the VJP of one lambda argument from its q2 words (split_q2): go = own component of the lambda argument,
+    // isc = 1 / (dt b_i); returns the stage's own component of k.  dW1 += q1 (x) x and db1 += q1 are accumulated here,
+    // once per stage: q1 is not summed over the two stages of a shared point
+    auto vjp = [&](const ChainRows<R> &c, const uint32_t (&eb)[R], const uint32_t (&q2hi)[R][4], const uint32_t (&q2lo)[R][4],
+                   float go, float isc) -> float {
+        float2 unscale[R];
+#pragma unroll
+        for (int r = 0; r < R; ++r) unscale[r] = bc(__uint_as_float(eb[r] << 23));
+        float e[4][4];
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int c4 = 0; c4 < 4; ++c4) e[nt][c4] = 0.0f;
+        gemm32h_w<R>(wt.w2t_hi, wt.w2t_lo, L, q2hi, q2lo, e);
+        // q1 = (W2^T q2) (1 - h1^2); (df/du)^T g; dW1 += q1 (x) x, db1 += q1
+        float x[R][2], y[R][2];
+        gather4<R>(L, c.xo, x);
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            float2 s0 = bc(0.0f), s1 = bc(0.0f);
+            const float2 x0 = bc(x[r][0]), x1 = bc(x[r][1]);
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                const float2 om = mul2(c.om1[r][nt], unscale[r]);
+                const float2 q1 = mul2(make_float2(e[nt][2 * r], e[nt][2 * r + 1]), om);
+                s0 = fma2(lds2(wt.w1a + 8 * nt + 2 * L.tig), q1, s0);
+                s1 = fma2(lds2(wt.w1b + 8 * nt + 2 * L.tig), q1, s1);
+                gB1[nt] = add2(gB1[nt], q1);
+                gW1a[nt] = fma2(q1, x0, gW1a[nt]);
+                gW1b[nt] = fma2(q1, x1, gW1b[nt]);
+            }
+            y[r][0] = s0.x + s0.y;
+            y[r][1] = s1.x + s1.y;
+        }
+        const float dxo = scatter_sum<R>(L, y);
+        return fmaf(pc, go, dxo * isc);   // LV physics: diag(p1, -p4)
+    };
+    // dW3 += sg (x) h2
+    auto acc_w3 = [&](const ChainRows<R> &c, const float (&sg)[R][2]) {
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const float2 s0 = bc(sg[r][0]), s1 = bc(sg[r][1]);
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                gW3a[nt] = fma2(s0, c.h2[r][nt], gW3a[nt]);
+                gW3b[nt] = fma2(s1, c.h2[r][nt], gW3b[nt]);
+            }
+        }
+    };
+    // one stage's dW2 += q2^T h1 from the words of its q2 (split_q2); first = the first stage since macc was flushed
+    auto acc_w2 = [&](const ChainRows<R> &c, const uint32_t (&eb)[R], const uint32_t (&q2hi)[R][4], const uint32_t (&q2lo)[R][4], bool first) {
         // dW2 += q2^T h1 (below) sums over rows, so the rows' scales become one per group: the words of row t are
         // multiplied by 2^(e_t - e_acc) (exact down to fp16's subnormals; below them the error is at most 2^-24 B_max per
         // element), e_acc >= every e_t since the last flush.  All maxima are over the integer exponents, so an inf/NaN row
-        // (255) poisons the sums as a non-finite q2 does.  Settled here, first in the stage, so that the rest is one block.
+        // (255) poisons the sums as a non-finite q2 does.
         int e_max = (int)eb[0];
         if constexpr (R == 2) e_max = max(e_max, (int)eb[1]);
 #pragma unroll
@@ -523,55 +637,11 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
 #pragma unroll
                 for (int nt = 0; nt < 4; ++nt)
 #pragma unroll
-                    for (int c = 0; c < 4; ++c) macc[mt][nt][c] *= rs;
+                    for (int c4 = 0; c4 < 4; ++c4) macc[mt][nt][c4] *= rs;
             e_acc = e_max;
         }
-        float2 h1[1][R][4];
-        layer1<TM, 1, R>(w, L, x, h1);
-        // h1 split once: A operand of the chain forward, (transposed) B operand of dW2
-        uint32_t h1hi[R][4], h1lo[R][4];
-        split_rows<R>(h1[0], h1hi, h1lo);
-        float d[4][4];
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-            const float2 bias = lds2(w.b2 + 8 * nt + 2 * L.tig);
-            d[nt][0] = bias.x; d[nt][1] = bias.y; d[nt][2] = bias.x; d[nt][3] = bias.y;
-        }
-        gemm32h_w<R>(w.w2h_hi, w.w2h_lo, L, h1hi, h1lo, d);
-        // h2 = tanh(.), q2 = (W3^T sg) (1 - h2^2); dW3 += sg (x) h2, db2 += q2; the rows scaled by 2^(127 - e_t) (above)
-        float2 q2s[R][4], unscale[R];
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            float2 v[4];
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt) v[nt] = make_float2(d[nt][2 * r], d[nt][2 * r + 1]);
-            tanh_quad_z<TM>(v[0], v[1]);
-            tanh_quad_z<TM>(v[2], v[3]);
-            const float2 s0 = bc(sg[r][0]), s1 = bc(sg[r][1]);
-            const float2 sc2 = bc(__uint_as_float((254u - eb[r]) << 23));
-            unscale[r] = bc(__uint_as_float(eb[r] << 23));
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt) {
-                const float2 w3a = lds2(w.w3a + 8 * nt + 2 * L.tig), w3b = lds2(w.w3b + 8 * nt + 2 * L.tig);
-                gW3a[nt] = fma2(s0, v[nt], gW3a[nt]);
-                gW3b[nt] = fma2(s1, v[nt], gW3b[nt]);
-                const float2 t = fma2(w3b, s1, mul2(w3a, s0));
-                const float2 om = fma2(make_float2(-v[nt].x, -v[nt].y), v[nt], bc(1.0f));
-                const float2 q2 = mul2(t, om);
-                q2s[r][nt] = mul2(q2, sc2);
-                gB2[nt] = add2(gB2[nt], q2);
-            }
-        }
-        uint32_t q2hi[R][4], q2lo[R][4];
-        split_rows<R>(q2s, q2hi, q2lo);
-        float e[4][4];
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) e[nt][c] = 0.0f;
-        gemm32h_w<R>(wt.w2t_hi, wt.w2t_lo, L, q2hi, q2lo, e);
         // dW2 += q2^T h1: M = j (2 tiles), N = i (4 tiles), K = the group's 8 R trajectories (m16n8k16 for R = 2, m16n8k8 for
-        // R = 1), 2-way split on the words of the two products above, each 8 x 8 block transposed by one movmatrix
+        // R = 1), 2-way split on the words of the two products, each 8 x 8 block transposed by one movmatrix
         uint32_t ah[2][2 * R], al[2][2 * R];   // A fragments of q2^T: (mt, 2 r + (nt & 1)) <- block (r, nt) of q2, nt >> 1 = mt
 #pragma unroll
         for (int r = 0; r < R; ++r) {
@@ -587,7 +657,7 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
         for (int nt = 0; nt < 4; ++nt) {
             uint32_t bh[R], bl[R];   // B fragment of h1: k-step half r <- block (r, nt) of h1
 #pragma unroll
-            for (int r = 0; r < R; ++r) { bh[r] = movm_t(h1hi[r][nt]); bl[r] = movm_t(h1lo[r][nt]); }
+            for (int r = 0; r < R; ++r) { bh[r] = movm_t(c.h1hi[r][nt]); bl[r] = movm_t(c.h1lo[r][nt]); }
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
                 if constexpr (R == 2) {
@@ -601,47 +671,51 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
                 }
             }
         }
-        // q1 = (W2^T q2) (1 - h1^2); (df/du)^T g; dW1 += q1 (x) x, db1 += q1
-        float y[R][2];
+    };
+    // the tensor core adds into its accumulator with truncation: keep the chains at most one step long and add them into the
+    // running sums with round-to-nearest, undoing the step's scale 2^(127 - e_acc) (exact: a power of two)
+    auto flush = [&]() {
+        const float us_acc = exp2_biased(e_acc);
 #pragma unroll
-        for (int r = 0; r < R; ++r) {
-            float2 s0 = bc(0.0f), s1 = bc(0.0f);
-            const float2 x0 = bc(x[0][r][0]), x1 = bc(x[0][r][1]);
+        for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt) {
-                const float2 hh = h1[0][r][nt];
-                const float2 om = mul2(fma2(make_float2(-hh.x, -hh.y), hh, bc(1.0f)), unscale[r]);
-                const float2 q1 = mul2(make_float2(e[nt][2 * r], e[nt][2 * r + 1]), om);
-                s0 = fma2(lds2(wt.w1a + 8 * nt + 2 * L.tig), q1, s0);
-                s1 = fma2(lds2(wt.w1b + 8 * nt + 2 * L.tig), q1, s1);
-                gB1[nt] = add2(gB1[nt], q1);
-                gW1a[nt] = fma2(q1, x0, gW1a[nt]);
-                gW1b[nt] = fma2(q1, x1, gW1b[nt]);
-            }
-            y[r][0] = s0.x + s0.y;
-            y[r][1] = s1.x + s1.y;
-        }
-        const float dxo = scatter_sum<R>(L, y);
-        return fmaf(pc, go, dxo * isc);   // LV physics: diag(p1, -p4)
+            for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+                for (int c4 = 0; c4 < 4; ++c4) {
+                    float &slot = T.sum[((mt * 4 + nt) * 4 + c4) * 32 + lane];
+                    slot = fmaf(macc[mt][nt][c4], us_acc, slot);
+                    macc[mt][nt][c4] = 0.0f;
+                }
     };
 
     jump(n_save - 1);
     // stage derivatives k_1..k_7 and the start state of the forward step being traversed: read once per step (the next
     // step's rows are requested while the last stage of the current one is evaluated), u(t) of every stage from registers
-    float kd[7], us;
+    float kd[7], us, kl[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) kl[j] = 0.0f;
     auto load_step = [&](int s) {
 #pragma unroll
         for (int j = 0; j < 7; ++j) kd[j] = __ldg(p.dense + (size_t)(s * 6 + j) * 2 * N + idx);
         us = __ldg(p.ustep + (size_t)s * 2 * N + idx);
     };
     load_step(p.n_steps - 1);
+    // lambda_s from the step's stage derivatives, then the data jump at a save point
+    auto step_end = [&](int s) {
+        float a = 0.0f;
+#pragma unroll
+        for (int j = 0; j < 6; ++j) a = fmaf((float)Tsit5::b(j), kl[j], a);
+        lam = fmaf(dt, a, lam);
+        if (s % p.save_every == 0) jump(s / p.save_every);
+    };
+    // backward stage i of step s evaluates at t_{s+1} - c_i dt.  Stage 5 (c = 1) of step s and stage 0 (c = 0) of step s - 1
+    // share the state u(t_s) = ustep[s]: the interpolant's weights are zero at theta = 0, and at theta = 1 they are the
+    // forward's b_j in fp32, so the same fma chain rebuilds ustep[s] bit for bit.  Both are evaluated at the end of step s.
 #pragma unroll 1
     for (int s = p.n_steps - 1; s >= 0; --s) {
-        float kl[6];
-#pragma unroll
-        for (int j = 0; j < 6; ++j) kl[j] = 0.0f;
+        // stage 0 of the last step and stage 5 of step 0 run alone; every other stage 0 runs with stage 5 of the step above
 #pragma unroll 1
-        for (int stage = 0; stage < 6; ++stage) {
+        for (int stage = s == p.n_steps - 1 ? 0 : 1; stage < (s == 0 ? 6 : 5); ++stage) {
             float xa = 0.0f, ga = 0.0f;
 #pragma unroll
             for (int j = 0; j < 7; ++j) xa = fmaf(c_bw[stage][j], kd[j], xa);
@@ -649,31 +723,72 @@ __global__ void __launch_bounds__(32 * WPC, MINB) adjoint_kernel(AdjParams p, Co
             for (int j = 0; j < 5; ++j) ga = fmaf(c_a[stage][j], kl[j], ga);
             const float xo = fmaf(dt, xa, us);      // u(t_{s+1} - c_i dt), own component (Tsit5 free interpolant)
             const float go = fmaf(dt, ga, lam);     // lambda argument of backward stage i
-            if (stage == 5 && s > 0) load_step(s - 1);
-            const float bi = c_a[6][stage];
-            const float kn = eval(xo, go, dt * bi, inv_dt * c_binv[stage], stage == 0);
+            const float sgo = lv * (dt * c_a[6][stage]) * go;
+            ChainRows<R> c;
+            chain(xo, c);
+            float sg[R][2];
+            gather4<R>(L, sgo, sg);
+            gb3 += sgo;
+            uint32_t eb[R];
+            row_exp(sg, eb);
+            float2 q2[R][4];
+            q2_rows(c, sg, q2);
+            uint32_t q2hi[R][4], q2lo[R][4];
+            split_q2(q2, eb, q2hi, q2lo);
+            acc_w3(c, sg);   // before the VJP: h2 and the h1 words end here
+            acc_w2(c, eb, q2hi, q2lo, stage == 0);
+            const float kn = vjp(c, eb, q2hi, q2lo, go, inv_dt * c_binv[stage]);
 #pragma unroll
             for (int j = 0; j < 6; ++j) kl[j] = (stage == j) ? kn : kl[j];
         }
-        float a = 0.0f;
+        if (s == 0) {
+            step_end(0);
+            break;
+        }
+        // stage 5 of step s and stage 0 of step s - 1 at u(t_s): the chain forward once, each stage's VJP and its dW2 product
+        // (on the words of its own q2, so that the sums are those of separate stages), dW3 once on the summed rows
+        flush();   // stages 0..4 of the step: the accumulators hold no registers through the chain forward
+        ChainRows<R> c;
+        chain(us, c);
+        float ga = 0.0f;
 #pragma unroll
-        for (int j = 0; j < 6; ++j) a = fmaf((float)Tsit5::b(j), kl[j], a);
-        lam = fmaf(dt, a, lam);
-        if (s % p.save_every == 0) jump(s / p.save_every);
-        // the tensor core adds into its accumulator with truncation: keep the chains one step long and add them into
-        // the running sums with round-to-nearest, undoing the step's scale 2^(127 - e_acc) (exact: a power of two)
-        const float us_acc = exp2_biased(e_acc);
+        for (int j = 0; j < 5; ++j) ga = fmaf(c_a[5][j], kl[j], ga);
+        const float go = fmaf(dt, ga, lam);
+        const float sgo = lv * (dt * c_a[6][5]) * go;
+        float sg[R][2];
+        gather4<R>(L, sgo, sg);
+        gb3 += sgo;
+        uint32_t eb[R];
+        row_exp(sg, eb);
+        float2 q2[R][4];
+        q2_rows(c, sg, q2);
+        uint32_t q2hi[R][4], q2lo[R][4];
+        split_q2(q2, eb, q2hi, q2lo);
+        acc_w2(c, eb, q2hi, q2lo, false);   // at the step's scale e_acc
+        flush();   // ... and stage 5, before the two VJPs
+        kl[5] = vjp(c, eb, q2hi, q2lo, go, inv_dt * c_binv[5]);
+        step_end(s);
+        // stage 0 of step s - 1: its lambda argument is lambda_s
+        const float sgo0 = lv * (dt * c_a[6][0]) * lam;
+        float sg0[R][2];
+        gather4<R>(L, sgo0, sg0);
+        gb3 += sgo0;
+        row_exp(sg0, eb);
+        q2_rows(c, sg0, q2);
+        split_q2(q2, eb, q2hi, q2lo);
+        const float k0 = vjp(c, eb, q2hi, q2lo, lam, inv_dt * c_binv[0]);
+        load_step(s - 1);
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
+        for (int j = 0; j < 6; ++j) kl[j] = j == 0 ? k0 : 0.0f;
 #pragma unroll
-            for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    float &slot = T.sum[((mt * 4 + nt) * 4 + c) * 32 + lane];
-                    slot = fmaf(macc[mt][nt][c], us_acc, slot);
-                    macc[mt][nt][c] = 0.0f;
-                }
+        for (int r = 0; r < R; ++r) {
+            sg[r][0] += sg0[r][0];
+            sg[r][1] += sg0[r][1];
+        }
+        acc_w3(c, sg);
+        acc_w2(c, eb, q2hi, q2lo, true);
     }
+    flush();
     if (p.grad_u0 && live) p.grad_u0[idx] = lam;
     loss *= lv;
 #pragma unroll
