@@ -1,7 +1,9 @@
 """Time one training iteration of the operator UDE (npde.jl's 30-8-30 tanh closure): forward, fused-L2 adjoint and reduce.
 
-Adaptive Tsit5 at (1e-6, 1e-3), fixed-step RKC2 at the save spacing with the stage count from eigen_est = rho(D2), and
-adaptive RKC2 at (1e-6, 1e-3) with the stage count of each step from eigen_est, fp32 and fp64, for N = 1 (the script's case) and
+Fixed-step Tsit5 at a quarter of the save spacing (h rho(D2) = 2.5 for npde's rho = 191.7, inside Tsit5's real stability
+interval of about 3.5), adaptive Tsit5 at
+(1e-6, 1e-3), fixed-step RKC2 at the save spacing with the stage count from eigen_est = rho(D2), and adaptive RKC2 at
+(1e-6, 1e-3) with the stage count of each step from eigen_est, fp32 and fp64, for N = 1 (the script's case) and
 ensembles of initial bumps; then the forward of the t = 10 solve (npde.jl:120-123: adaptive, (1e-4, 1e-2), save grid 10/194),
 adaptive RKC2 against adaptive Tsit5.  CUDA events; the configurations alternate
 round by round, and the median and the spread over rounds are printed with the GPU's name and power limit.
@@ -43,11 +45,13 @@ def main():
     n10 = int(np.ceil(10.0 / saveat[1]))
 
     def make(N, dt, solver, t10=False):
-        kw = {"tsit5_adaptive": dict(adaptive=True), "rkc2": dict(alg=ude.RKC2(stages=stages)),
+        kw = {"tsit5": {}, "tsit5_adaptive": dict(adaptive=True), "rkc2": dict(alg=ude.RKC2(stages=stages)),
               "rkc2_adaptive": dict(alg=ude.RKC2(eigen_est=191.7), adaptive=True)}[solver]
         if t10:   # npde.jl:120-123: the forward of the t = 10 solve at (1e-4, 1e-2) on the save grid 10/194
             s = ude.UDESolver(f, 0.0, 10.0 / n10, n10, 1, max_trajectories=1, device="cuda:0", dtype=dt, abstol=1e-4, reltol=1e-2,
                               max_steps=2000, **kw)
+        elif solver == "tsit5":
+            s = ude.UDESolver(f, 0.0, saveat[1] / 4, 29 * 4, 4, max_trajectories=N, device="cuda:0", dtype=dt)
         else:
             s = ude.UDESolver(f, 0.0, saveat[1], 29, 1, max_trajectories=N, device="cuda:0", dtype=dt, abstol=1e-6, reltol=1e-3,
                               max_steps=400, **kw)
@@ -61,10 +65,10 @@ def main():
         if c["data"] is not None:
             c["s"].adjoint_l2(c["data"])
 
-    # one group per ensemble size and dtype (at N = 65 536 the records of all six do not fit the device at once); the
+    # one group per ensemble size and dtype (at N = 65 536 the records of all eight do not fit the device at once); the
     # configurations of a group alternate round by round
     dts = (torch.float32, torch.float64)
-    groups = [[(N, dt, sv, False) for sv in ("tsit5_adaptive", "rkc2", "rkc2_adaptive")] for N in [int(x) for x in a.sizes.split(",")] for dt in dts]
+    groups = [[(N, dt, sv, False) for sv in ("tsit5", "tsit5_adaptive", "rkc2", "rkc2_adaptive")] for N in [int(x) for x in a.sizes.split(",")] for dt in dts]
     groups.append([(1, dt, sv, True) for dt in dts for sv in ("tsit5_adaptive", "rkc2_adaptive")])
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     print(f"# GPU: {q}; fixed-step RKC2 stages = {stages}; ms per iteration (forward + fused-L2 adjoint + reduce; *_t10_forward: "

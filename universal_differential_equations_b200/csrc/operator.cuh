@@ -81,6 +81,13 @@ struct V {
     R a, b;   // components lane, lane + 32
 };
 
+// x + y on both slots
+template <typename R>
+__device__ __forceinline__ V<R> add2(V<R> x, V<R> y)
+{
+    return {x.a + y.a, x.b + y.b};
+}
+
 template <typename R>
 __device__ __forceinline__ R act(int k, R z);
 template <>
@@ -178,9 +185,7 @@ __device__ __forceinline__ V<R> rhs(const Run<R> &p, const R *sops, const R *sth
     const V<R> y = chain<R, false>(p, sth, u, nullptr, nullptr, lane);
     V<R> f = matvec(sops + LW, p.ld1, p.D, p.M, y, lane);
     if (p.has_d2) {
-        const V<R> e = matvec(sops + LW + p.ld1 * p.M, p.ld2, p.D, p.D, u, lane);
-        f.a += e.a;
-        f.b += e.b;
+        f = add2(f, matvec(sops + LW + p.ld1 * p.M, p.ld2, p.D, p.D, u, lane));
     }
     return f;
 }
@@ -212,9 +217,7 @@ __device__ __forceinline__ V<R> rhs_vjp(const Run<R> &p, const R *sops, const R 
         }
     }
     if (p.has_d2) {
-        const V<R> e = matvec_t(sops + LW + p.ld1 * p.M, p.ld2, p.D, p.D, g, lane);
-        v.a += e.a;
-        v.b += e.b;
+        v = add2(v, matvec_t(sops + LW + p.ld1 * p.M, p.ld2, p.D, p.D, g, lane));
     }
     return v;
 }
@@ -294,9 +297,16 @@ __device__ __forceinline__ void save_jump(const Run<R> &p, const R *sops, int is
         lam.a = fma((R)2 * wa, ra, lam.a);
         lam.b = fma((R)2 * wb, rb, lam.b);
     } else {
-        lam.a += c.a;
-        lam.b += c.b;
+        lam = add2(lam, c);
     }
+}
+
+// the cubic Hermite interpolant on (a0, g0, a1, g1) over a step of length h at fraction Th (OrdinaryDiffEq's dense output of
+// the ROCK methods)
+template <typename R>
+__device__ __forceinline__ R herm3(R Th, R h, R a0, R a1, R g0, R g1)
+{
+    return ((R)1 - Th) * a0 + Th * a1 + Th * (Th - (R)1) * (((R)1 - (R)2 * Th) * (a1 - a0) + (Th - (R)1) * h * g0 + Th * h * g1);
 }
 
 // ---- 1. fixed-step Tsit5 forward, with the dense record ----
@@ -617,11 +627,7 @@ __global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
             V<R> D0{(R)0, (R)0}, D1{(R)0, (R)0}, F0{(R)0, (R)0};   // increments Y_j - lambda (kernel 5)
             for (int j = 0; j < p.S; ++j) {
                 const R Th = (R)1 - __ldg(p.rkc + RKC_C + j);
-                // x = (1 - Th) y0 + Th y1 + Th (Th - 1) ((1 - 2 Th) (y1 - y0) + (Th - 1) dt f0 + Th dt f1)
-                auto herm = [&](R a0, R a1, R g0, R g1) {
-                    return ((R)1 - Th) * a0 + Th * a1 + Th * (Th - (R)1) * (((R)1 - (R)2 * Th) * (a1 - a0) + (Th - (R)1) * dt * g0 + Th * dt * g1);
-                };
-                const V<R> x{herm(y0.a, y1.a, f0.a, f1.a), herm(y0.b, y1.b, f0.b, f1.b)};
+                const V<R> x{herm3(Th, dt, y0.a, y1.a, f0.a, f1.a), herm3(Th, dt, y0.b, y1.b, f0.b, f1.b)};
                 const V<R> F = rhs_vjp(p, sm.ops, sm.th, x, V<R>{lam.a + D1.a, lam.b + D1.b}, dt * __ldg(p.rkc + RKC_W + j), gw, lane);
                 if (j == 0) {
                     F0 = F;
@@ -646,14 +652,6 @@ __global__ void __launch_bounds__(128) rkc2_adjoint_kernel(Run<R> p)
 }
 
 // The adaptive RKC2 kernels below repeat the stage recurrence of kernels 5 / 6 instead of calling shared helpers.
-
-// the cubic Hermite interpolant on (a0, g0, a1, g1) over a step of length h at fraction Th (OrdinaryDiffEq's dense output of
-// the ROCK methods; kernel 6 writes the same expression inline)
-template <typename R>
-__device__ __forceinline__ R herm3(R Th, R h, R a0, R a1, R g0, R g1)
-{
-    return ((R)1 - Th) * a0 + Th * a1 + Th * (Th - (R)1) * (((R)1 - (R)2 * Th) * (a1 - a0) + (Th - (R)1) * h * g0 + Th * h * g1);
-}
 
 // ---- 7. adaptive RKC2 forward (ROCK2(eigen_est = rho) without dt, npde.jl:80-84,120-123).  Per attempt the fewest stages
 // s in 2..S with beta(s) >= 1.05 h rho (none: s = S and h = beta(S) / (1.05 rho)), the s-stage recurrence of kernel 5, the
